@@ -544,10 +544,11 @@ __device__ __forceinline__ bool mag_ok(float x)
 }
 
 // The "plain" step (see fold_chunk for the argument): Kalman update or clear gate decision for ordinary magnitudes.
-// Returns false when the step must be decided by the literal code instead (near the gate, numerator out of the
-// guarded range); e / var then hold garbage and the caller redoes the list literally.
+// Returns false when the step must be decided by the literal code instead (the cell is empty, near the gate,
+// numerator out of the guarded range); e / var then hold garbage and the caller redoes the list literally.
 __device__ __forceinline__ bool plain_step(float &e, float &var, float h, float v, bool &take)
 {
+    const bool empty = e == -10.0f; // gpu.cu:484 on EVERY step: an earlier step of the list may have returned to -10
     const float ov = (var <= 1e-4f) ? 1e-4f : var;
     const float den = ov + v;
     float rc;
@@ -562,7 +563,7 @@ __device__ __forceinline__ bool plain_step(float &e, float &var, float h, float 
     const float d = fabsf(h - e), dd = d * d;
     const bool lo = dd < ov * 24.9995f, hi = dd > ov * 25.0005f, higher = e < h;
     const uint32_t u0 = __float_as_uint(n0) & 0x7fffffffu;
-    const bool ok = (lo | hi) & (!lo | ((u0 - 0x1e800000u) < (0x60800000u - 0x1e800000u)) | (u0 == 0u));
+    const bool ok = (lo | hi) & (!lo | ((u0 - 0x1e800000u) < (0x60800000u - 0x1e800000u)) | (u0 == 0u)) & !empty;
     take = lo | higher;
     e = lo ? qe : (higher ? h : e);
     var = lo ? qv : (higher ? v : ov); // an ignored lower point leaves the FLOORED variance behind (gpu.cu:500-501)
@@ -709,7 +710,10 @@ __device__ __forceinline__ void fold_chunk(CellState &s, const uint4 r, int m, b
             const float d = fabsf(h - e), dd = d * d;
             const bool lo = dd < ov * 24.9995f, hi = dd > ov * 25.0005f, higher = e < h;
             const uint32_t u0 = __float_as_uint(n0) & 0x7fffffffu;
-            leave |= !(lo | hi) | (lo & !(((u0 - 0x1e800000u) < (0x60800000u - 0x1e800000u)) | (u0 == 0u)));
+            // a state that is exactly -10 (replaced by, or Kalman-averaged to, -10 earlier in the list) is "empty"
+            // (gpu.cu:484): the general step takes the next record as it is.  Off the serial chain: nothing reads
+            // `leave` before the end of the chunk
+            leave |= !(lo | hi) | (lo & !(((u0 - 0x1e800000u) < (0x60800000u - 0x1e800000u)) | (u0 == 0u))) | (e == -10.0f);
             takes |= ((lo | higher) ? 1u : 0u) << t;
             e = lo ? qe : (higher ? h : e);
             var = lo ? qv : (higher ? v : ov); // an ignored lower point leaves the FLOORED variance behind (gpu.cu:500-501)

@@ -292,10 +292,11 @@ int launch_fold(gem_map *m, cudaStream_t st, const PendingFold &p, const RegionO
 {
     const int fb = fold_blocks_for(m, p.n);
     const int slice = fold_slice(p.n, fb);
-    RegionOps none{};
     // the long lists first (their blocks claim whole SMs), then everything else; on one stream the two run back to back
-    // (disjoint cells, so the order is free) -- the frame graph of the pipelined mode runs them side by side
-    GEM_LAUNCH_ON(m, st, GEM_PROF_FOLD_LONG, k_fold_long<<<long_blocks_for(m, p.n), LONG_BLOCK, m->long_smem, st>>>(p.geom, m->ml, p.sc, p.src, none, do_fuse ? 1 : 0, do_lowest ? 1 : 0));
+    // (disjoint cells, so the order is free) -- the frame graph of the pipelined mode runs them side by side.  Both get
+    // the next call's clears `ro`: a long list inside a cleared band must store the cleared value itself, because
+    // k_fold's region blocks may clear the cell before k_fold_long writes it (cell_end)
+    GEM_LAUNCH_ON(m, st, GEM_PROF_FOLD_LONG, k_fold_long<<<long_blocks_for(m, p.n), LONG_BLOCK, m->long_smem, st>>>(p.geom, m->ml, p.sc, p.src, ro, do_fuse ? 1 : 0, do_lowest ? 1 : 0));
     GEM_LAUNCH_ON(m, st, GEM_PROF_FOLD, k_fold<<<fb + region_blocks, ADD_BLOCK, m->fold_smem, st>>>(p.geom, m->ml, p.sc, p.src, ro, p.n, fb, slice, do_fuse ? 1 : 0, do_lowest ? 1 : 0, p.n_dev));
     GEM_CUDA(m, cudaGetLastError());
     return GEM_OK;
@@ -624,7 +625,7 @@ int enqueue_add(gem_map *m, const BinSource &in, const FoldSrc &fsrc, int n, con
             int pbk = pb, one = 1, fbk = fb;
             void *bin_args[] = {&g, &ml, &f, &bin, &nn, &sc, &none, &pbk, &st, (void *)&frames};
             void *fold_args[] = {&prev.geom, &ml, &prev.sc, &prev.src, &ro, &prev.n, &fbk, &slice, &one, &one, (void *)&prev.n_dev};
-            void *long_args[] = {&prev.geom, &ml, &prev.sc, &prev.src, &none, &one, &one};
+            void *long_args[] = {&prev.geom, &ml, &prev.sc, &prev.src, &ro, &one, &one}; // the clears, like k_fold (launch_fold)
             if ((rc = launch_frame_graph(m, bk, bin_args, pb, fold_args, fb + rb, long_args, long_blocks_for(m, prev.n)))) return rc;
         } else {
             GEM_CUDA(m, cudaStreamWaitEvent(m->front_stream, m->ev_fold[par], 0)); // the fold that last used this parity's scratch
