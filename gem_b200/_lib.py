@@ -14,6 +14,8 @@ ERR_NAMES = {0: "GEM_OK", 1: "GEM_ERR_INVALID", 2: "GEM_ERR_CUDA", 3: "GEM_ERR_N
 SENSOR_LASER = 0
 SENSOR_STRUCTURED_LIGHT = 1
 
+GRID_SOURCES = {"shown": 0, "snapshot": 1}   # GEM_GRID_SHOWN / GEM_GRID_SNAPSHOT
+
 LAYERS = {"elevation": 0, "variance": 1, "intensity": 2, "color_r": 3, "color_g": 4, "color_b": 5,
           "traver": 6, "lowest": 7, "rough": 8, "slope": 9}
 INT_LAYERS = {3, 4, 5}
@@ -112,6 +114,11 @@ SYMBOLS = {
     "gem_export_visual_points": (C.c_int, [_P, _P, _P, C.c_int, C.POINTER(C.c_int)]),
     "gem_snapshot_shown": (C.c_int, [_P]),
     "gem_harvest_scrolled_out": (C.c_int, [_P, C.POINTER(C.c_float), C.POINTER(C.c_float), _P, C.c_int, C.POINTER(C.c_int)]),
+    "gem_export_grid_cloud": (C.c_int, [_P, C.c_int, _P, C.c_int, C.POINTER(C.c_int)]),
+    "gem_harvest_to_local_map": (C.c_int, [_P, C.POINTER(C.c_float), C.POINTER(C.c_float), _P, C.c_int, C.POINTER(C.c_int)]),
+    "gem_local_map_take": (C.c_int, [_P, _P, C.c_int, C.POINTER(C.c_int)]),
+    "gem_local_map_clear": (C.c_int, [_P]),
+    "gem_local_map_reserve": (C.c_int, [_P, C.c_int]),
     "gem_get_layer_device": (C.c_int, [_P, C.c_int, _P]),
     "gem_compute_features_tiled": (C.c_int, [_P, _P]),
     "gem_raytracing_tiled": (C.c_int, [_P, _P]),

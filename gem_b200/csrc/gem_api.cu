@@ -58,6 +58,16 @@ struct TiledState { // gem_tiled_attach
     cudaGraphNode_t long_node = nullptr, fold_node = nullptr, route_node = nullptr, bin_node = nullptr;
 };
 
+struct LocalStore { // localMap_ on the device (gem_harvest_to_local_map, gem_local_map_take / _clear; gem_submap.cuh)
+    void *buf = nullptr;               // one allocation: log, index keys, index positions, take scratch
+    float4 *log = nullptr;             // 2 x float4 per record, in harvest order
+    unsigned long long *keys = nullptr; // open-addressing index, HASH_EMPTY = free slot
+    int *latest = nullptr;             // per slot: the latest log position of its key
+    int *cnt = nullptr;                // take: kept entries per 32 log entries, then the scan's segment totals
+    int n = 0, cap = 0;                // records in the log, records it can hold
+    size_t slots = 0;                  // index slots (a power of two >= 2 * cap)
+};
+
 struct FrameGraph { // {long lists || the other lists of the previous call || bin of this call} as one three-node CUDA graph
     cudaGraph_t graph = nullptr;
     cudaGraphExec_t exec = nullptr;
@@ -108,6 +118,7 @@ struct gem_map {
     float *prev_tr = nullptr;
     MapGeom prev_geom{};
     bool prev_valid = false;
+    LocalStore local;
     int *d_viscnt = nullptr;       // visual-cloud export: per (column, row chunk) counts / offsets
     unsigned long long *d_stamps = nullptr; // gem_debug_stamps
     int *d_raylist = nullptr;      // ray clean-up: cells that cast a ray + their count
@@ -817,6 +828,7 @@ int gem_destroy(gem_map *m)
         for (auto &sp : m->spans) { cudaEventDestroy(sp.e0); cudaEventDestroy(sp.e1); }
         for (cudaEvent_t e : m->free_events) cudaEventDestroy(e);
         for (void *p : m->allocs) cudaFree(p);
+        if (m->local.buf) cudaFree(m->local.buf);
         if (m->h_ctr) cudaFreeHost(m->h_ctr);
         if (m->h_ctr_ring) cudaFreeHost(m->h_ctr_ring);
         if (m->h_frames) cudaFreeHost(m->h_frames);
@@ -1509,6 +1521,23 @@ int gem_snapshot_shown(gem_map *m)
     return GEM_OK;
 }
 
+// the harvest of :716-765 into the read-out staging buffer (the first `cap` records); the caller holds the lock
+static int harvest_to_staging(gem_map *m, const float current_xy[2], const float shift_xy[2], int cap, int *total)
+{
+    int rc = ensure_out_staging(m);
+    if (rc) return rc;
+    HarvestSrc src;
+    src.s = snapshot_cells(m->prev_ev, m->prev_ci, m->prev_tr);
+    src.f = grid_frame(m, m->prev_geom.cx, m->prev_geom.cy, m->prev_geom.sx, m->prev_geom.sy);
+    // :727-734: current_x (float) -+ length_ * resolution_ / 2 with the node's double resolution_
+    const double halfwin = (double)m->L * src.f.res / 2;
+    src.lox = (double)current_xy[0] - halfwin; src.hix = (double)current_xy[0] + halfwin;
+    src.loy = (double)current_xy[1] - halfwin; src.hiy = (double)current_xy[1] + halfwin;
+    src.dx = shift_xy[0]; src.dy = shift_xy[1];
+    src.out = reinterpret_cast<float4 *>(m->d_out); // 8 of the 9 staging floats per cell
+    return compact_cells(m, src, cap, total);
+}
+
 int gem_harvest_scrolled_out(gem_map *m, const float current_xy[2], const float shift_xy[2], void *host_points32,
                              int capacity, int *count_out)
 {
@@ -1517,27 +1546,168 @@ int gem_harvest_scrolled_out(gem_map *m, const float current_xy[2], const float 
     if (!m->prev_valid) return fail(m, GEM_ERR_INVALID, "gem_harvest_scrolled_out: no snapshot (call gem_snapshot_shown first)");
     Lock lk(m->mu);
     SetDev sd(m->dev);
-    int rc = ensure_out_staging(m);
-    if (rc) return rc;
-    HarvestSrc src;
-    src.pev = m->prev_ev; src.pci = m->prev_ci; src.ptr = m->prev_tr;
-    src.f = grid_frame(m, m->prev_geom.cx, m->prev_geom.cy, m->prev_geom.sx, m->prev_geom.sy);
-    // :727-734: current_x (float) -+ length_ * resolution_ / 2 with the node's double resolution_
-    const double halfwin = (double)m->L * src.f.res / 2;
-    src.lox = (double)current_xy[0] - halfwin; src.hix = (double)current_xy[0] + halfwin;
-    src.loy = (double)current_xy[1] - halfwin; src.hiy = (double)current_xy[1] + halfwin;
-    src.dx = shift_xy[0]; src.dy = shift_xy[1];
-    src.out = reinterpret_cast<float4 *>(m->d_out); // 8 of the 9 staging floats per cell
     const int cap = (int)std::min<size_t>((size_t)capacity, m->nc);
-    int total = 0;
-    if ((rc = compact_cells(m, src, cap, &total))) return rc;
+    int total = 0, rc;
+    if ((rc = harvest_to_staging(m, current_xy, shift_xy, cap, &total))) return rc;
     *count_out = total;
     const size_t n = (size_t)std::min(total, cap);
     if (n) {
-        GEM_CUDA(m, cudaMemcpyAsync(host_points32, src.out, n * 32, cudaMemcpyDeviceToHost, m->stream));
+        GEM_CUDA(m, cudaMemcpyAsync(host_points32, m->d_out, n * 32, cudaMemcpyDeviceToHost, m->stream));
         GEM_CUDA(m, cudaStreamSynchronize(m->stream));
     }
     return GEM_OK;
+}
+
+int gem_export_grid_cloud(gem_map *m, int source, void *points32_device, int capacity, int *count_out)
+{
+    if (!m || !count_out || capacity < 0 || (capacity > 0 && !points32_device) || (source != GEM_GRID_SHOWN && source != GEM_GRID_SNAPSHOT))
+        return fail(m, GEM_ERR_INVALID, "gem_export_grid_cloud: bad argument");
+    if (m->geom.tiled) return fail(m, GEM_ERR_INVALID, "gem_export_grid_cloud: not available on tiled handles");
+    Lock lk(m->mu);
+    SetDev sd(m->dev);
+    if (source == GEM_GRID_SNAPSHOT && !m->prev_valid)
+        return fail(m, GEM_ERR_INVALID, "gem_export_grid_cloud: no snapshot (call gem_snapshot_shown first)");
+    int rc = flush_for_observer(m);
+    if (rc) return rc;
+    GridCloudSrc src;
+    const MapGeom &g = source == GEM_GRID_SHOWN ? m->geom : m->prev_geom;
+    src.s = source == GEM_GRID_SHOWN ? live_cells(m->ml) : snapshot_cells(m->prev_ev, m->prev_ci, m->prev_tr);
+    src.f = grid_frame(m, g.cx, g.cy, g.sx, g.sy);
+    src.out = reinterpret_cast<float4 *>(points32_device);
+    int total = 0;
+    if ((rc = compact_cells(m, src, (int)std::min<size_t>((size_t)capacity, m->nc), &total))) return rc;
+    *count_out = total; // the number of cells taken; min(total, capacity) records are written
+    return GEM_OK;
+}
+
+// ---- localMap_ on the device ----------------------------------------------------------------------------------------
+// Grow the store to hold `need` records (capacity doubles from LOCAL_MIN_RECORDS).  Everything is allocated before
+// anything is released, so a failed growth leaves the store as it was.
+static constexpr int LOCAL_MIN_RECORDS = 1024;
+static int local_reserve(gem_map *m, long long need)
+{
+    LocalStore &s = m->local;
+    if (need <= s.cap) return GEM_OK;
+    long long cap = s.cap > 0 ? s.cap : LOCAL_MIN_RECORDS;
+    while (cap < need) cap *= 2;
+    if (cap > (1 << 30)) return fail(m, GEM_ERR_NOMEM, "local map: more than 2^30 records");
+    size_t slots = 64;
+    while (slots < 2 * (size_t)cap) slots <<= 1;
+    const size_t nchunk = (size_t)cap / 32 + 1, nseg = nchunk / SCAN_SEG + 1;
+    const size_t bytes = (size_t)cap * 32 + slots * (8 + 4) + (nchunk + nseg) * 4;
+    void *buf = nullptr;
+    cudaError_t e = cudaMalloc(&buf, bytes);
+    if (e != cudaSuccess) {
+        cudaGetLastError();
+        return fail(m, GEM_ERR_NOMEM, std::string("local map: cudaMalloc: ") + cudaGetErrorString(e));
+    }
+    LocalStore t;
+    t.buf = buf;
+    t.log = (float4 *)buf;
+    t.keys = (unsigned long long *)(t.log + 2 * (size_t)cap);
+    t.latest = (int *)(t.keys + slots);
+    t.cnt = t.latest + slots;
+    t.n = s.n; t.cap = (int)cap; t.slots = slots;
+    e = cudaMemsetAsync(t.keys, 0xff, slots * 8, m->stream);
+    if (e == cudaSuccess) e = cudaMemsetAsync(t.latest, 0xff, slots * 4, m->stream);
+    if (e == cudaSuccess && s.n) e = cudaMemcpyAsync(t.log, s.log, (size_t)s.n * 32, cudaMemcpyDeviceToDevice, m->stream);
+    if (e == cudaSuccess && s.n) {
+        GEM_LAUNCH(m, GEM_PROF_OTHER, k_local_index<<<blocks_for((size_t)s.n, 256, 1 << 30), 256, 0, m->stream>>>(t.log, 0, s.n, t.keys, t.latest, (unsigned)(slots - 1)));
+        e = cudaGetLastError();
+    }
+    if (e == cudaSuccess) e = cudaStreamSynchronize(m->stream);
+    if (e != cudaSuccess) {
+        cudaFree(buf);
+        return fail(m, GEM_ERR_CUDA, std::string("local map: growth: ") + cudaGetErrorString(e));
+    }
+    if (s.buf) cudaFree(s.buf);
+    s = t;
+    return GEM_OK;
+}
+
+// forget every record: the index back to all-free slots
+static int local_reset(gem_map *m)
+{
+    LocalStore &s = m->local;
+    s.n = 0;
+    if (!s.buf) return GEM_OK;
+    GEM_CUDA(m, cudaMemsetAsync(s.keys, 0xff, s.slots * 8, m->stream));
+    GEM_CUDA(m, cudaMemsetAsync(s.latest, 0xff, s.slots * 4, m->stream));
+    GEM_CUDA(m, cudaStreamSynchronize(m->stream));
+    return GEM_OK;
+}
+
+int gem_local_map_reserve(gem_map *m, int records)
+{
+    if (!m || records < 0) return fail(m, GEM_ERR_INVALID, "gem_local_map_reserve: bad argument");
+    if (m->geom.tiled) return fail(m, GEM_ERR_INVALID, "gem_local_map_reserve: not available on tiled handles");
+    Lock lk(m->mu);
+    SetDev sd(m->dev);
+    return local_reserve(m, records);
+}
+
+int gem_harvest_to_local_map(gem_map *m, const float current_xy[2], const float shift_xy[2], void *host_points32, int capacity,
+                             int *count_out)
+{
+    if (!m || !current_xy || !shift_xy || !count_out || capacity < 0 || (capacity > 0 && !host_points32))
+        return fail(m, GEM_ERR_INVALID, "gem_harvest_to_local_map: bad argument");
+    if (m->geom.tiled) return fail(m, GEM_ERR_INVALID, "gem_harvest_to_local_map: not available on tiled handles");
+    Lock lk(m->mu);
+    SetDev sd(m->dev);
+    if (!m->prev_valid) return fail(m, GEM_ERR_INVALID, "gem_harvest_to_local_map: no snapshot (call gem_snapshot_shown first)");
+    int total = 0, rc;
+    if ((rc = harvest_to_staging(m, current_xy, shift_xy, (int)m->nc, &total))) return rc;
+    if ((rc = local_reserve(m, (long long)m->local.n + total))) return rc;
+    LocalStore &s = m->local;
+    if (total) { // append, then point every key of this call at its latest position (:740-747)
+        GEM_CUDA(m, cudaMemcpyAsync(s.log + 2 * (size_t)s.n, m->d_out, (size_t)total * 32, cudaMemcpyDeviceToDevice, m->stream));
+        GEM_LAUNCH(m, GEM_PROF_OTHER, k_local_index<<<blocks_for((size_t)total, 256, 1 << 30), 256, 0, m->stream>>>(s.log, s.n, s.n + total, s.keys, s.latest, (unsigned)(s.slots - 1)));
+        GEM_CUDA(m, cudaGetLastError());
+        s.n += total;
+    }
+    const size_t n = (size_t)std::min(total, capacity);
+    if (n) GEM_CUDA(m, cudaMemcpyAsync(host_points32, m->d_out, n * 32, cudaMemcpyDeviceToHost, m->stream));
+    GEM_CUDA(m, cudaStreamSynchronize(m->stream));
+    *count_out = total;
+    return GEM_OK;
+}
+
+int gem_local_map_take(gem_map *m, void *points32_device, int capacity, int *count_out)
+{
+    if (!m || !count_out || capacity < 0 || (capacity > 0 && !points32_device))
+        return fail(m, GEM_ERR_INVALID, "gem_local_map_take: bad argument");
+    if (m->geom.tiled) return fail(m, GEM_ERR_INVALID, "gem_local_map_take: not available on tiled handles");
+    Lock lk(m->mu);
+    SetDev sd(m->dev);
+    LocalStore &s = m->local;
+    if (s.n == 0) { *count_out = 0; return GEM_OK; }
+    // the kept entries (those the index points at) in log order: count per warp -> multi-block scan -> write
+    const int nchunk = (s.n + 31) / 32, nseg = (nchunk + SCAN_SEG - 1) / SCAN_SEG, nb = (s.n + TAKE_BLOCK - 1) / TAKE_BLOCK;
+    const unsigned mask = (unsigned)(s.slots - 1);
+    int *segtot = s.cnt + nchunk;
+    GEM_LAUNCH(m, GEM_PROF_OTHER, k_local_count<<<nb, TAKE_BLOCK, 0, m->stream>>>(s.log, s.n, s.keys, s.latest, mask, s.cnt));
+    GEM_LAUNCH(m, GEM_PROF_OTHER, k_compact_scan<<<nseg, SCAN_SEG, 0, m->stream>>>(s.cnt, nchunk, segtot));
+    GEM_CUDA(m, cudaGetLastError());
+    std::vector<int> h((size_t)nseg);
+    GEM_CUDA(m, cudaMemcpyAsync(h.data(), segtot, (size_t)nseg * 4, cudaMemcpyDeviceToHost, m->stream));
+    GEM_CUDA(m, cudaStreamSynchronize(m->stream));
+    long long total = 0;
+    for (int v : h) total += v;
+    *count_out = (int)total;
+    if (total > capacity) return GEM_OK; // nothing written, the store is kept: *count_out is the size needed
+    GEM_LAUNCH(m, GEM_PROF_OTHER, k_local_write<<<nb, TAKE_BLOCK, 0, m->stream>>>(s.log, s.n, s.keys, s.latest, mask, s.cnt, segtot, SCAN_SEG,
+                                                                                 reinterpret_cast<float4 *>(points32_device)));
+    GEM_CUDA(m, cudaGetLastError());
+    return local_reset(m);
+}
+
+int gem_local_map_clear(gem_map *m)
+{
+    if (!m) return GEM_ERR_INVALID;
+    if (m->geom.tiled) return fail(m, GEM_ERR_INVALID, "gem_local_map_clear: not available on tiled handles");
+    Lock lk(m->mu);
+    SetDev sd(m->dev);
+    return local_reset(m);
 }
 
 int gem_get_layer(gem_map *m, int layer, void *host_out)

@@ -125,6 +125,65 @@ k_refuse_pair(SubPoint *pn, int nn, SubPoint *po, int no, double res, const unsi
     pn[i] = a;
 }
 
+// ---- localMap_ on the device (ElevationMapping.cpp:740-747, localHashtoPointCloud :1124-1140) -----------------------
+// The store is an append log of harvested PointXYZRGBICT records (2 x float4 each) plus an open-addressing index from a
+// cell's key to the LATEST log position holding it.  GridPointEqual compares the float (x, y) of a grid_map cell centre;
+// those are finite and never -0, so the key is their bit pattern.  find / erase / insert (:740-747) leaves the last write
+// of a key, and it moves the key to the end of an insertion-ordered iteration: keeping log entry i iff the index points
+// at i, in log order, is that iteration (DESIGN.md "local submap", order DEFINED).
+__device__ __forceinline__ unsigned long long point_key(float x, float y)
+{
+    return ((unsigned long long)__float_as_uint(x) << 32) | (unsigned long long)__float_as_uint(y);
+}
+// index the log entries [from, to); a key's slot keeps the largest position (the later cell of one call, or a later call)
+__global__ void __launch_bounds__(256) k_local_index(const float4 *log, int from, int to, unsigned long long *keys, int *latest, unsigned mask)
+{
+    const int i = from + (int)(blockIdx.x * blockDim.x + threadIdx.x);
+    if (i >= to) return;
+    const float4 p = log[2 * (size_t)i];
+    const unsigned long long k = point_key(p.x, p.y);
+    unsigned s = hash_slot(k, mask);
+    for (;;) {
+        const unsigned long long prev = atomicCAS(&keys[s], HASH_EMPTY, k);
+        if (prev == HASH_EMPTY || prev == k) { atomicMax(&latest[s], i); return; }
+        s = (s + 1) & mask;
+    }
+}
+__device__ __forceinline__ bool local_kept(const float4 *log, int i, int n, const unsigned long long *keys, const int *latest, unsigned mask)
+{
+    if (i >= n) return false;
+    const float4 p = log[2 * (size_t)i];
+    return hash_find(keys, latest, mask, point_key(p.x, p.y)) == i;
+}
+// take, pass 1: kept entries per 32 log entries (one warp each); the counts are then scanned by k_compact_scan
+constexpr int TAKE_BLOCK = 1024;
+__global__ void __launch_bounds__(TAKE_BLOCK) k_local_count(const float4 *log, int n, const unsigned long long *keys, const int *latest,
+                                                            unsigned mask, int *cnt)
+{
+    const int i = blockIdx.x * TAKE_BLOCK + threadIdx.x;
+    const unsigned b = __ballot_sync(0xffffffffu, local_kept(log, i, n, keys, latest, mask));
+    if ((threadIdx.x & 31u) == 0u && i < n) cnt[i >> 5] = __popc(b);
+}
+// take, pass 2: entry i goes to (totals of the scan segments in front) + (scanned count of its warp) + (rank in the warp)
+__global__ void __launch_bounds__(TAKE_BLOCK) k_local_write(const float4 *log, int n, const unsigned long long *keys, const int *latest,
+                                                            unsigned mask, const int *ofs, const int *segtot, int seg_size, float4 *out)
+{
+    const int i = blockIdx.x * TAKE_BLOCK + threadIdx.x;
+    const unsigned lane = threadIdx.x & 31u;
+    const bool keep = local_kept(log, i, n, keys, latest, mask);
+    const unsigned b = __ballot_sync(0xffffffffu, keep);
+    const int chunk = i >> 5, seg = chunk / seg_size;
+    int pre = 0;
+    for (int q = (int)lane; q < seg; q += 32) pre += segtot[q];
+#pragma unroll
+    for (int d = 16; d > 0; d >>= 1) pre += __shfl_xor_sync(0xffffffffu, pre, d);
+    if (keep) {
+        const size_t pos = (size_t)pre + ofs[chunk] + __popc(b & ((1u << lane) - 1u));
+        out[2 * pos + 0] = log[2 * (size_t)i + 0];
+        out[2 * pos + 1] = log[2 * (size_t)i + 1];
+    }
+}
+
 // order-preserving compaction of the kept points (one block; a loop-closure event is rare and a submap has < 1e6 points)
 __global__ void __launch_bounds__(1024) k_compact_points(const SubPoint *in, const unsigned char *keep, int n, SubPoint *out, int *n_out)
 {

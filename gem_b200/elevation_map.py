@@ -131,6 +131,7 @@ class ElevationMap:
             raise _lib.GemError(f"gem_create: {_lib.ERR_NAMES.get(rc, rc)}: {msg.decode() if msg else ''}")
         self.length = int(length)
         self.resolution = float(resolution)
+        self._cfg_device = int(device)
         self.tile = tile
         self.ncells = (tile[1] * tile[3]) if tile is not None else self.length * self.length
         self.shape = (tile[1], tile[3]) if tile is not None else (self.length, self.length)
@@ -420,6 +421,85 @@ class ElevationMap:
         check(self._lib.gem_harvest_scrolled_out(self._h, cur, sh, _ptr(out), cap, C.byref(cnt)), self._h,
               "gem_harvest_scrolled_out")
         return out[:min(cnt.value, cap)], cnt.value
+
+    # -- local submaps on the device (ElevationMapping.cpp:609-767, :1124-1140, :1198-1226) ----------------------------
+    def _records_out(self, n: int, out, what: str):
+        """an (n, 8) float32 tensor on the map's device for n records: `out`'s first n rows, or a new tensor"""
+        import torch
+        if out is None:
+            dev = torch.device("cuda", self._device_index())
+            torch.cuda.current_stream(dev).synchronize()   # the library writes on its own stream
+            return torch.empty((n, 8), dtype=torch.float32, device=dev)
+        if not (_is_device(out) and out.dtype == torch.float32 and out.dim() == 2 and out.shape[1] == 8 and out.is_contiguous()):
+            raise ValueError(f"{what}: out must be a contiguous (k, 8) float32 CUDA tensor")
+        if out.shape[0] < n:
+            raise ValueError(f"{what}: out holds {out.shape[0]} records, {n} are needed")
+        return out[:n]
+
+    def _device_index(self) -> int:
+        import torch
+        if not hasattr(self, "_dev"):
+            self._dev = self._cfg_device if self._cfg_device >= 0 else torch.cuda.current_device()
+        return self._dev
+
+    def grid_cloud_count(self, source: str = "shown") -> int:
+        """number of cells export_grid_cloud(source) takes"""
+        cnt = C.c_int()
+        check(self._lib.gem_export_grid_cloud(self._h, _lib.GRID_SOURCES[source], None, 0, C.byref(cnt)), self._h,
+              "gem_export_grid_cloud")
+        return cnt.value
+
+    def export_grid_cloud(self, source: str = "shown", out=None):
+        """gridMaptoPointCloud (ElevationMapping.cpp:1198-1226) of the shown map ("shown", visualMap_) or of the snapshot
+        ("snapshot", prevMap_): (n, 8) float32 CUDA tensor of PointXYZRGBICT records in GridMapIterator order"""
+        n = self.grid_cloud_count(source)
+        rec = self._records_out(n, out, "export_grid_cloud")
+        cnt = C.c_int()
+        check(self._lib.gem_export_grid_cloud(self._h, _lib.GRID_SOURCES[source], _ptr(rec), n, C.byref(cnt)), self._h,
+              "gem_export_grid_cloud")
+        return rec
+
+    def harvest_to_local_map(self, current_xy, shift_xy, records: bool = False):
+        """the harvest of harvest_scrolled_out, upserted into the device-resident localMap_ (ElevationMapping.cpp:740-747).
+        Returns the number of harvested records, or (records (n, 8) float32 host array, n) with records=True"""
+        cur = (C.c_float * 2)(*[float(v) for v in current_xy])
+        sh = (C.c_float * 2)(*[float(v) for v in shift_xy])
+        cnt = C.c_int()
+        out = np.empty((self.ncells, 8), np.float32) if records else None
+        check(self._lib.gem_harvest_to_local_map(self._h, cur, sh, _ptr(out), self.ncells if records else 0, C.byref(cnt)),
+              self._h, "gem_harvest_to_local_map")
+        return (out[:cnt.value], cnt.value) if records else cnt.value
+
+    def local_map_size(self) -> int:
+        """records local_map_take would return now (distinct cells harvested since the last take / clear)"""
+        cnt = C.c_int()
+        check(self._lib.gem_local_map_take(self._h, None, 0, C.byref(cnt)), self._h, "gem_local_map_take")
+        return cnt.value
+
+    def local_map_take(self, out=None):
+        """localHashtoPointCloud (ElevationMapping.cpp:1124-1140): the local map as an (n, 8) float32 CUDA tensor (last
+        occurrence of each cell, in the order of those occurrences); the local map is empty afterwards"""
+        n = self.local_map_size()
+        rec = self._records_out(n, out, "local_map_take")
+        cnt = C.c_int()
+        check(self._lib.gem_local_map_take(self._h, _ptr(rec), n, C.byref(cnt)), self._h, "gem_local_map_take")
+        return rec
+
+    def local_map_clear(self):
+        check(self._lib.gem_local_map_clear(self._h), self._h, "gem_local_map_clear")
+
+    def local_map_reserve(self, records: int):
+        """room for `records` harvested records now, so that later harvests do not allocate"""
+        check(self._lib.gem_local_map_reserve(self._h, int(records)), self._h, "gem_local_map_reserve")
+
+    def cut_submap(self, out=None):
+        """the submap of a keyframe cut (ElevationMapping.cpp:653-661): local_map_take() followed by
+        export_grid_cloud("shown"), in one (n, 8) float32 CUDA tensor; the local map is empty afterwards"""
+        nl, ng = self.local_map_size(), self.grid_cloud_count("shown")
+        rec = self._records_out(nl + ng, out, "cut_submap")
+        self.local_map_take(out=rec[:nl])
+        self.export_grid_cloud("shown", out=rec[nl:])
+        return rec
 
     def get_layer_device(self, name: str, out):
         """dense (rows, cols) copy of a layer into a device tensor (float32, int32 for colours)"""

@@ -251,6 +251,38 @@ int gem_snapshot_shown(gem_map *m);
 int gem_harvest_scrolled_out(gem_map *m, const float current_xy[2], const float shift_xy[2], void *host_points32,
                              int capacity, int *count_out);
 
+/* ---- local submaps on the device (ElevationMapping.cpp:609-767, :1124-1140, :1198-1226) ----
+ * gem_export_grid_cloud: gridMaptoPointCloud (:1198-1226).  source GEM_GRID_SHOWN reads the state show() publishes
+ *   (visualMap_: the current map after gem_compute_features), GEM_GRID_SNAPSHOT what gem_snapshot_shown kept (prevMap_),
+ *   with that snapshot's geometry; an error without a snapshot.  A cell is taken when elevation != -10 && traver != -10
+ *   && traver is not NaN (:1208) -- on show()'s output these are exactly the shown cells; unlike the harvest, cells
+ *   with a negative traversability other than -10 are taken.  One 32-byte PointXYZRGBICT record per cell, GridMapIterator
+ *   order, the layout of gem_harvest_scrolled_out (w = 1, a = 0xff), into caller-owned device memory.
+ *   *count_out = number of cells taken; min(count, capacity) records are written.  Host-synchronous.
+ * gem_harvest_to_local_map: the harvest of gem_harvest_scrolled_out (same cells, records and order), upserted into a
+ *   store owned by the handle, keyed by the bit patterns of the record's float (x, y) (GridPointEqual): a key already
+ *   present is replaced, across calls and within one call (the later cell in GridMapIterator order wins), as the
+ *   find / erase / insert of :740-747 does.  host_points32 may be NULL; when given, min(count, capacity) harvested
+ *   records are also copied there (for visualCloud_, :750-760).  *count_out = records harvested by this call.
+ * gem_local_map_take: localHashtoPointCloud (:1124-1140): the store's records into device memory, then the store is
+ *   empty.  Order DEFINED: all harvests since the last take / clear concatenated, only the last occurrence of each key
+ *   kept (an insertion-ordered map with erase-then-insert).  Fields DEFINED: intensity = the harvested value, w = 1,
+ *   a = 0xff.  If capacity < count nothing is written and the store is unchanged; *count_out is the size needed
+ *   (capacity 0 = size query).
+ * gem_local_map_clear: empty the store (the init branch, :697-698).
+ * gem_local_map_reserve: make room for `records` log records now.  The store is otherwise allocated on first use and
+ *   grows by doubling (from 1024 records) when a harvest needs more; once large enough, no call allocates.  A failed
+ *   growth returns GEM_ERR_NOMEM and leaves the store as it was.  Freed by gem_destroy.
+ * Tiled handles refuse all of these.  The store keeps every harvested record until the next take / clear (an append
+ * log, 32 B per record, plus an index of 24-48 B per record of capacity). */
+enum { GEM_GRID_SHOWN = 0, GEM_GRID_SNAPSHOT = 1 };
+int gem_export_grid_cloud(gem_map *m, int source, void *points32_device, int capacity, int *count_out);
+int gem_harvest_to_local_map(gem_map *m, const float current_xy[2], const float shift_xy[2], void *host_points32,
+                             int capacity, int *count_out);
+int gem_local_map_take(gem_map *m, void *points32_device, int capacity, int *count_out);
+int gem_local_map_clear(gem_map *m);
+int gem_local_map_reserve(gem_map *m, int records);
+
 /* raw layer access (row-major L*L, float or int32 for the colour ids) for tests and
  * checkpoint/restore (the dead G_get_mapinfo/G_set_mapinfo of gpu.cu:457-475). */
 int gem_get_layer(gem_map *m, int layer, void *host_out);

@@ -211,6 +211,43 @@ class ElevationMap {
         if (n) check(gem_harvest_scrolled_out(h_, current, shift, out.data(), n, &n), "gem_harvest_scrolled_out");
         return n;
     }
+    // The local submap on the device (ElevationMapping.cpp:609-767).  gridCloud: gridMaptoPointCloud (:1198-1226) of the
+    // shown map (GEM_GRID_SHOWN, visualMap_) or of the snapshot (GEM_GRID_SNAPSHOT, prevMap_) into device memory; returns
+    // the number of cells, min(that, capacity) records are written.  harvestToLocalMap: harvest() upserted into the
+    // handle's localMap_ (:740-747); `visual` (may be null) also receives the records, for visualCloud_.  localMapTake:
+    // localHashtoPointCloud (:1124-1140) into device memory, the store empties; with capacity < size nothing is written
+    // and the size is returned (capacity 0 = size query).  cutSubmap: the keyframe cut of :653-661, local map then grid
+    // cloud of the shown map, into one device buffer of `capacity` records; returns the size, writes only if it fits.
+    int gridCloud(int source, void *points32_device, size_t capacity)
+    {
+        int n = 0;
+        check(gem_export_grid_cloud(h_, source, points32_device, (int)capacity, &n), "gem_export_grid_cloud");
+        return n;
+    }
+    int harvestToLocalMap(const float current[2], const float shift[2], std::vector<PointXYZRGBICT> *visual = nullptr)
+    {
+        int n = 0;
+        if (visual) visual->resize((size_t)length_ * length_);
+        check(gem_harvest_to_local_map(h_, current, shift, visual ? visual->data() : nullptr, visual ? (int)visual->size() : 0, &n),
+              "gem_harvest_to_local_map");
+        if (visual) visual->resize((size_t)n);
+        return n;
+    }
+    int localMapTake(void *points32_device, size_t capacity)
+    {
+        int n = 0;
+        check(gem_local_map_take(h_, points32_device, (int)capacity, &n), "gem_local_map_take");
+        return n;
+    }
+    void localMapClear() { check(gem_local_map_clear(h_), "gem_local_map_clear"); }
+    int cutSubmap(void *points32_device, size_t capacity)
+    {
+        const int nl = localMapTake(nullptr, 0), ng = gridCloud(GEM_GRID_SHOWN, nullptr, 0);
+        if ((size_t)nl + (size_t)ng > capacity) return nl + ng;
+        localMapTake(points32_device, (size_t)nl);
+        gridCloud(GEM_GRID_SHOWN, (char *)points32_device + (size_t)nl * sizeof(PointXYZRGBICT), (size_t)ng);
+        return nl + ng;
+    }
     // Loop closure (ElevationMapping::updateGlobalMap, ElevationMapping.cpp:773-905), on device-resident submaps of
     // PointXYZRGBICT records: re-pose a submap (:805), and one pass of the pairwise fuse loop (:847-883) -- both clouds
     // come back reduced to one point per cell and compacted, *n_new / *n_old updated.  compat_precedence = true evaluates
