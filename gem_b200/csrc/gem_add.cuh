@@ -7,13 +7,14 @@
 //                            in a chunk addressed by the cell key, ranks 8..39 in a chunk addressed by the INDEX of
 //                            the point that drew rank 8 (published in the cell record); only the few cells with more
 //                            than 40 points take geometric chunks from a bump pool
-//   k_fold  1 thread or 1 warp/touched cell : order the cell's records by point index (== the order in which
-//                            G_fuse's per-cell loop visits them), sequential Kalman fold with the 5-sigma gate,
+//   k_fold  1 thread/touched cell with at most 8 records : order the cell's records by point index (== the order in
+//                            which G_fuse's per-cell loop visits them), sequential Kalman fold with the 5-sigma gate,
 //                            lowest-scan update, one 16 B write-back per cell.  The cells are found through a
-//                            per-point mark array (point i drew rank 0 / 8 / 40 of cell c): no global lists
-//   k_fold_long  1 warp/cell with more than 40 records, drawn from the queue k_bin filled (one atomic per such cell):
-//                            the longest list of a frame is the latency of the fold, and it runs 2-4x faster on a
-//                            scheduler of its own than next to seven busy warps
+//                            per-point mark array (point i drew rank 0 of cell c): no global list of touched cells
+//   k_fold_long  1 warp/cell with more than 8 records, drawn from the two queues k_bin filled (one atomic per cell that
+//                            reaches rank 8, one more per cell that reaches rank 40): a serial list runs 2-4x faster
+//                            on a scheduler of its own than next to seven busy warps, and the longest list of a frame
+//                            is the latency of the fold
 //
 // Round 1 had four kernels (transform+bin, per-cell allocation, scatter, fold) and five per-cell arrays; every
 // touched cell cost five random 32-byte sectors per call.  Here a cell IS one sector and the allocation and scatter
@@ -45,31 +46,35 @@ constexpr int FOLD_LONG_FROM = 40;       // = level_base(2): a cell with more re
 
 struct BinCounters { // one counter per 128-byte line
     int pool;     int pad0[31];  // pool slots handed out to chunks of level >= 2 (offset of the next chunk - 1)
-    int nlong;    int pad1[31];  // cells with more than 40 records (the long-list queue, a few hundred per frame)
-    int next_long;int pad2[31];  // k_fold_long's draw counter
+    int nlong;    int pad1[31];  // cells with more than 40 records (the long-list queue, ~100 per frame)
+    int next_long;int pad2[31];  // k_fold_long's draw counter (over the long-list queue, then the large-list queue)
     int ntouched; int pad3[31];  // statistics, accumulated by the folds: cells touched,
     int total;    int pad4[31];  //   points binned (accepted AND inside the grid / tile),
     int maxk;     int pad5[31];  //   longest per-cell list
     int nmarks;   int pad6[31];  // tiled maps: marks written by k_bin_peer (the fold's work list length)
+    int nlarge;   int pad7[31];  // cells with more than 8 records (the large-list queue, a few hundred per frame)
 };
 
-static_assert(sizeof(BinCounters) == 7 * 128, "one counter per 128-byte line");
+static_assert(sizeof(BinCounters) == 8 * 128, "one counter per 128-byte line");
 static_assert(sizeof(BinCounters) / sizeof(int) <= 256, "zero_next_counters: one thread per word of a 256-thread block");
 static_assert(FOLD_LONG_FROM == CHUNK0 + 32 && CHUNK1_SLOTS == 33, "second chunk = header + ranks 8..39");
 
-// what point i was for its cell: nothing, or the point that drew rank 0 / 8 / 40.  The fold finds its work here.
-enum { MARK_NONE = 0, MARK_FIRST = 1, MARK_LARGE = 2, MARK_LONG = 3 };
+// the queues of k_fold_long hold {key, LIST_*, i8, p2}: i8 = index of the cell's rank-8 point, p2 = pool offset of its
+// level-2 chunk (0 in a LIST_LARGE entry).  A cell with more than 40 records has an entry in both queues.
+enum { LIST_LARGE = 2, LIST_LONG = 3 };
 
 struct BinScratch { // one set per call parity
-    int4 *mark;        // [P]   {key, MARK_*, i8, p2}: i8 = index of the cell's rank-8 point, p2 = pool offset of its level-2 chunk
+    int2 *mark;        // [P]   {key, index of the cell in the lowest layer} if point i drew rank 0 of cell `key`, else key = -1
     uint4 *chunk0;     // [8 * cells] records of rank 0..7 of cell `key`
     uint4 *pool1;      // [33 * P]    level-1 chunks, addressed by the index of the rank-8 point
     uint4 *pool;       // [pool_cap + 1] chunks of level >= 2; offset 0 is never handed out
-    int4 *tlong;       // [P / 41 + 1] {key, MARK_LONG, i8, p2} of the cells that reached rank 40: the queue of k_fold_long
+    int4 *tlong;       // [long_cap]  {key, LIST_LONG, i8, p2} of the cells that reached rank 40: k_fold_long's first queue
+    int4 *tlarge;      // [large_cap] {key, LIST_LARGE, i8, 0} of the cells that reached rank 8: its second queue
     BinCounters *ctr;      // counters of this call (zero when it starts)
     BinCounters *ctr_next; // zeroed by this call's bin kernel for the call after
     int par;           // which {counter, i8 + 1} pair of the cell records this call uses
     int pool_cap;
+    int long_cap, large_cap; // entries of tlong / tlarge: P / 41 + 1 and P / 9 + 1 (at most as many as the map has cells, + 1)
     unsigned long long *stamps; // debug (gem_debug_stamps): %globaltimer marks of the kernels, else null
 };
 
@@ -288,7 +293,7 @@ __device__ __forceinline__ void bin_points(const MapGeom &g, const FrameParams &
         }
 #pragma unroll
         for (int u = 0; u < U; u++) rank[u] = (key[u] >= 0) ? atomicAdd(&cells[key[u]].bin[par].x, 1) : -1;
-        // ---- marks; the rank-8 point publishes itself; allocators of level >= 2 reserve their chunk --------------
+        // ---- marks; the rank-8 point publishes itself and queues the cell; allocators of level >= 2 reserve their chunk
         int lvl[U], myp[U];
 #pragma unroll
         for (int u = 0; u < U; u++) {
@@ -296,12 +301,9 @@ __device__ __forceinline__ void bin_points(const MapGeom &g, const FrameParams &
             lvl[u] = 0;
             myp[u] = 0;
             if (i >= n) continue;
-            int kind = MARK_NONE, i8 = 0;
-            if (rank[u] == 0) { kind = MARK_FIRST; i8 = geo[u]; } // a FIRST mark carries the cell's index in the lowest layer instead
-            else if (rank[u] == CHUNK0) {
-                kind = MARK_LARGE;
-                i8 = i;
+            if (rank[u] == CHUNK0) {
                 st_relaxed(&cells[key[u]].bin[par].y, i + 1);
+                sc.tlarge[atomicAdd(&sc.ctr->nlarge, 1)] = make_int4(key[u], LIST_LARGE, i, 0); // a few hundred per frame
             } else if (rank[u] >= FOLD_LONG_FROM) {
                 const int j = level_of(rank[u]);
                 if (rank[u] == level_base(j)) {
@@ -309,7 +311,7 @@ __device__ __forceinline__ void bin_points(const MapGeom &g, const FrameParams &
                     myp[u] = 1 + atomicAdd(&sc.ctr->pool, level_cap(j) + 1); // one per 128+ records of one cell: rare
                 }
             }
-            sc.mark[i] = make_int4(key[u], kind, i8, 0); // every point writes its mark (clears the previous call's)
+            sc.mark[i] = (rank[u] == 0) ? make_int2(key[u], geo[u]) : make_int2(-1, 0); // every point writes its mark (clears the previous call's)
         }
         // ---- chunk pointers of level >= 2, level by level ---------------------------------------------------------
         int maxl = 0;
@@ -322,7 +324,7 @@ __device__ __forceinline__ void bin_points(const MapGeom &g, const FrameParams &
                 const int i8 = spin_nonzero(&cells[key[u]].bin[par].y) - 1;
                 uint4 *q = sc.pool1 + (size_t)CHUNK1_SLOTS * i8;
                 for (int k = 2; k < l; k++) q = sc.pool + spin_next(q);
-                if (l == 2) sc.tlong[atomicAdd(&sc.ctr->nlong, 1)] = make_int4(key[u], MARK_LONG, i8, myp[u]); // a few hundred per frame
+                if (l == 2) sc.tlong[atomicAdd(&sc.ctr->nlong, 1)] = make_int4(key[u], LIST_LONG, i8, myp[u]); // ~100 per frame
                 publish_next(q, myp[u]);
             }
         }
@@ -347,7 +349,7 @@ __device__ __forceinline__ void bin_points(const MapGeom &g, const FrameParams &
 
 __device__ __forceinline__ void zero_next_counters(const BinScratch &sc, int tid)
 {
-    if (tid < (int)(sizeof(BinCounters) / sizeof(int))) ((int *)sc.ctr_next)[tid] = 0; // 224 ints: the bin grids have >= 256 threads
+    if (tid < (int)(sizeof(BinCounters) / sizeof(int))) ((int *)sc.ctr_next)[tid] = 0; // 256 ints: the bin grids have >= 256 threads
 }
 
 template <int SRC, int U>
@@ -578,13 +580,23 @@ __device__ __forceinline__ bool plain_state(float elev, float var)
     return elev != -10.0f && (elev == 0.0f || mag_ok(elev)) && ((var <= 1e-4f) ? 1e-4f : var) < 0x1p20f;
 }
 
+// 4-byte asynchronous copy global -> shared (no register holds the value in flight); cp.async.wait_all completes it
+__device__ __forceinline__ void cp_async4(float *dst, const char *src)
+{
+    const unsigned d = (unsigned)__cvta_generic_to_shared(dst);
+    asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"(d), "l"(src) : "memory");
+}
+
 // short lists (k <= 8): one thread per cell, records of chunk 0 held in registers, selection in index order.
-// The cell's record, its lowest value (index from the mark) and its first four records are requested together: one
-// round trip after the mark.  Nothing here is latency critical (the longest lists are): what counts is the instruction
-// count -- the plain step is tried first, the literal one only when a step leaves it, and the one intensity the cell
-// ends up with is read at the end.  Returns the list length (0 when the cell is folded by a warp instead).
+// The cell's record, its lowest value (index from the mark) and all eight slots of chunk 0 (one 128-byte line; the
+// slots beyond k hold stale bits and are masked) are requested together: one round trip after the mark.  The intensity
+// of every record that may give the cell its colour is requested as soon as the records are there, into the thread's
+// eight slots of s_int (s_int[e * ADD_BLOCK + threadIdx.x]), so it arrives under the fold instead of one round trip
+// after it.  What counts besides those round trips is the instruction count: the plain step is tried first, the
+// literal one only when a step leaves it.  Returns the list length (0 when the cell is k_fold_long's).
 __device__ __forceinline__ int fold_small_cell(const MapGeom &g, const MapLayers &ml, const BinScratch &sc, const FoldSrc &src,
-                                               const RegionOps &ro_next, int key, int low_idx, bool do_fuse, bool do_lowest)
+                                               const RegionOps &ro_next, int key, int low_idx, bool do_fuse, bool do_lowest,
+                                               float *s_int)
 {
     const uint4 *c0 = sc.chunk0 + (size_t)CHUNK0 * key;
     const int k = ml.cell[key].bin[sc.par].x;
@@ -592,16 +604,18 @@ __device__ __forceinline__ int fold_small_cell(const MapGeom &g, const MapLayers
     cell_begin(s, g, ml, key, do_lowest, low_idx);
     uint4 rr[CHUNK0];
 #pragma unroll
-    for (int e = 0; e < 4; e++) rr[e] = c0[e];
-    // k > 8: folded by a warp (fold_cell_warp).  k == 0: that warp (or k_fold_long, which may run concurrently) has already
-    // folded the cell and reset its counter -- a cell with a FIRST mark has at least one record until its owner resets it.
-    // Either way the cell is not this thread's: it must not even rewrite the state it loaded.
+    for (int e = 0; e < CHUNK0; e++) rr[e] = c0[e];
+    // k > 8: folded by a warp of k_fold_long.  k == 0: k_fold_long, which may run concurrently, has already folded the
+    // cell and reset its counter -- a cell with a mark has at least one record until its owner resets it.  Either way
+    // the cell is not this thread's: it must not even rewrite the state it loaded.
     if (k > CHUNK0 || k == 0) return 0;
 #pragma unroll
-    for (int e = 4; e < CHUNK0; e++) {
-        rr[e] = make_uint4(0u, 0u, 0u, 0u);
-        if (e < k) rr[e] = c0[e];
+    for (int e = 0; e < CHUNK0; e++) {
+        if (e >= k) rr[e].x = 0x7fffffffu; // index padding: never selected
+        if (e < k && do_fuse && src.base && (rr[e].w & REC_COLOUR_OK)) // lands in s_int without holding a register
+            cp_async4(s_int + e * ADD_BLOCK + threadIdx.x, src.base + (size_t)rr[e].x * src.stride);
     }
+    asm volatile("cp.async.commit_group;" ::: "memory");
     const CellState s0 = s;
     const bool start_plain = do_fuse && plain_state(s.elev, s.var);
     bool plain = start_plain;
@@ -612,7 +626,7 @@ __device__ __forceinline__ int fold_small_cell(const MapGeom &g, const MapLayers
             uint4 b = make_uint4(0u, 0u, 0u, 0u);
 #pragma unroll
             for (int e = 0; e < CHUNK0; e++) {
-                const int ie = (e < k) ? (int)rr[e].x : 0x7fffffff;
+                const int ie = (int)rr[e].x;
                 const bool c = ie > last && ie < best;
                 if (c) { best = ie; b = rr[e]; }
             }
@@ -630,7 +644,13 @@ __device__ __forceinline__ int fold_small_cell(const MapGeom &g, const MapLayers
         if (pass == 0 && start_plain && !plain) { s = s0; continue; } // left the plain path: literal from the start
         break;
     }
-    cell_end(s, g, ml, sc, src, ro_next, key, do_fuse, do_lowest, false);
+    int se = 0;
+#pragma unroll
+    for (int e = 0; e < CHUNK0; e++) // the slot of the record the cell took its colour from (indices are unique)
+        if (rr[e].x == s.src) se = e;
+    asm volatile("cp.async.wait_all;" ::: "memory");
+    s.inten = (src.base && s.ci_dirty) ? s_int[se * ADD_BLOCK + threadIdx.x] : 0.0f;
+    cell_end(s, g, ml, sc, src, ro_next, key, do_fuse, do_lowest, true);
     return k;
 }
 
@@ -816,68 +836,62 @@ __device__ __forceinline__ void warp_bitonic(uint32_t (&key)[R], unsigned lane)
     }
 }
 
-// per-warp shared scratch.  k_fold_long's warps fold lists of any length; k_fold's only lists of 9..40 records.
-template <int N> struct WarpScratchT {
-    uint4 rec[N];          // the records of a list of <= N (N = 256: or the sort keys of a list of <= 1024)
-    uint32_t idx[N];       // their point indices, compact (read four at a time by the rank count)
-    unsigned char perm[N]; // position in index order -> rank
-};
-typedef WarpScratchT<FOLD_RANK_K> LongScratch; // 5.25 KB
-typedef WarpScratchT<64> LargeScratch;         // 1.3 KB
-struct WarpScratch { // a view of either
-    uint4 *rec;
-    uint32_t *idx;
-    unsigned char *perm;
-    int cap; // lists longer than this are not this warp's job
-    template <int N> __device__ explicit WarpScratch(WarpScratchT<N> &s) : rec(s.rec), idx(s.idx), perm(s.perm), cap(N) {}
+// per-warp shared scratch of k_fold_long
+struct WarpScratch {
+    uint4 rec[FOLD_RANK_K];          // the records of a list of <= 256 (or the sort keys of a list of <= 1024)
+    uint32_t idx[FOLD_RANK_K];       // their point indices, compact (read four at a time by the rank count)
+    unsigned char perm[FOLD_RANK_K]; // position in index order -> rank
 };
 
-// one warp folds one cell with more than 8 records.  info = the cell's mark {key, MARK_LARGE | MARK_LONG, i8, p2}.
-// Returns the list length (0: not this mark's job).
+constexpr int FOLD_ROWS = 8; // 32-record rows a list may occupy in registers
+
+// one warp folds one cell with more than 8 records.  info = the cell's queue entry {key, LIST_LARGE | LIST_LONG, i8, p2}.
+// Returns the list length (0: not this entry's job).
 //   k <= 256: the records are read ONCE, coalesced in rank order, into shared memory; the intensity of every record
 //     is requested from the input as soon as the records are there (it arrives under the ordering work); every lane
 //     counts, for each of its records, how many records of the list carry a smaller point index (16-byte broadcast
 //     reads of the compact index array) -- that count is the record's position in G_fuse's visiting order;
 //   k <= 1024: bitonic sort of packed (index, rank) keys in shared memory, records gathered per chunk;
 //   longer: repeated selection of the next smallest index from global memory.
-// ROWS: 32-record rows the list may occupy in registers (2: k_fold, lists of at most 40; 8: k_fold_long)
-template <int ROWS>
 __device__ __noinline__ int fold_cell_warp(const MapGeom &g, const MapLayers &ml, const BinScratch &sc, const FoldSrc &src,
-                                           const RegionOps &ro_next, bool do_fuse, bool do_lowest, const WarpScratch ws, int4 info)
+                                           const RegionOps &ro_next, bool do_fuse, bool do_lowest, WarpScratch &ws, int4 info)
 {
+    constexpr int ROWS = FOLD_ROWS;
     const unsigned lane = threadIdx.x & 31u;
-    const bool from_long = info.y == MARK_LONG;
+    const bool from_long = info.y == LIST_LONG;
     const int key = info.x;
     ChunkRefs c;
     c.key = key; c.i8 = info.z; c.p[0] = 0; c.p[1] = 0; c.p[2] = info.w; c.p[3] = 0; c.p[4] = 0;
     const unsigned long long t0 = (sc.stamps && from_long) ? globaltimer_ns() : 0ull;
-    // k_fold (lists of 9..40): where the 40 slots are follows from the mark alone (chunk0 by key, the second chunk by the
-    // index of the rank-8 point), so they are requested together with the cell instead of one round trip later; the slots
-    // beyond the list length hold stale bits and are masked once the length has arrived
-    uint4 spec0 = make_uint4(0u, 0u, 0u, 0u), spec1 = spec0;
-    if (ROWS == 2) {
-        spec0 = *record_ptr(sc, c, (int)lane);
-        if (lane < (unsigned)(FOLD_LONG_FROM - 32)) spec1 = *record_ptr(sc, c, (int)lane + 32);
-    }
+    // where the first 40 slots are follows from the entry alone (chunk0 by key, the second chunk by the index of the
+    // rank-8 point), and so does the header of a long list's level-2 chunk: all are requested together with the cell
+    // instead of one round trip later.  The slots beyond the list length hold stale bits and are masked once the length
+    // has arrived; the header is used only by lists that have a level-3 chunk (pool offset 0, where a LARGE entry's p2
+    // points, is never handed out and reads as zeros)
+    const uint4 spec0 = *record_ptr(sc, c, (int)lane);
+    uint4 spec1 = make_uint4(0u, 0u, 0u, 0u);
+    if (lane < (unsigned)(FOLD_LONG_FROM - 32)) spec1 = *record_ptr(sc, c, (int)lane + 32);
+    const int p3 = next_chunk(sc.pool + c.p[2]);
     const int k = ml.cell[key].bin[sc.par].x;
     CellState s;
     cell_begin(s, g, ml, key, do_lowest);
-    // a LARGE mark whose cell also reached rank 40 is k_fold_long's; its counter reads > 40, or 0 once that kernel is done with it
+    // a LARGE entry whose cell also reached rank 40 is folded by its LONG entry; its counter reads > 40, or 0 once that
+    // entry is done with it
     if (!from_long && (k > FOLD_LONG_FROM || k == 0)) return 0;
     if (k > 0) stamp_since(sc, 3, t0); // list length arrived
-    if (k > level_base(3)) c.p[3] = next_chunk(sc.pool + c.p[2]);
+    if (k > level_base(3)) c.p[3] = p3;
     if (k > level_base(4)) c.p[4] = next_chunk(sc.pool + c.p[3]);
     bool have_inten = false;
     uint32_t *s_key = reinterpret_cast<uint32_t *>(ws.rec);
     if (k <= 32 * ROWS) {
         have_inten = true;
         const int rows = (k + 31) >> 5;
-        uint4 rec[ROWS < 2 ? 2 : ROWS];
+        uint4 rec[ROWS];
 #pragma unroll
         for (int r = 0; r < ROWS; r++) { // all record loads first ...
             const int e = (int)lane + 32 * r;
             rec[r] = make_uint4(0x7fffffffu, 0u, 0u, 0u); // index padding: never smaller than a real index
-            if (r < rows && e < k) rec[r] = (ROWS == 2) ? (r == 0 ? spec0 : spec1) : *record_ptr(sc, c, e);
+            if (r < rows && e < k) rec[r] = (e < FOLD_LONG_FROM) ? (r == 0 ? spec0 : spec1) : *record_ptr(sc, c, e);
         }
         float it[ROWS];
 #pragma unroll
@@ -891,7 +905,7 @@ __device__ __noinline__ int fold_cell_warp(const MapGeom &g, const MapLayers &ml
         }
         __syncwarp();
         if (rec[0].y != 0x7fc12345u) stamp_since(sc, 4, t0); // records arrived, indices in shared memory
-        if (ROWS < 8 || k <= 64) {
+        if (k <= 64) {
             // position of a record = number of records with a smaller point index.  Indices are < 2^22 and the padding
             // is 0x7fffffff, so (x - mine) >> 31 is exactly [x < mine]: three independent instructions per comparison
             const int k4 = (k + 3) >> 2;
@@ -906,7 +920,7 @@ __device__ __noinline__ int fold_cell_warp(const MapGeom &g, const MapLayers &ml
             if ((int)lane + 32 < k) ws.perm[p1] = (unsigned char)(lane + 32);
         } else {
             // register bitonic network on (index << 10 | rank) keys; the padding sorts last
-            uint32_t key8[ROWS < 8 ? 8 : ROWS];
+            uint32_t key8[ROWS];
 #pragma unroll
             for (int r = 0; r < 8; r++) key8[r] = 0xffffffffu;
 #pragma unroll
@@ -936,7 +950,7 @@ __device__ __noinline__ int fold_cell_warp(const MapGeom &g, const MapLayers &ml
         }
         __syncwarp();
         stamp_since(sc, 5, t0); // ordered, intensities in place
-    } else if (ROWS == 8 && k <= FOLD_KMAX) {
+    } else if (k <= FOLD_KMAX) {
         int P = 512;
         while (P < k) P <<= 1;
         for (int e = (int)lane; e < P; e += 32)
@@ -955,7 +969,7 @@ __device__ __noinline__ int fold_cell_warp(const MapGeom &g, const MapLayers &ml
             }
         }
     }
-    if (k <= 32 * ROWS || (ROWS == 8 && k <= FOLD_KMAX)) { // the one chunk loop of the kernel (order the records by point index == G_fuse's visiting order)
+    if (k <= FOLD_KMAX) { // the one chunk loop of the kernel (order the records by point index == G_fuse's visiting order)
         for (int c0 = 0; c0 < k; c0 += 32) {
             uint4 r = make_uint4(0u, 0u, 0u, 0u);
             if (c0 + (int)lane < k) {
@@ -987,7 +1001,8 @@ __device__ __noinline__ int fold_cell_warp(const MapGeom &g, const MapLayers &ml
         }
     }
     if (s.elev != 12345.678f) stamp_since(sc, 6, t0); // folded
-    stamp_lane0(sc, 12, from_long && s.elev != 12345.678f);
+    stamp_lane0(sc, 12, from_long && s.elev != 12345.678f);  // latest list of > 40 folded
+    stamp_lane0(sc, 14, !from_long && s.elev != 12345.678f); // latest list of 9..40 folded
     if (lane == 0u) {
         cell_end(s, g, ml, sc, src, ro_next, key, do_fuse, do_lowest, have_inten);
         if (k > FOLD_LONG_FROM) { // clear the headers this list's chunks published (every chunk but the last): no stale tags
@@ -1004,23 +1019,20 @@ __device__ __noinline__ int fold_cell_warp(const MapGeom &g, const MapLayers &ml
 
 constexpr int FOLD_MARKS = 2; // marks per thread and pass: a block's slice is FOLD_MARKS * blockDim.x consecutive points
 
-// k_fold: everything but the long lists.  One block folds the cells whose marks lie in its slices of the point index
-// range.  The marks of a slice are read coalesced and sorted into two shared-memory queues: cells with 9..40 records
-// (MARK_LARGE; a cell that also reached rank 40 is k_fold_long's) and the keys of all touched cells.  The warps draw
-// work from the queues dynamically: first the large cells, one per warp, then the short lists, 32 at a time, one per
-// thread.  fold_blocks blocks fold; blocks beyond them execute `ro` (row / column clears of the NEXT call's Move,
-// pipelined mode only: a cell inside such a region is written with the cleared value by whoever touches it, see cell_end).
+// k_fold: the cells with at most 8 records.  One block folds the cells whose marks lie in its slices of the point index
+// range.  The marks of a slice are read coalesced and the touched cells queued in shared memory; the warps draw them 32
+// at a time, one per thread (a cell with more records is skipped: k_fold_long folds it).  fold_blocks blocks fold;
+// blocks beyond them execute `ro` (row / column clears of the NEXT call's Move, pipelined mode only: a cell inside such
+// a region is written with the cleared value by whoever touches it, see cell_end).
 __global__ void __launch_bounds__(ADD_BLOCK, 3)
 k_fold(MapGeom g, MapLayers ml, BinScratch sc, FoldSrc src, const __grid_constant__ RegionOps ro, int n, int fold_blocks, int slice, int do_fuse_i, int do_lowest_i,
        const int *n_dev)
 {
     if (n_dev) n = min(n, *n_dev); // tiled maps: the number of marks is known on the device only (k_bin_peer)
-    constexpr int SLICE = FOLD_MARKS * ADD_BLOCK;
-    extern __shared__ __align__(16) unsigned char s_dyn[]; // FOLD_SMEM_BYTES: per-warp scratch + the two queues (+ padding, see k_fold_long)
-    LargeScratch *s_ws = reinterpret_cast<LargeScratch *>(s_dyn);
-    int4 *s_big = reinterpret_cast<int4 *>(s_dyn + (ADD_BLOCK / 32) * sizeof(LargeScratch));
-    int2 *s_first = reinterpret_cast<int2 *>(s_big + SLICE);
-    __shared__ int s_nlarge, s_nfirst, s_next_big, s_next_first, s_stat[3];
+    extern __shared__ __align__(16) unsigned char s_dyn[]; // FOLD_SMEM_BYTES: the queue, the intensities (+ padding, see k_fold_long)
+    int2 *s_first = reinterpret_cast<int2 *>(s_dyn);
+    float *s_int = reinterpret_cast<float *>(s_first + FOLD_MARKS * ADD_BLOCK);
+    __shared__ int s_nfirst, s_next_first, s_stat[3];
     if ((int)blockIdx.x >= fold_blocks) {
         const size_t rb = gridDim.x - fold_blocks;
         phase_regions(g, ml, ro, (size_t)(blockIdx.x - fold_blocks) * blockDim.x + threadIdx.x, rb * blockDim.x);
@@ -1031,51 +1043,40 @@ k_fold(MapGeom g, MapLayers ml, BinScratch sc, FoldSrc src, const __grid_constan
     const unsigned lane = threadIdx.x & 31u;
     stamp_start(sc, 8);
     if (threadIdx.x == 0) { s_stat[0] = 0; s_stat[1] = 0; s_stat[2] = 0; }
-    // slice = points per block and pass (<= SLICE, chosen by the host so that one pass covers a frame-sized call)
+    // slice = points per block and pass (<= FOLD_MARKS * ADD_BLOCK, chosen by the host so that one pass covers a frame-sized call)
     for (int base = blockIdx.x * slice; base < n; base += fold_blocks * slice) {
-        if (threadIdx.x == 0) { s_nlarge = 0; s_nfirst = 0; s_next_big = 0; s_next_first = 0; }
+        if (threadIdx.x == 0) { s_nfirst = 0; s_next_first = 0; }
         __syncthreads();
 #pragma unroll
         for (int u = 0; u < FOLD_MARKS; u++) {
             const int o = u * ADD_BLOCK + threadIdx.x, i = base + o;
-            int4 mk = make_int4(-1, MARK_NONE, 0, 0);
+            int2 mk = make_int2(-1, 0);
             if (o < slice && i < n) mk = sc.mark[i];
-            if (mk.y == MARK_LARGE) s_big[atomicAdd(&s_nlarge, 1)] = mk;
-            const unsigned fm = __ballot_sync(0xffffffffu, mk.y == MARK_FIRST);
+            const unsigned fm = __ballot_sync(0xffffffffu, mk.x >= 0);
             if (fm) { // warp-aggregated append of the touched cells {key, lowest index}
                 int fb = 0;
                 if (lane == 0u) fb = atomicAdd(&s_nfirst, __popc(fm));
                 fb = __shfl_sync(0xffffffffu, fb, 0);
-                if (mk.y == MARK_FIRST) s_first[fb + __popc(fm & ((1u << lane) - 1u))] = make_int2(mk.x, mk.z);
+                if (mk.x >= 0) s_first[fb + __popc(fm & ((1u << lane) - 1u))] = mk;
             }
         }
         __syncthreads();
-        const int nbig = s_nlarge, nfirst = s_nfirst;
+        const int nfirst = s_nfirst;
         stamp_mark(sc, 9); // marks of the slice read and queued
-        int wk = 0, wtot = 0, tk = 0, tsum = 0;
-        for (;;) { // large cells: one per warp and draw
-            int j = 0;
-            if (lane == 0u) j = atomicAdd(&s_next_big, 1);
-            j = __shfl_sync(0xffffffffu, j, 0);
-            if (j >= nbig) break;
-            const int k = fold_cell_warp<2>(g, ml, sc, src, ro, do_fuse, do_lowest, WarpScratch(s_ws[w]), s_big[j]);
-            wk = max(wk, k);
-            wtot += k;
-        }
-        stamp_mark(sc, 11); // the block's first warp has no large cell left
-        for (;;) { // short lists: 32 per warp and draw, one per thread
+        int tk = 0, tsum = 0;
+        for (;;) { // 32 cells per warp and draw, one per thread
             int j = 0;
             if (lane == 0u) j = atomicAdd(&s_next_first, 32);
             j = __shfl_sync(0xffffffffu, j, 0);
             if (j >= nfirst) break;
             if (j + (int)lane < nfirst) {
                 const int2 c = s_first[j + lane];
-                const int k = fold_small_cell(g, ml, sc, src, ro, c.x, c.y, do_fuse, do_lowest);
+                const int k = fold_small_cell(g, ml, sc, src, ro, c.x, c.y, do_fuse, do_lowest, s_int);
                 tk = max(tk, k);
                 tsum += k;
             }
         }
-        stamp_mark(sc, 13); // ... and no short list
+        stamp_mark(sc, 13); // the block's first warp has no cell left
         // statistics: points binned, longest list (cells touched = nfirst)
         int tmax = tk;
 #pragma unroll
@@ -1084,11 +1085,11 @@ k_fold(MapGeom g, MapLayers ml, BinScratch sc, FoldSrc src, const __grid_constan
             tmax = max(tmax, __shfl_xor_sync(0xffffffffu, tmax, d));
         }
         if (lane == 0u) {
-            if (tsum + wtot) atomicAdd(&s_stat[1], tsum + wtot);
-            atomicMax(&s_stat[2], max(tmax, wk));
+            if (tsum) atomicAdd(&s_stat[1], tsum);
+            atomicMax(&s_stat[2], tmax);
             if (w == 0) s_stat[0] += nfirst;
         }
-        __syncthreads(); // the queues are reset by the next pass
+        __syncthreads(); // the queue is reset by the next pass
     }
     if (threadIdx.x == 0) { // three reductions per block, no return value
         if (s_stat[0]) atomicAdd(&sc.ctr->ntouched, s_stat[0]);
@@ -1097,15 +1098,16 @@ k_fold(MapGeom g, MapLayers ml, BinScratch sc, FoldSrc src, const __grid_constan
     }
     stamp_mark(sc, 10);
 }
-constexpr size_t FOLD_SMEM_USED = (ADD_BLOCK / 32) * sizeof(LargeScratch) + (size_t)FOLD_MARKS * ADD_BLOCK * (sizeof(int4) + sizeof(int2));
+constexpr size_t FOLD_SMEM_USED = (size_t)FOLD_MARKS * ADD_BLOCK * sizeof(int2) + (size_t)CHUNK0 * ADD_BLOCK * sizeof(float);
 
-// k_fold_long: the cells with more than 40 records, drawn from the queue the bin kernel filled (one atomic per cell,
-// a few hundred per frame).  A long list is a serial chain of dependent steps per record, several times slower next
-// to busy warps than with a scheduler to itself (scripts/micro_fold.cu measures both) -- and the longest list of a
-// frame IS the latency of the fold.  So the long
-// lists get SMs of their own: LONG_BLOCKS blocks of four warps (one per scheduler), each asking for so much shared
-// memory (LONG_SMEM_BYTES, mostly unused) that no other block of this or a concurrently running kernel fits beside it
-// (k_fold needs 51 KB, k_bin asks for BIN_SMEM_BYTES for exactly this reason).
+// k_fold_long: the cells with more than 8 records, drawn from the two queues the bin kernel filled (one atomic per cell
+// and queue, a few hundred per frame): the cells with more than 40 records first, so that the longest lists start
+// first, then those with more than 8 (a cell on both queues is folded by its first entry).  A list is a serial chain of
+// dependent steps per record, several times slower next to busy warps than with a scheduler to itself
+// (scripts/micro_fold.cu measures both) -- and the longest list of a frame IS the latency of the fold.  So the lists
+// get warps of their own, away from k_fold's short-list selection loops: blocks of four warps (one per scheduler).  With GEM_B200_EXCLUSIVE=1 they get SMs of their own as well: each block asks for so
+// much shared memory (LONG_SMEM_BYTES, mostly unused) that no other block of this or a concurrently running kernel fits
+// beside it (k_fold and k_bin then ask for at least BIN_SMEM_BYTES for exactly this reason).
 constexpr int LONG_BLOCK = 128;
 constexpr int LONG_BLOCKS = 32;
 constexpr size_t LONG_SMEM_BYTES = 200 * 1024;
@@ -1115,21 +1117,22 @@ __global__ void __launch_bounds__(LONG_BLOCK, 1)
 k_fold_long(MapGeom g, MapLayers ml, BinScratch sc, FoldSrc src, const __grid_constant__ RegionOps ro, int do_fuse_i, int do_lowest_i)
 {
     extern __shared__ __align__(16) unsigned char s_dyn[];
-    LongScratch *s_ws = reinterpret_cast<LongScratch *>(s_dyn);
+    WarpScratch *s_ws = reinterpret_cast<WarpScratch *>(s_dyn);
     const int w = threadIdx.x >> 5;
     const unsigned lane = threadIdx.x & 31u;
-    const int nlong = sc.ctr->nlong;
+    const int nlong = sc.ctr->nlong, nall = nlong + sc.ctr->nlarge;
     int wk = 0, wtot = 0;
     for (;;) {
         int j = 0;
         if (lane == 0u) j = atomicAdd(&sc.ctr->next_long, 1);
         j = __shfl_sync(0xffffffffu, j, 0);
-        if (j >= nlong) break;
-        const int k = fold_cell_warp<8>(g, ml, sc, src, ro, do_fuse_i != 0, do_lowest_i != 0, WarpScratch(s_ws[w]), sc.tlong[j]);
+        if (j >= nall) break;
+        const int4 info = (j < nlong) ? sc.tlong[j] : sc.tlarge[j - nlong];
+        const int k = fold_cell_warp(g, ml, sc, src, ro, do_fuse_i != 0, do_lowest_i != 0, s_ws[w], info);
         wk = max(wk, k);
         wtot += k;
     }
-    if (lane == 0u && wtot) { // the short-list statistics come from k_fold (these cells' FIRST marks count them as touched)
+    if (lane == 0u && wtot) { // the short-list statistics come from k_fold (these cells' marks count them as touched)
         atomicAdd(&sc.ctr->total, wtot);
         atomicMax(&sc.ctr->maxk, wk);
     }

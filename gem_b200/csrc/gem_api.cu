@@ -97,7 +97,7 @@ struct gem_map {
     // tuning (scripts/pipe_sweep.sh sweeps them): GEM_B200_FOLD_BLOCKS, GEM_B200_LONG_BLOCKS,
     // GEM_B200_EXCLUSIVE=1 pads the kernels' shared memory so that k_fold_long's blocks get SMs of their own
     int fold_max_blocks = NUM_SMS * 2, long_blocks = LONG_BLOCKS;
-    size_t bin_smem = 0, fold_smem = FOLD_SMEM_USED, long_smem = (LONG_BLOCK / 32) * sizeof(LongScratch);
+    size_t bin_smem = 0, fold_smem = FOLD_SMEM_USED, long_smem = (LONG_BLOCK / 32) * sizeof(WarpScratch);
     int pipe_mode = 2;               // 0: never defer the fold; 1: two streams + events; 2: CUDA graph per call
     std::map<const void *, FrameGraph> graphs; // keyed by the bin kernel function
     cudaStream_t front_stream = nullptr;      // pipe_mode 1: the bin kernels run here
@@ -153,11 +153,12 @@ struct gem_map {
 namespace {
 
 using Lock = std::lock_guard<std::recursive_mutex>;
-// k_fold_long's grid (four warps per block, one long list per warp and draw): a frame has a few hundred long lists, a
-// million-point call a few thousand
+// k_fold_long's grid (four warps per block, one list per warp and draw): a c2 lidar frame (125k points) has 330-420
+// lists of more than 8 records and runs best with ~100-150 blocks; a c3 depth frame (307k points, ~13 per touched cell)
+// has far more lists and runs faster the more blocks it gets, up to the cap (DESIGN.md section 4, decision 5)
 inline int long_blocks_for(const gem_map *m, int n)
 {
-    const int b = n / 2048;
+    const int b = n / 1024;
     return b < m->long_blocks ? m->long_blocks : (b > NUM_SMS * 4 ? NUM_SMS * 4 : b);
 }
 // points per block and pass of k_fold: an even share of the call, in whole warps, at most FOLD_MARKS marks per thread
@@ -467,6 +468,7 @@ int read_counters(gem_map *m, long long n_in, bool accumulate)
     m->stats.points_binned += m->h_ctr->total;
     m->stats.cells_touched += m->h_ctr->ntouched;
     if (m->h_ctr->pool > m->bs[0].pool_cap) return fail(m, GEM_ERR_CUDA, "internal: record pool exhausted");
+    if (m->h_ctr->nlong >= m->bs[0].long_cap || m->h_ctr->nlarge >= m->bs[0].large_cap) return fail(m, GEM_ERR_CUDA, "internal: list queue overflow");
     if (m->h_ctr->maxk > m->stats.max_points_per_cell) m->stats.max_points_per_cell = m->h_ctr->maxk;
     return GEM_OK;
 }
@@ -741,7 +743,7 @@ int gem_create(const gem_config *cfg, gem_map **out)
     m->geom.c0 = tiled ? cfg->tile_col0 : 0;
     m->geom.cols = tiled ? cfg->tile_cols : m->L;
     m->nc = (size_t)m->geom.rows * m->geom.cols;
-    m->P = cfg->max_points > 0 ? cfg->max_points : (1 << 20); // per point: 16 B mark + 528 B level-1 chunk space, x 2 parities
+    m->P = cfg->max_points > 0 ? cfg->max_points : (1 << 20); // per point: 8 B mark + 528 B level-1 chunk space, x 2 parities
     // the fold's sort key packs the point index of a launch into 22 bits; larger calls are chunked
     if (m->P > (1 << FOLD_INDEX_BITS)) m->P = 1 << FOLD_INDEX_BITS;
     {
@@ -780,9 +782,11 @@ int gem_create(const gem_config *cfg, gem_map **out)
         sc.par = p;
         // only cells with more than 40 records take pool chunks: at most 4k + 12 slots for a cell of k records
         sc.pool_cap = (int)std::min<size_t>(5 * P + 64, (size_t)0x7ffffff0);
+        sc.long_cap = (int)list_cap(P, nc, FOLD_LONG_FROM);
+        sc.large_cap = (int)list_cap(P, nc, CHUNK0);
         if ((rc = dev_alloc(m, &sc.mark, P)) || (rc = dev_alloc(m, &sc.chunk0, (size_t)CHUNK0 * nc)) ||
             (rc = dev_alloc(m, &sc.pool1, (size_t)CHUNK1_SLOTS * P)) || (rc = dev_alloc(m, &sc.pool, (size_t)sc.pool_cap + 1)) ||
-            (rc = dev_alloc(m, &sc.tlong, list_cap(P, nc, FOLD_LONG_FROM))))
+            (rc = dev_alloc(m, &sc.tlong, (size_t)sc.long_cap)) || (rc = dev_alloc(m, &sc.tlarge, (size_t)sc.large_cap)))
             return bail(rc);
         // no stale chunk headers (the fold clears the ones it consumes); records and marks need no initialisation
         e = cudaMemsetAsync(sc.pool1, 0, (size_t)CHUNK1_SLOTS * P * sizeof(uint4), m->stream);

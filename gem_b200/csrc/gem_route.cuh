@@ -283,14 +283,15 @@ __device__ __forceinline__ void bin_one(Cell *cells, const BinScratch &sc, int k
 {
     const int par = sc.par;
     const int rank = (key >= 0) ? atomicAdd(&cells[key].bin[par].x, 1) : -1;
-    int kind = MARK_NONE, z = 0, lvl = 0, myp = 0;
-    if (rank == 0) { kind = MARK_FIRST; z = geo; }
-    else if (rank == CHUNK0) { kind = MARK_LARGE; z = i_rec; st_relaxed(&cells[key].bin[par].y, i_rec + 1); }
-    else if (rank >= FOLD_LONG_FROM) {
+    int lvl = 0, myp = 0;
+    if (rank == CHUNK0) {
+        st_relaxed(&cells[key].bin[par].y, i_rec + 1);
+        sc.tlarge[atomicAdd(&sc.ctr->nlarge, 1)] = make_int4(key, LIST_LARGE, i_rec, 0);
+    } else if (rank >= FOLD_LONG_FROM) {
         const int j = level_of(rank);
         if (rank == level_base(j)) { lvl = j; myp = 1 + atomicAdd(&sc.ctr->pool, level_cap(j) + 1); }
     }
-    sc.mark[i_mark] = make_int4(key, kind, z, 0);
+    sc.mark[i_mark] = (rank == 0) ? make_int2(key, geo) : make_int2(-1, 0);
     if (rank < 0) return;
     uint4 *dst;
     if (rank < CHUNK0) {
@@ -302,7 +303,7 @@ __device__ __forceinline__ void bin_one(Cell *cells, const BinScratch &sc, int k
         if (lvl >= 2) { // publish the chunk this point allocated in the header of the level below
             uint4 *below = q;
             for (int k = 2; k < lvl; k++) below = sc.pool + spin_next(below);
-            if (lvl == 2) sc.tlong[atomicAdd(&sc.ctr->nlong, 1)] = make_int4(key, MARK_LONG, i8, myp);
+            if (lvl == 2) sc.tlong[atomicAdd(&sc.ctr->nlong, 1)] = make_int4(key, LIST_LONG, i8, myp);
             publish_next(below, myp);
         }
         for (int k = 2; k <= j; k++) q = sc.pool + ((lvl == k) ? myp : spin_next(q));

@@ -37,6 +37,6 @@ if os.environ.get("ADD_LOOP_STAMPS", "0") == "1":
         m.debug_stamps(True)
         step(K + 300 + s)
         st = m.debug_stamps(True)
-        res.append([(st[9] - st[8]) / 1e3, (st[11] - st[8]) / 1e3, (st[13] - st[8]) / 1e3, (st[10] - st[8]) / 1e3] + [st[i] / 1e3 for i in (3, 4, 7, 5, 6)])
-    res = np.median(np.array(res), axis=0)
-    print("k_fold us since its first block started (latest first warp of any block): marks queued %.2f, large cells done %.2f, short lists done %.2f, end %.2f || slowest long list since its own start: k known %.2f, records arrived %.2f, positions counted %.2f, intensities in place %.2f, folded %.2f" % tuple(res))
+        res.append([(st[i] - st[8]) / 1e3 if st[i] else np.nan for i in (9, 13, 10, 14, 12)] + [st[i] / 1e3 for i in (3, 4, 7, 5, 6)])
+    res = np.nanmedian(np.array(res), axis=0)
+    print("us since k_fold's first block started: k_fold (latest first warp of any block): marks queued %.2f, short lists done %.2f, end %.2f; k_fold_long: last list of 9..40 folded %.2f, last list of > 40 folded %.2f || slowest list of > 40 since its own start: k known %.2f, records arrived %.2f, positions counted %.2f, intensities in place %.2f, folded %.2f" % tuple(res))
