@@ -65,6 +65,11 @@ class GemProfile(C.Structure):
     _fields_ = [("launches", C.c_longlong), ("ms", C.c_double * 9), ("count", C.c_longlong * 9)]
 
 
+class GemGridSplit(C.Structure):
+    _fields_ = [("points", C.c_int), ("valid", C.c_int), ("road", C.c_int), ("obstacle", C.c_int),
+                ("mean", C.c_double), ("stddev", C.c_double), ("threshold", C.c_double)]
+
+
 PROF_CLASSES = ["bin", "fold_long", "unused", "fold", "clear_floor", "features", "raytrace", "other", "route"]
 
 # every symbol include/gem_b200.h declares: name -> (restype, argtypes)
@@ -119,6 +124,8 @@ SYMBOLS = {
     "gem_local_map_take": (C.c_int, [_P, _P, C.c_int, C.POINTER(C.c_int)]),
     "gem_local_map_clear": (C.c_int, [_P]),
     "gem_local_map_reserve": (C.c_int, [_P, C.c_int]),
+    "gem_grid_cloud_split": (C.c_int, [_P, C.c_int, C.c_int, C.c_double, C.c_double, _P, C.c_int, _P, C.c_int, _P, C.c_int,
+                                       C.POINTER(GemGridSplit)]),
     "gem_get_layer_device": (C.c_int, [_P, C.c_int, _P]),
     "gem_compute_features_tiled": (C.c_int, [_P, _P]),
     "gem_raytracing_tiled": (C.c_int, [_P, _P]),

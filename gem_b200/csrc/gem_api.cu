@@ -24,6 +24,7 @@
 #include "../../include/gem_b200.h"
 #include "gem_add.cuh"
 #include "gem_kernels.cuh"
+#include "gem_global.cuh"
 #include "gem_route.cuh"
 #include "gem_submap.cuh"
 
@@ -120,6 +121,10 @@ struct gem_map {
     bool prev_valid = false;
     LocalStore local;
     int *d_viscnt = nullptr;       // visual-cloud export: per (column, row chunk) counts / offsets
+    // gem_grid_cloud_split: geographic z, row x, column y, per-cell distance, compacted distances, queue, counters, stats
+    float *split_zg = nullptr, *split_xg = nullptr, *split_yg = nullptr, *split_dcell = nullptr, *split_dist = nullptr;
+    int *split_queue = nullptr, *split_ctr = nullptr;
+    SplitStats *split_stats = nullptr;
     unsigned long long *d_stamps = nullptr; // gem_debug_stamps
     int *d_raylist = nullptr;      // ray clean-up: cells that cast a ray + their count
     uint32_t *d_bitmap = nullptr;  // ray clean-up: validity bitmap of the lowest layer (own tile / map-wide)
@@ -669,8 +674,9 @@ static GridMapFrame grid_frame(const gem_map *m, float cx, float cy, int sx, int
     return f;
 }
 
-// count -> scan -> write of the cells Src takes, in GridMapIterator order; returns the total through *total_out
-template <class Src> static int compact_cells(gem_map *m, const Src &src, int capacity, int *total_out)
+// count -> scan -> write of the cells Src takes, in GridMapIterator order, issued on the handle's stream; the total is
+// left in device memory (*d_total_out: the compaction scratch, valid until the next compaction)
+template <class Src> static int compact_cells_issue(gem_map *m, const Src &src, int capacity, int **d_total_out)
 {
     const int L = m->L, nch = (L + 31) / 32;
     int rc;
@@ -682,6 +688,15 @@ template <class Src> static int compact_cells(gem_map *m, const Src &src, int ca
     GEM_LAUNCH(m, GEM_PROF_OTHER, k_compact_scan<<<nseg, SCAN_SEG, 0, m->stream>>>(m->d_viscnt, n, d_segtot));
     GEM_LAUNCH(m, GEM_PROF_OTHER, k_compact_write<Src><<<grid, 1024, 0, m->stream>>>(src, L, nch, m->d_viscnt, d_segtot, nseg, d_total, capacity));
     GEM_CUDA(m, cudaGetLastError());
+    *d_total_out = d_total;
+    return GEM_OK;
+}
+// the same, host-synchronous; returns the total through *total_out
+template <class Src> static int compact_cells(gem_map *m, const Src &src, int capacity, int *total_out)
+{
+    int *d_total = nullptr;
+    const int rc = compact_cells_issue(m, src, capacity, &d_total);
+    if (rc) return rc;
     GEM_CUDA(m, cudaMemcpyAsync(total_out, d_total, sizeof(int), cudaMemcpyDeviceToHost, m->stream));
     GEM_CUDA(m, cudaStreamSynchronize(m->stream));
     return GEM_OK;
@@ -1581,6 +1596,88 @@ int gem_export_grid_cloud(gem_map *m, int source, void *points32_device, int cap
     int total = 0;
     if ((rc = compact_cells(m, src, (int)std::min<size_t>((size_t)capacity, m->nc), &total))) return rc;
     *count_out = total; // the number of cells taken; min(total, capacity) records are written
+    return GEM_OK;
+}
+
+// composingGlobalMap's numeric block (ElevationMapping.cpp:1152-1170): statistical outlier removal over the grid cloud,
+// then the road / obstacle split of the survivors (gem_global.cuh, DESIGN.md f6)
+int gem_grid_cloud_split(gem_map *m, int source, int mean_k, double stddev_mul, double travers_threshold,
+                         void *road_points32_device, int road_capacity, void *obstacle_points32_device, int obstacle_capacity,
+                         float *mean_distance_device, int distance_capacity, gem_grid_split *out)
+{
+    if (!m || !out || (source != GEM_GRID_SHOWN && source != GEM_GRID_SNAPSHOT) || road_capacity < 0 || obstacle_capacity < 0 ||
+        distance_capacity < 0 || (road_capacity > 0 && !road_points32_device) || (obstacle_capacity > 0 && !obstacle_points32_device) ||
+        (distance_capacity > 0 && !mean_distance_device))
+        return fail(m, GEM_ERR_INVALID, "gem_grid_cloud_split: bad argument");
+    if (mean_k < 1 || mean_k > SPLIT_MAX_K) return fail(m, GEM_ERR_INVALID, "gem_grid_cloud_split: mean_k must be in [1, 64]");
+    if (m->geom.tiled) return fail(m, GEM_ERR_INVALID, "gem_grid_cloud_split: not available on tiled handles");
+    Lock lk(m->mu);
+    SetDev sd(m->dev);
+    if (source == GEM_GRID_SNAPSHOT && !m->prev_valid)
+        return fail(m, GEM_ERR_INVALID, "gem_grid_cloud_split: no snapshot (call gem_snapshot_shown first)");
+    int rc = flush_for_observer(m);
+    if (rc) return rc;
+    const int L = m->L;
+    if (!m->split_stats) { // the scratch is published only once every buffer exists (a failed call leaves it unset)
+        float *zg, *xg, *yg, *dcell, *dist;
+        int *queue, *ctr;
+        SplitStats *st;
+        if ((rc = dev_alloc(m, &zg, m->nc)) || (rc = dev_alloc(m, &xg, (size_t)L)) || (rc = dev_alloc(m, &yg, (size_t)L)) ||
+            (rc = dev_alloc(m, &dcell, m->nc)) || (rc = dev_alloc(m, &dist, m->nc)) || (rc = dev_alloc(m, &queue, m->nc)) ||
+            (rc = dev_alloc(m, &ctr, 2)) || (rc = dev_alloc(m, &st, 1)))
+            return rc;
+        m->split_zg = zg; m->split_xg = xg; m->split_yg = yg; m->split_dcell = dcell; m->split_dist = dist;
+        m->split_queue = queue; m->split_ctr = ctr; m->split_stats = st;
+    }
+    GridCloudSrc g;
+    const MapGeom &geo = source == GEM_GRID_SHOWN ? m->geom : m->prev_geom;
+    g.s = source == GEM_GRID_SHOWN ? live_cells(m->ml) : snapshot_cells(m->prev_ev, m->prev_ci, m->prev_tr);
+    g.f = grid_frame(m, geo.cx, geo.cy, geo.sx, geo.sy);
+    g.out = nullptr;
+    GEM_CUDA(m, cudaMemsetAsync(m->split_ctr, 0, 2 * sizeof(int), m->stream));
+    GEM_LAUNCH(m, GEM_PROF_OTHER, k_split_stage<<<blocks_for(m->nc, 256), 256, 0, m->stream>>>(g, m->split_zg, m->split_xg, m->split_yg, m->split_dcell));
+    const int nt = (L + SPLIT_TILE - 1) / SPLIT_TILE;
+    const dim3 grid(nt, nt);
+    const int K = mean_k + 1;
+    // the queue's length stays on the device: k_split_knn_far's fixed grid strides over it
+#define GEM_SPLIT_KNN(KC)                                                                                                              \
+    do {                                                                                                                               \
+        GEM_LAUNCH(m, GEM_PROF_OTHER, k_split_knn<KC><<<grid, SPLIT_TILE * SPLIT_TILE, 0, m->stream>>>(m->split_zg, m->split_xg, m->split_yg, L, geo.sx, geo.sy, mean_k, m->split_dcell, m->split_queue, m->split_ctr)); \
+        GEM_LAUNCH(m, GEM_PROF_OTHER, k_split_knn_far<KC><<<NUM_SMS * 4, 128, 0, m->stream>>>(m->split_zg, m->split_xg, m->split_yg, L, geo.sx, geo.sy, mean_k, m->split_dcell, m->split_queue, m->split_ctr)); \
+    } while (0)
+    if (K <= 8) GEM_SPLIT_KNN(8);
+    else if (K <= 24) GEM_SPLIT_KNN(24);
+    else GEM_SPLIT_KNN(SPLIT_MAX_K + 1);
+#undef GEM_SPLIT_KNN
+    GEM_CUDA(m, cudaGetLastError());
+    // distances in cloud order -> statistics -> road -> obstacle, all on the stream; the three counts are copied beside
+    // the statistics on the device, and the call waits once, for the one small read-back
+    SplitStats *dst = m->split_stats;
+    int *d_total = nullptr;
+    SplitDistSrc ds{g, m->split_dcell, m->split_dist, mean_distance_device, distance_capacity};
+    if ((rc = compact_cells_issue(m, ds, (int)m->nc, &d_total))) return rc;
+    GEM_CUDA(m, cudaMemcpyAsync(&dst->points, d_total, sizeof(int), cudaMemcpyDeviceToDevice, m->stream));
+    GEM_LAUNCH(m, GEM_PROF_OTHER, k_split_stats<<<1, 32, 0, m->stream>>>(m->split_dist, &dst->points, m->split_ctr, mean_k, stddev_mul, dst,
+                                                                         mean_distance_device, distance_capacity));
+    GEM_CUDA(m, cudaGetLastError());
+    SplitSrc rs{g, m->split_dcell, dst, travers_threshold, 1};
+    rs.g.out = reinterpret_cast<float4 *>(road_points32_device);
+    if ((rc = compact_cells_issue(m, rs, (int)std::min<size_t>((size_t)road_capacity, m->nc), &d_total))) return rc;
+    GEM_CUDA(m, cudaMemcpyAsync(&dst->road, d_total, sizeof(int), cudaMemcpyDeviceToDevice, m->stream));
+    SplitSrc os{g, m->split_dcell, dst, travers_threshold, 0};
+    os.g.out = reinterpret_cast<float4 *>(obstacle_points32_device);
+    if ((rc = compact_cells_issue(m, os, (int)std::min<size_t>((size_t)obstacle_capacity, m->nc), &d_total))) return rc;
+    GEM_CUDA(m, cudaMemcpyAsync(&dst->obstacle, d_total, sizeof(int), cudaMemcpyDeviceToDevice, m->stream));
+    SplitStats st;
+    GEM_CUDA(m, cudaMemcpyAsync(&st, dst, sizeof st, cudaMemcpyDeviceToHost, m->stream));
+    GEM_CUDA(m, cudaStreamSynchronize(m->stream));
+    out->points = st.points;
+    out->valid = st.valid;
+    out->road = st.road;
+    out->obstacle = st.obstacle;
+    out->mean = st.mean;
+    out->stddev = st.stddev;
+    out->threshold = st.threshold;
     return GEM_OK;
 }
 

@@ -459,6 +459,28 @@ class ElevationMap:
               "gem_export_grid_cloud")
         return rec
 
+    def grid_cloud_split(self, source: str = "snapshot", mean_k: int = 20, stddev_mul: float = 1.0,
+                         travers_threshold: float = 0.0, distances: bool = False):
+        """composingGlobalMap's filter (ElevationMapping.cpp:1152-1170): PCL's statistical outlier removal over
+        export_grid_cloud(source), then the survivors split by travers > travers_threshold.  Returns (road, obstacle,
+        stats) with road / obstacle (n, 8) float32 CUDA tensors of PointXYZRGBICT records in grid-cloud order and stats a
+        dict {points, valid, road, obstacle, mean, stddev, threshold}; with distances=True also the per-point mean
+        distances (float32 CUDA tensor, grid-cloud order) as a fourth item"""
+        import torch
+        # one filter pass: every output is sized for the whole grid cloud (the cheap count of export_grid_cloud), which
+        # road and obstacle together never exceed
+        n = self.grid_cloud_count(source)
+        road = self._records_out(n, None, "grid_cloud_split")
+        obstacle = self._records_out(n, None, "grid_cloud_split")
+        dist = torch.empty(n if distances else 0, dtype=torch.float32, device=road.device)
+        st = _lib.GemGridSplit()
+        check(self._lib.gem_grid_cloud_split(self._h, _lib.GRID_SOURCES[source], int(mean_k), float(stddev_mul),
+                                             float(travers_threshold), _ptr(road), n, _ptr(obstacle), n, _ptr(dist), dist.shape[0],
+                                             C.byref(st)), self._h, "gem_grid_cloud_split")
+        stats = {k: getattr(st, k) for k, _ in _lib.GemGridSplit._fields_}
+        road, obstacle = road[:st.road], obstacle[:st.obstacle]
+        return (road, obstacle, stats, dist[:st.points]) if distances else (road, obstacle, stats)
+
     def harvest_to_local_map(self, current_xy, shift_xy, records: bool = False):
         """the harvest of harvest_scrolled_out, upserted into the device-resident localMap_ (ElevationMapping.cpp:740-747).
         Returns the number of harvested records, or (records (n, 8) float32 host array, n) with records=True"""

@@ -283,6 +283,29 @@ int gem_local_map_take(gem_map *m, void *points32_device, int capacity, int *cou
 int gem_local_map_clear(gem_map *m);
 int gem_local_map_reserve(gem_map *m, int records);
 
+/* ---- the global-map filter of composingGlobalMap (ElevationMapping.cpp:482-514, :1146-1174; DESIGN.md f6) ----
+ * gem_grid_cloud_split: PCL's StatisticalOutlierRemoval (setMeanK(mean_k), setStddevMulThresh(stddev_mul); :1152-1156)
+ *   over the grid cloud gem_export_grid_cloud(source) defines (same points, records and order), then the survivors
+ *   split by (double)travers > travers_threshold into the road cloud and the rest into the obstacle cloud (:1161-1170).
+ *   Unpinned: restated from PCL 1.8 applyFilterIndices with an exact FLANN search.  Per point with finite x, y, z the
+ *   mean distance to its mean_k nearest other points (float d2 in FLANN's order, double sqrt and sum); 0 otherwise.
+ *   mean / stddev / threshold and the removal test (distance > threshold) are PCL's, the sums sequential in point order.
+ *   With at most mean_k finite points every point is kept, the distances and statistics are NaN and valid = 0.
+ *   road / obstacle receive min(count, capacity) 32-byte PointXYZRGBICT records each, in grid-cloud order; the counts
+ *   are reported in *out.  mean_distance_device (may be NULL with distance_capacity 0) receives min(points, capacity)
+ *   per-point distances in grid-cloud order.  mean_k in [1, 64].  Host-synchronous; the map is not modified.  Tiled
+ *   handles and a missing snapshot are errors.  The octomap insertion stays with the caller. */
+typedef struct gem_grid_split {
+    int points, valid;            /* grid-cloud points; points with a computed mean distance */
+    int road, obstacle;           /* records each output needs (min(count, capacity) are written) */
+    double mean, stddev, threshold;
+} gem_grid_split;
+int gem_grid_cloud_split(gem_map *m, int source, int mean_k, double stddev_mul, double travers_threshold,
+                         void *road_points32_device, int road_capacity,
+                         void *obstacle_points32_device, int obstacle_capacity,
+                         float *mean_distance_device, int distance_capacity,
+                         gem_grid_split *out);
+
 /* raw layer access (row-major L*L, float or int32 for the colour ids) for tests and
  * checkpoint/restore (the dead G_get_mapinfo/G_set_mapinfo of gpu.cu:457-475). */
 int gem_get_layer(gem_map *m, int layer, void *host_out);

@@ -224,6 +224,20 @@ class ElevationMap {
         check(gem_export_grid_cloud(h_, source, points32_device, (int)capacity, &n), "gem_export_grid_cloud");
         return n;
     }
+    // The filter of composingGlobalMap (ElevationMapping.cpp:1152-1170): statistical outlier removal over gridCloud(source)
+    // and the split of the survivors into road (travers > traversThreshold) and obstacle records, written into device
+    // memory (min(count, capacity) each; capacity 0 = size query).  meanDistance (may be null) receives the per-point mean
+    // distances in grid-cloud order.  Returns the counts and statistics; the octomap insertion stays with the caller.
+    gem_grid_split gridCloudSplit(int source, int meanK, double stddevMul, double traversThreshold, void *road_device,
+                                  size_t roadCapacity, void *obstacle_device, size_t obstacleCapacity,
+                                  float *meanDistance_device = nullptr, size_t distanceCapacity = 0)
+    {
+        gem_grid_split s{};
+        check(gem_grid_cloud_split(h_, source, meanK, stddevMul, traversThreshold, road_device, (int)roadCapacity, obstacle_device,
+                                   (int)obstacleCapacity, meanDistance_device, (int)distanceCapacity, &s),
+              "gem_grid_cloud_split");
+        return s;
+    }
     int harvestToLocalMap(const float current[2], const float shift[2], std::vector<PointXYZRGBICT> *visual = nullptr)
     {
         int n = 0;
