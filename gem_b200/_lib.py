@@ -70,6 +70,10 @@ class GemGridSplit(C.Structure):
                 ("mean", C.c_double), ("stddev", C.c_double), ("threshold", C.c_double)]
 
 
+class GemOctree(C.Structure):
+    _fields_ = [("bytes", C.c_longlong), ("nodes", C.c_int), ("leaves", C.c_int), ("inserted", C.c_int), ("skipped", C.c_int)]
+
+
 PROF_CLASSES = ["bin", "fold_long", "unused", "fold", "clear_floor", "features", "raytrace", "other", "route"]
 
 # every symbol include/gem_b200.h declares: name -> (restype, argtypes)
@@ -126,6 +130,8 @@ SYMBOLS = {
     "gem_local_map_reserve": (C.c_int, [_P, C.c_int]),
     "gem_grid_cloud_split": (C.c_int, [_P, C.c_int, C.c_int, C.c_double, C.c_double, _P, C.c_int, _P, C.c_int, _P, C.c_int,
                                        C.POINTER(GemGridSplit)]),
+    "gem_color_octree": (C.c_int, [_P, _P, C.c_int, C.c_double, C.POINTER(GemOctree)]),
+    "gem_color_octree_read": (C.c_int, [_P, _P, C.c_longlong]),
     "gem_get_layer_device": (C.c_int, [_P, C.c_int, _P]),
     "gem_compute_features_tiled": (C.c_int, [_P, _P]),
     "gem_raytracing_tiled": (C.c_int, [_P, _P]),

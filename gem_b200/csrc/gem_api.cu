@@ -25,6 +25,7 @@
 #include "gem_add.cuh"
 #include "gem_kernels.cuh"
 #include "gem_global.cuh"
+#include "gem_octree.cuh"
 #include "gem_route.cuh"
 #include "gem_submap.cuh"
 
@@ -57,6 +58,17 @@ struct TiledState { // gem_tiled_attach
     cudaGraph_t graph = nullptr;
     cudaGraphExec_t exec = nullptr;
     cudaGraphNode_t long_node = nullptr, fold_node = nullptr, route_node = nullptr, bin_node = nullptr;
+};
+
+struct OctBuf { // a device scratch buffer of gem_color_octree: grows on demand, never shrinks
+    void *p = nullptr;
+    size_t cap = 0;
+    template <typename T> T *as() const { return static_cast<T *>(p); }
+};
+struct OctScratch { // gem_color_octree (gem_octree.cuh); every buffer is consistent with its own capacity at all times
+    OctBuf code[2], idx[2], leaf, cnt, off, level, ghead, gid, val, groups, ctr, temp, key2[2], nkey[2], nrec[2], dense;
+    long long bytes = -1; // size of the last stream (in nrec[1]); -1: none
+    gem_octree info{};
 };
 
 struct LocalStore { // localMap_ on the device (gem_harvest_to_local_map, gem_local_map_take / _clear; gem_submap.cuh)
@@ -125,6 +137,7 @@ struct gem_map {
     float *split_zg = nullptr, *split_xg = nullptr, *split_yg = nullptr, *split_dcell = nullptr, *split_dist = nullptr;
     int *split_queue = nullptr, *split_ctr = nullptr;
     SplitStats *split_stats = nullptr;
+    OctScratch oct;                // gem_color_octree: scratch and the last stream
     unsigned long long *d_stamps = nullptr; // gem_debug_stamps
     int *d_raylist = nullptr;      // ray clean-up: cells that cast a ray + their count
     uint32_t *d_bitmap = nullptr;  // ray clean-up: validity bitmap of the lowest layer (own tile / map-wide)
@@ -848,6 +861,11 @@ int gem_destroy(gem_map *m)
         for (cudaEvent_t e : m->free_events) cudaEventDestroy(e);
         for (void *p : m->allocs) cudaFree(p);
         if (m->local.buf) cudaFree(m->local.buf);
+        for (OctBuf *b : {&m->oct.code[0], &m->oct.code[1], &m->oct.idx[0], &m->oct.idx[1], &m->oct.leaf, &m->oct.cnt, &m->oct.off,
+                          &m->oct.level, &m->oct.ghead, &m->oct.gid, &m->oct.val, &m->oct.groups, &m->oct.ctr, &m->oct.temp,
+                          &m->oct.key2[0], &m->oct.key2[1], &m->oct.nkey[0], &m->oct.nkey[1], &m->oct.nrec[0], &m->oct.nrec[1],
+                          &m->oct.dense})
+            if (b->p) cudaFree(b->p);
         if (m->h_ctr) cudaFreeHost(m->h_ctr);
         if (m->h_ctr_ring) cudaFreeHost(m->h_ctr_ring);
         if (m->h_frames) cudaFreeHost(m->h_frames);
@@ -1678,6 +1696,154 @@ int gem_grid_cloud_split(gem_map *m, int source, int mean_k, double stddev_mul, 
     out->mean = st.mean;
     out->stddev = st.stddev;
     out->threshold = st.threshold;
+    return GEM_OK;
+}
+
+// Grow one gem_color_octree scratch buffer to at least `bytes`.  The new buffer is allocated before the old one is
+// released, so a failed growth leaves the buffer as it was.
+static int oct_grow(gem_map *m, OctBuf &b, size_t bytes)
+{
+    if (b.cap >= bytes) return GEM_OK;
+    bytes = std::max(bytes + bytes / 4, (size_t)4096);
+    void *q = nullptr;
+    const cudaError_t e = cudaMalloc(&q, bytes);
+    if (e != cudaSuccess) return fail(m, GEM_ERR_NOMEM, std::string("gem_color_octree: cudaMalloc: ") + cudaGetErrorString(e));
+    if (b.p) cudaFree(b.p);
+    b.p = q;
+    b.cap = bytes;
+    return GEM_OK;
+}
+
+// pointCloudtoOctomap's tree (ElevationMapping.cpp:1157-1174) as the ColorOcTree::writeData stream (gem_octree.cuh,
+// DESIGN.md f7)
+int gem_color_octree(gem_map *m, const void *points32_device, int n, double resolution, gem_octree *info)
+{
+    if (!m || !info || n < 0 || (n > 0 && !points32_device)) return fail(m, GEM_ERR_INVALID, "gem_color_octree: bad argument");
+    if (!std::isfinite(resolution) || !(resolution > 0.0))
+        return fail(m, GEM_ERR_INVALID, "gem_color_octree: resolution must be finite and positive");
+    if (m->geom.tiled) return fail(m, GEM_ERR_INVALID, "gem_color_octree: not available on tiled handles");
+    Lock lk(m->mu);
+    SetDev sd(m->dev);
+    OctScratch &S = m->oct;
+    S.bytes = -1; // the buffers of the last stream are overwritten from here on
+    gem_octree r{};
+    if (n == 0) {
+        S.bytes = 0;
+        S.info = r;
+        *info = r;
+        return GEM_OK;
+    }
+    // O2: the constants and the value states, with the host's libm as octomap computes them
+    OctParams P{};
+    {
+        const float hit = (float)std::log(0.7 / 0.3), vmax = (float)std::log(0.971 / 0.029);
+        float v = 0.0f;
+        int s = 0;
+        while (!(v >= vmax) && s + 1 < OCT_STATES) {
+            v = v + hit;
+            if (v > vmax) v = vmax;
+            P.v[++s] = v;
+            P.p[s] = 1.0 - 1.0 / (1.0 + std::exp((double)v));
+            P.q[s] = 0.99 - P.p[s];
+        }
+        P.sat = s;
+    }
+    const double rf = 1.0 / resolution;
+    const size_t N = (size_t)n;
+    using u64 = unsigned long long;
+    cudaStream_t st = m->stream;
+    int rc;
+    // phase 1: keys, the sort by code, the leaves and their runs, the classification (sizes of phase 2)
+    size_t t_sort = 0, t_rle = 0, t_scan = 0;
+    GEM_CUDA(m, cub::DeviceRadixSort::SortPairs(nullptr, t_sort, (u64 *)nullptr, (u64 *)nullptr, (int *)nullptr, (int *)nullptr, n, 0, 49, st));
+    GEM_CUDA(m, cub::DeviceRunLengthEncode::Encode(nullptr, t_rle, (u64 *)nullptr, (u64 *)nullptr, (int *)nullptr, (int *)nullptr, n, st));
+    GEM_CUDA(m, cub::DeviceScan::ExclusiveSum(nullptr, t_scan, (int *)nullptr, (int *)nullptr, n, st));
+    if ((rc = oct_grow(m, S.code[0], N * 8)) || (rc = oct_grow(m, S.code[1], N * 8)) || (rc = oct_grow(m, S.idx[0], N * 4)) ||
+        (rc = oct_grow(m, S.idx[1], N * 4)) || (rc = oct_grow(m, S.leaf, N * 8)) || (rc = oct_grow(m, S.cnt, N * 4)) ||
+        (rc = oct_grow(m, S.off, N * 4)) || (rc = oct_grow(m, S.level, N * 4)) || (rc = oct_grow(m, S.ghead, N * 4)) ||
+        (rc = oct_grow(m, S.gid, N * 4)) || (rc = oct_grow(m, S.val, N * 4)) ||
+        (rc = oct_grow(m, S.groups, (N / 8 + 1) * sizeof(OctGroup))) || (rc = oct_grow(m, S.ctr, sizeof(OctCounters))) ||
+        (rc = oct_grow(m, S.temp, std::max(t_sort, std::max(t_rle, t_scan)))))
+        return rc;
+    const float4 *pts = static_cast<const float4 *>(points32_device);
+    OctCounters *ctr = S.ctr.as<OctCounters>();
+    u64 *leaf = S.leaf.as<u64>();
+    int *cnt = S.cnt.as<int>(), *off = S.off.as<int>(), *level = S.level.as<int>(), *sidx = S.idx[1].as<int>();
+    uint32_t *val = S.val.as<uint32_t>();
+    size_t tcap = S.temp.cap;
+    GEM_CUDA(m, cudaMemsetAsync(ctr, 0, sizeof(OctCounters), st));
+    // the run-length encoding writes nruns <= n counts (a device-side number); the scan below runs over all n, so the
+    // rest must be defined
+    GEM_CUDA(m, cudaMemsetAsync(cnt, 0, N * sizeof(int), st));
+    GEM_LAUNCH(m, GEM_PROF_OTHER, k_oct_keys<<<blocks_for(N, 256, 1 << 30), 256, 0, st>>>(pts, n, rf, S.code[0].as<u64>(), S.idx[0].as<int>(), ctr));
+    GEM_CUDA(m, cudaGetLastError());
+    GEM_CUDA(m, cub::DeviceRadixSort::SortPairs(S.temp.p, tcap, S.code[0].as<u64>(), S.code[1].as<u64>(), S.idx[0].as<int>(), sidx, n, 0, 49, st));
+    GEM_CUDA(m, cub::DeviceRunLengthEncode::Encode(S.temp.p, tcap, S.code[1].as<u64>(), leaf, cnt, &ctr->nruns, n, st));
+    GEM_CUDA(m, cub::DeviceScan::ExclusiveSum(S.temp.p, tcap, cnt, off, n, st));
+    GEM_LAUNCH(m, GEM_PROF_OTHER, k_oct_classify<<<blocks_for(N, 256, 1 << 30), 256, 0, st>>>(leaf, cnt, off, sidx, pts, P, level, S.ghead.as<int>(), S.gid.as<int>(),
+                                                                                             S.groups.as<OctGroup>(), val, ctr, n));
+    GEM_CUDA(m, cudaGetLastError());
+    OctCounters hc;
+    GEM_CUDA(m, cudaMemcpyAsync(&hc, ctr, sizeof hc, cudaMemcpyDeviceToHost, st));
+    GEM_CUDA(m, cudaStreamSynchronize(st));
+    // phase 2: the groups, the nodes above them, the preorder sort
+    const int nleaf = hc.inserted > 0 ? hc.nruns - (hc.inserted < n) : 0;
+    const size_t ngp = (size_t)hc.grouped, nnode = (size_t)hc.upper + (size_t)hc.indep + (size_t)hc.dense;
+    if (nnode > (size_t)INT32_MAX) return fail(m, GEM_ERR_INVALID, "gem_color_octree: too many nodes");
+    if (nnode > 0) {
+        int gbits = 0;
+        while ((1ll << gbits) < (long long)hc.groups) gbits++;
+        size_t t_keys = 0, t_nodes = 0;
+        GEM_CUDA(m, cub::DeviceRadixSort::SortKeys(nullptr, t_keys, (u64 *)nullptr, (u64 *)nullptr, (int)ngp, 0, 32 + gbits, st));
+        GEM_CUDA(m, cub::DeviceRadixSort::SortPairs(nullptr, t_nodes, (u64 *)nullptr, (u64 *)nullptr, (u64 *)nullptr, (u64 *)nullptr, (int)nnode, 0, 53, st));
+        if ((rc = oct_grow(m, S.key2[0], ngp * 8)) || (rc = oct_grow(m, S.key2[1], ngp * 8)) || (rc = oct_grow(m, S.nkey[0], nnode * 8)) ||
+            (rc = oct_grow(m, S.nkey[1], nnode * 8)) || (rc = oct_grow(m, S.nrec[0], nnode * 8)) || (rc = oct_grow(m, S.nrec[1], nnode * 8)) ||
+            (rc = oct_grow(m, S.dense, (size_t)hc.dense * 4)) || (rc = oct_grow(m, S.temp, std::max(t_keys, t_nodes))))
+            return rc;
+        tcap = S.temp.cap;
+        u64 *nkey = S.nkey[0].as<u64>(), *nrec = S.nrec[0].as<u64>();
+        GEM_CUDA(m, cudaMemsetAsync(nkey, 0xFF, nnode * 8, st)); // OCT_EMPTY: unused group slots sort last
+        if (ngp) {
+            GEM_CUDA(m, cudaMemsetAsync(S.dense.p, 0, (size_t)hc.dense * 4, st));
+            GEM_LAUNCH(m, GEM_PROF_OTHER, k_oct_group_keys<<<blocks_for((size_t)nleaf, 256, 1 << 30), 256, 0, st>>>(leaf, nleaf, cnt, off, sidx, level, S.ghead.as<int>(),
+                                                                                                                    S.gid.as<int>(), S.key2[0].as<u64>(), ctr));
+            GEM_CUDA(m, cub::DeviceRadixSort::SortKeys(S.temp.p, tcap, S.key2[0].as<u64>(), S.key2[1].as<u64>(), (int)ngp, 0, 32 + gbits, st));
+            // every subtree up to level OCT_SMEM_LEVEL is simulated in shared memory sized for the largest such group
+            const int smem_words = (int)oct_dense_size(std::min(hc.max_level, OCT_SMEM_LEVEL));
+            const size_t smem = (size_t)smem_words * sizeof(uint32_t);
+            if (smem > 48 * 1024) GEM_CUDA(m, cudaFuncSetAttribute(k_oct_group_sim, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+            GEM_LAUNCH(m, GEM_PROF_OTHER, k_oct_group_sim<<<hc.groups, 32, smem, st>>>(S.groups.as<OctGroup>(), S.key2[1].as<u64>(), (int)ngp, leaf, pts, rf, P,
+                                                                                       S.dense.as<uint32_t>(), smem_words, nkey, nrec, (long long)hc.upper + hc.indep, val, ctr));
+        }
+        for (int k = 0; k <= 16; k++)
+            GEM_LAUNCH(m, GEM_PROF_OTHER, k_oct_upper<<<blocks_for((size_t)nleaf, 256, 1 << 30), 256, 0, st>>>(leaf, nleaf, level, k, P, val, nkey, nrec, ctr));
+        GEM_CUDA(m, cudaGetLastError());
+        GEM_CUDA(m, cub::DeviceRadixSort::SortPairs(S.temp.p, tcap, nkey, S.nkey[1].as<u64>(), nrec, S.nrec[1].as<u64>(), (int)nnode, 0, 53, st));
+        GEM_CUDA(m, cudaMemcpyAsync(&hc, ctr, sizeof hc, cudaMemcpyDeviceToHost, st));
+        GEM_CUDA(m, cudaStreamSynchronize(st));
+    }
+    r.nodes = hc.upper + hc.indep + hc.group_nodes;
+    r.leaves = hc.indep + hc.group_leaves;
+    r.bytes = 8ll * r.nodes;
+    r.inserted = hc.inserted;
+    r.skipped = n - hc.inserted;
+    S.bytes = r.bytes;
+    S.info = r;
+    *info = r;
+    return GEM_OK;
+}
+
+int gem_color_octree_read(gem_map *m, void *out, long long capacity)
+{
+    if (!m) return GEM_ERR_INVALID;
+    Lock lk(m->mu);
+    const long long bytes = m->oct.bytes;
+    if (bytes < 0) return fail(m, GEM_ERR_INVALID, "gem_color_octree_read: no octree has been built");
+    if (capacity < bytes || (bytes > 0 && !out)) return fail(m, GEM_ERR_INVALID, "gem_color_octree_read: capacity < bytes");
+    if (bytes == 0) return GEM_OK;
+    SetDev sd(m->dev);
+    GEM_CUDA(m, cudaMemcpyAsync(out, m->oct.nrec[1].p, (size_t)bytes, cudaMemcpyDefault, m->stream));
+    GEM_CUDA(m, cudaStreamSynchronize(m->stream));
     return GEM_OK;
 }
 

@@ -481,6 +481,35 @@ class ElevationMap:
         road, obstacle = road[:st.road], obstacle[:st.obstacle]
         return (road, obstacle, stats, dist[:st.points]) if distances else (road, obstacle, stats)
 
+    def color_octree(self, points, resolution: float):
+        """pointCloudtoOctomap's octomap::ColorOcTree (ElevationMapping.cpp:1157-1174) of `points`, a contiguous (n, 8)
+        float32 CUDA tensor of PointXYZRGBICT records, inserted in order at `resolution`.  Returns (stream, info): the
+        ColorOcTree::writeData bytes as a uint8 CUDA tensor (octomap_msgs::Octomap::data with id "ColorOcTree",
+        binary false) and a dict {bytes, nodes, leaves, inserted, skipped}"""
+        import torch
+        if not (_is_device(points) and points.dtype == torch.float32 and points.dim() == 2 and points.shape[1] == 8
+                and points.is_contiguous()):
+            raise ValueError("color_octree: points must be a contiguous (n, 8) float32 CUDA tensor")
+        dev = torch.device("cuda", self._device_index())
+        torch.cuda.current_stream(dev).synchronize()   # the library reads the points on its own stream
+        info = _lib.GemOctree()
+        n = points.shape[0]
+        check(self._lib.gem_color_octree(self._h, _ptr(points) if n else None, n, float(resolution), C.byref(info)), self._h,
+              "gem_color_octree")
+        out = torch.empty(info.bytes, dtype=torch.uint8, device=dev)
+        check(self._lib.gem_color_octree_read(self._h, _ptr(out), out.numel()), self._h, "gem_color_octree_read")
+        return out, {k: getattr(info, k) for k, _ in _lib.GemOctree._fields_}
+
+    def global_octrees(self, source: str = "snapshot", mean_k: int = 20, stddev_mul: float = 1.0,
+                       travers_threshold: float = 0.0, road_resolution: float = 0.2, obstacle_resolution: float = 0.1):
+        """the numeric work of composingGlobalMap (ElevationMapping.cpp:482-514, :1146-1174): grid_cloud_split, then the
+        road and obstacle ColorOcTrees of its device outputs (the node's 0.2 m and 0.1 m trees, :146-147).  Returns
+        (road stream, obstacle stream, split stats), the streams as color_octree returns them"""
+        road, obstacle, stats = self.grid_cloud_split(source, mean_k, stddev_mul, travers_threshold)
+        road_stream, _ = self.color_octree(road, road_resolution)
+        obstacle_stream, _ = self.color_octree(obstacle, obstacle_resolution)
+        return road_stream, obstacle_stream, stats
+
     def harvest_to_local_map(self, current_xy, shift_xy, records: bool = False):
         """the harvest of harvest_scrolled_out, upserted into the device-resident localMap_ (ElevationMapping.cpp:740-747).
         Returns the number of harvested records, or (records (n, 8) float32 host array, n) with records=True"""

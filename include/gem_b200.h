@@ -294,7 +294,8 @@ int gem_local_map_reserve(gem_map *m, int records);
  *   road / obstacle receive min(count, capacity) 32-byte PointXYZRGBICT records each, in grid-cloud order; the counts
  *   are reported in *out.  mean_distance_device (may be NULL with distance_capacity 0) receives min(points, capacity)
  *   per-point distances in grid-cloud order.  mean_k in [1, 64].  Host-synchronous; the map is not modified.  Tiled
- *   handles and a missing snapshot are errors.  The octomap insertion stays with the caller. */
+ *   handles and a missing snapshot are errors.  The two octrees are built from road and obstacle with
+ *   gem_color_octree. */
 typedef struct gem_grid_split {
     int points, valid;            /* grid-cloud points; points with a computed mean distance */
     int road, obstacle;           /* records each output needs (min(count, capacity) are written) */
@@ -305,6 +306,26 @@ int gem_grid_cloud_split(gem_map *m, int source, int mean_k, double stddev_mul, 
                          void *obstacle_points32_device, int obstacle_capacity,
                          float *mean_distance_device, int distance_capacity,
                          gem_grid_split *out);
+
+/* ---- the global-map octrees of composingGlobalMap (ElevationMapping.cpp:1146-1174; DESIGN.md f7) ----
+ * gem_color_octree: the octomap::ColorOcTree pointCloudtoOctomap builds at `resolution` from n 32-byte PointXYZRGBICT
+ *   records in device memory (updateNode(point, true) then integrateNodeColor(x, y, z, r, g, b) per point in cloud
+ *   order, r, g, b = bytes 2, 1, 0 of the bgra word; then updateInnerOccupancy), from an empty tree.  The result is the
+ *   byte stream ColorOcTree::writeData produces, i.e. octomap_msgs::Octomap::data as fullMapToMsg fills it (the caller
+ *   sets id "ColorOcTree", binary false and the resolution); 8 bytes per node, 0 for an empty tree.  Unpinned:
+ *   restated from octomap 1.9 with default parameters (items O1-O6 of DESIGN.md f7).  The stream stays in the
+ *   handle until the next build; *info receives its size and counts.  Host-synchronous; the map is not modified.
+ *   n < 0, NULL points with n > 0, a non-finite or non-positive resolution and tiled handles are errors, which leave
+ *   the last stream as it was.
+ * gem_color_octree_read: copies the last built stream to `out` (host or device memory).  An error, writing nothing,
+ *   before any build or when capacity < bytes. */
+typedef struct gem_octree {
+    long long bytes;              /* stream size: 8 * nodes */
+    int nodes, leaves;            /* leaves: childless nodes, pruned ones included */
+    int inserted, skipped;        /* points inserted / skipped because a key is out of range or non-finite */
+} gem_octree;
+int gem_color_octree(gem_map *m, const void *points32_device, int n, double resolution, gem_octree *info);
+int gem_color_octree_read(gem_map *m, void *out, long long capacity);
 
 /* raw layer access (row-major L*L, float or int32 for the colour ids) for tests and
  * checkpoint/restore (the dead G_get_mapinfo/G_set_mapinfo of gpu.cu:457-475). */

@@ -13,6 +13,7 @@
 #pragma once
 
 #include <cmath>
+#include <cstdint>
 #include <cstddef>
 #include <cstring>
 #include <limits>
@@ -91,6 +92,13 @@ struct Layers {
         const size_t n = (size_t)L * L;
         for (auto *v : {&elevation, &variance, &rough, &slope, &traver, &color_r, &color_g, &color_b, &intensity}) v->resize(n);
     }
+};
+
+// The outputs of ElevationMap::globalOctrees: the two ColorOcTree streams (octomap_msgs::Octomap::data) and the counts.
+struct GlobalOctrees {
+    std::vector<int8_t> road, obstacle;
+    gem_octree roadInfo, obstacleInfo;
+    gem_grid_split split;
 };
 
 class ElevationMap {
@@ -227,7 +235,8 @@ class ElevationMap {
     // The filter of composingGlobalMap (ElevationMapping.cpp:1152-1170): statistical outlier removal over gridCloud(source)
     // and the split of the survivors into road (travers > traversThreshold) and obstacle records, written into device
     // memory (min(count, capacity) each; capacity 0 = size query).  meanDistance (may be null) receives the per-point mean
-    // distances in grid-cloud order.  Returns the counts and statistics; the octomap insertion stays with the caller.
+    // distances in grid-cloud order.  Returns the counts and statistics; colorOctree builds the octrees of the two
+    // outputs, globalOctrees does both steps.
     gem_grid_split gridCloudSplit(int source, int meanK, double stddevMul, double traversThreshold, void *road_device,
                                   size_t roadCapacity, void *obstacle_device, size_t obstacleCapacity,
                                   float *meanDistance_device = nullptr, size_t distanceCapacity = 0)
@@ -237,6 +246,35 @@ class ElevationMap {
                                    (int)obstacleCapacity, meanDistance_device, (int)distanceCapacity, &s),
               "gem_grid_cloud_split");
         return s;
+    }
+    // pointCloudtoOctomap's octomap::ColorOcTree (ElevationMapping.cpp:1157-1174) of n PointXYZRGBICT records in device
+    // memory at `resolution`, as the ColorOcTree::writeData stream: the octomap_msgs::Octomap::data of fullMapToMsg (set
+    // id = "ColorOcTree", binary = false, resolution).  info (may be null) receives the counts.
+    std::vector<int8_t> colorOctree(const void *points32_device, size_t n, double resolution, gem_octree *info = nullptr)
+    {
+        if (n > (size_t)std::numeric_limits<int>::max()) throw std::runtime_error("colorOctree: more than INT_MAX points");
+        gem_octree o{};
+        check(gem_color_octree(h_, points32_device, (int)n, resolution, &o), "gem_color_octree");
+        std::vector<int8_t> data((size_t)o.bytes);
+        check(gem_color_octree_read(h_, data.data(), o.bytes), "gem_color_octree_read");
+        if (info) *info = o;
+        return data;
+    }
+    // composingGlobalMap's numeric work (ElevationMapping.cpp:482-514, :1146-1174): gridCloudSplit into the caller's
+    // device buffers (each must hold the whole split output, gridCloud(source) records always do), then the road and the
+    // obstacle trees of the node (0.2 m and 0.1 m, :146-147).
+    GlobalOctrees globalOctrees(void *road_device, size_t roadCapacity, void *obstacle_device, size_t obstacleCapacity,
+                                int source = GEM_GRID_SNAPSHOT, int meanK = 20, double stddevMul = 1.0,
+                                double traversThreshold = 0.0, double roadResolution = 0.2, double obstacleResolution = 0.1)
+    {
+        GlobalOctrees g{};
+        g.split = gridCloudSplit(source, meanK, stddevMul, traversThreshold, road_device, roadCapacity, obstacle_device,
+                                 obstacleCapacity);
+        if ((size_t)g.split.road > roadCapacity || (size_t)g.split.obstacle > obstacleCapacity)
+            throw std::runtime_error("globalOctrees: the road or obstacle buffer is smaller than the split output");
+        g.road = colorOctree(road_device, (size_t)g.split.road, roadResolution, &g.roadInfo);
+        g.obstacle = colorOctree(obstacle_device, (size_t)g.split.obstacle, obstacleResolution, &g.obstacleInfo);
+        return g;
     }
     int harvestToLocalMap(const float current[2], const float shift[2], std::vector<PointXYZRGBICT> *visual = nullptr)
     {
