@@ -74,6 +74,19 @@ class GemOctree(C.Structure):
     _fields_ = [("bytes", C.c_longlong), ("nodes", C.c_int), ("leaves", C.c_int), ("inserted", C.c_int), ("skipped", C.c_int)]
 
 
+class GemCostmapWindow(C.Structure):
+    _fields_ = [("origin_x", C.c_double), ("origin_y", C.c_double), ("resolution", C.c_double), ("size_x", C.c_int),
+                ("size_y", C.c_int)]
+
+
+class GemCostmapMarks(C.Structure):
+    _fields_ = [("marked", C.c_longlong), ("lethal", C.c_longlong), ("min_x", C.c_double), ("min_y", C.c_double),
+                ("max_x", C.c_double), ("max_y", C.c_double)]
+
+
+COST_FREE, COST_LETHAL, COST_UNKNOWN = 0, 254, 255           # GEM_COST_*
+COSTMAP_MODES = {"max": 0, "overwrite": 1}                  # GEM_COSTMAP_MAX / GEM_COSTMAP_OVERWRITE
+
 PROF_CLASSES = ["bin", "fold_long", "unused", "fold", "clear_floor", "features", "raytrace", "other", "route"]
 
 # every symbol include/gem_b200.h declares: name -> (restype, argtypes)
@@ -132,6 +145,12 @@ SYMBOLS = {
                                        C.POINTER(GemGridSplit)]),
     "gem_color_octree": (C.c_int, [_P, _P, C.c_int, C.c_double, C.POINTER(GemOctree)]),
     "gem_color_octree_read": (C.c_int, [_P, _P, C.c_longlong]),
+    "gem_costmap_mark_map": (C.c_int, [_P, C.c_int, C.POINTER(GemCostmapWindow), C.c_double, C.c_int, _P,
+                                       C.POINTER(GemCostmapMarks)]),
+    "gem_costmap_mark_points": (C.c_int, [_P, _P, C.c_int, C.POINTER(GemCostmapWindow), C.c_double, _P,
+                                          C.POINTER(GemCostmapMarks)]),
+    "gem_costmap_update_origin": (C.c_int, [_P, C.POINTER(GemCostmapWindow), C.c_double, C.c_double, C.c_ubyte, _P]),
+    "gem_costmap_combine": (C.c_int, [_P, C.c_int, _P, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int]),
     "gem_get_layer_device": (C.c_int, [_P, C.c_int, _P]),
     "gem_compute_features_tiled": (C.c_int, [_P, _P]),
     "gem_raytracing_tiled": (C.c_int, [_P, _P]),

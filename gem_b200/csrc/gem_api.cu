@@ -23,6 +23,7 @@
 
 #include "../../include/gem_b200.h"
 #include "gem_add.cuh"
+#include "gem_costmap.cuh"
 #include "gem_kernels.cuh"
 #include "gem_global.cuh"
 #include "gem_octree.cuh"
@@ -138,6 +139,8 @@ struct gem_map {
     int *split_queue = nullptr, *split_ctr = nullptr;
     SplitStats *split_stats = nullptr;
     OctScratch oct;                // gem_color_octree: scratch and the last stream
+    OctBuf cost_scratch;           // costmap calls: the winner per costmap cell (int), or the copy of a rolled grid
+    CostMarksDev *cost_acc = nullptr; // costmap mark calls: counts and encoded touch bounds
     unsigned long long *d_stamps = nullptr; // gem_debug_stamps
     int *d_raylist = nullptr;      // ray clean-up: cells that cast a ray + their count
     uint32_t *d_bitmap = nullptr;  // ray clean-up: validity bitmap of the lowest layer (own tile / map-wide)
@@ -864,7 +867,7 @@ int gem_destroy(gem_map *m)
         for (OctBuf *b : {&m->oct.code[0], &m->oct.code[1], &m->oct.idx[0], &m->oct.idx[1], &m->oct.leaf, &m->oct.cnt, &m->oct.off,
                           &m->oct.level, &m->oct.ghead, &m->oct.gid, &m->oct.val, &m->oct.groups, &m->oct.ctr, &m->oct.temp,
                           &m->oct.key2[0], &m->oct.key2[1], &m->oct.nkey[0], &m->oct.nkey[1], &m->oct.nrec[0], &m->oct.nrec[1],
-                          &m->oct.dense})
+                          &m->oct.dense, &m->cost_scratch})
             if (b->p) cudaFree(b->p);
         if (m->h_ctr) cudaFreeHost(m->h_ctr);
         if (m->h_ctr_ring) cudaFreeHost(m->h_ctr_ring);
@@ -1844,6 +1847,147 @@ int gem_color_octree_read(gem_map *m, void *out, long long capacity)
     SetDev sd(m->dev);
     GEM_CUDA(m, cudaMemcpyAsync(out, m->oct.nrec[1].p, (size_t)bytes, cudaMemcpyDefault, m->stream));
     GEM_CUDA(m, cudaStreamSynchronize(m->stream));
+    return GEM_OK;
+}
+
+// ---- navigation costmaps (gem_costmap.cuh, DESIGN.md f8) ---------------------------------------------------------
+// a window every costmap call accepts: sizes > 0 with fewer than 2^31 cells, a finite positive resolution
+static bool cost_sizes_ok(int sx, int sy) { return sx > 0 && sy > 0 && (long long)sx * sy < (1ll << 31); }
+static bool cost_window_ok(const gem_costmap_window *w)
+{
+    return w && cost_sizes_ok(w->size_x, w->size_y) && std::isfinite(w->resolution) && w->resolution > 0.0;
+}
+// Grow the costmap scratch to at least `bytes`.  The stream is drained before the old buffer goes (an update_origin may
+// still read it), and the new buffer is allocated first, so a failed growth leaves the scratch as it was.
+static int cost_grow(gem_map *m, size_t bytes)
+{
+    OctBuf &b = m->cost_scratch;
+    if (b.cap >= bytes) return GEM_OK;
+    void *q = nullptr;
+    const cudaError_t e = cudaMalloc(&q, bytes);
+    if (e != cudaSuccess) return fail(m, GEM_ERR_NOMEM, std::string("costmap scratch: cudaMalloc: ") + cudaGetErrorString(e));
+    if (b.p) {
+        cudaStreamSynchronize(m->stream);
+        cudaFree(b.p);
+    }
+    b.p = q;
+    b.cap = bytes;
+    return GEM_OK;
+}
+// the last-writer scatter of both mark calls (pass 1, pass 2), then the marks back to the host
+extern "C++" {
+template <class Src> static int cost_mark(gem_map *m, const Src &src, long long nchunks, const gem_costmap_window *w, unsigned char *cost,
+                                         gem_costmap_marks *out)
+{
+    const int ncells = w->size_x * w->size_y;
+    int rc;
+    if ((rc = cost_grow(m, (size_t)ncells * sizeof(int)))) return rc;
+    if (!m->cost_acc && (rc = dev_alloc(m, &m->cost_acc, 1))) return rc;
+    const CostWindow cw{w->origin_x, w->origin_y, w->resolution, w->size_x, w->size_y};
+    CostMarksDev init{0, 0, cm_key(INFINITY), cm_key(INFINITY), cm_key(-INFINITY), cm_key(-INFINITY)};
+    int *winner = m->cost_scratch.as<int>();
+    GEM_CUDA(m, cudaMemsetAsync(winner, 0xFF, (size_t)ncells * sizeof(int), m->stream)); // -1: no writer
+    GEM_CUDA(m, cudaMemcpyAsync(m->cost_acc, &init, sizeof init, cudaMemcpyHostToDevice, m->stream));
+    if (nchunks > 0) {
+        const int grid = (int)std::min<long long>((nchunks + COST_BLOCK / 32 - 1) / (COST_BLOCK / 32), NUM_SMS * 8);
+        GEM_LAUNCH(m, GEM_PROF_OTHER, k_costmap_scatter<Src><<<grid, COST_BLOCK, 0, m->stream>>>(src, nchunks, cw, winner, m->cost_acc));
+        GEM_LAUNCH(m, GEM_PROF_OTHER, k_costmap_store<Src><<<(unsigned)(((long long)ncells + COST_BLOCK - 1) / COST_BLOCK), COST_BLOCK, 0, m->stream>>>(src, winner, ncells, cost));
+        GEM_CUDA(m, cudaGetLastError());
+    }
+    CostMarksDev r;
+    GEM_CUDA(m, cudaMemcpyAsync(&r, m->cost_acc, sizeof r, cudaMemcpyDeviceToHost, m->stream));
+    GEM_CUDA(m, cudaStreamSynchronize(m->stream));
+    out->marked = (long long)r.marked;
+    out->lethal = (long long)r.lethal;
+    out->min_x = cm_unkey(r.minx); out->min_y = cm_unkey(r.miny);
+    out->max_x = cm_unkey(r.maxx); out->max_y = cm_unkey(r.maxy);
+    return GEM_OK;
+}
+} // extern "C++"
+
+int gem_costmap_mark_map(gem_map *m, int source, const gem_costmap_window *w, double travers_thresh, int mark_unknown,
+                         unsigned char *cost_device, gem_costmap_marks *out)
+{
+    if (!m || !cost_device || !out || (source != GEM_GRID_SHOWN && source != GEM_GRID_SNAPSHOT))
+        return fail(m, GEM_ERR_INVALID, "gem_costmap_mark_map: bad argument");
+    if (!cost_window_ok(w)) return fail(m, GEM_ERR_INVALID, "gem_costmap_mark_map: bad window");
+    if (m->geom.tiled) return fail(m, GEM_ERR_INVALID, "gem_costmap_mark_map: not available on tiled handles");
+    Lock lk(m->mu);
+    SetDev sd(m->dev);
+    if (source == GEM_GRID_SNAPSHOT && !m->prev_valid)
+        return fail(m, GEM_ERR_INVALID, "gem_costmap_mark_map: no snapshot (call gem_snapshot_shown first)");
+    int rc = flush_for_observer(m);
+    if (rc) return rc;
+    CostGridSrc src;
+    const MapGeom &g = source == GEM_GRID_SHOWN ? m->geom : m->prev_geom;
+    src.g.s = source == GEM_GRID_SHOWN ? live_cells(m->ml) : snapshot_cells(m->prev_ev, m->prev_ci, m->prev_tr);
+    src.g.f = grid_frame(m, g.cx, g.cy, g.sx, g.sy);
+    src.g.out = nullptr;
+    src.thresh = travers_thresh;
+    src.mark_unknown = mark_unknown ? 1 : 0;
+    src.nch = (m->L + 31) / 32;
+    return cost_mark(m, src, (long long)m->L * src.nch, w, cost_device, out);
+}
+
+int gem_costmap_mark_points(gem_map *m, const void *points32_device, int n, const gem_costmap_window *w, double travers_thresh,
+                            unsigned char *cost_device, gem_costmap_marks *out)
+{
+    if (!m || !cost_device || !out || n < 0 || (n > 0 && !points32_device))
+        return fail(m, GEM_ERR_INVALID, "gem_costmap_mark_points: bad argument");
+    if (!cost_window_ok(w)) return fail(m, GEM_ERR_INVALID, "gem_costmap_mark_points: bad window");
+    Lock lk(m->mu);
+    SetDev sd(m->dev);
+    CostPointSrc src{static_cast<const float4 *>(points32_device), n, travers_thresh};
+    return cost_mark(m, src, ((long long)n + 31) / 32, w, cost_device, out);
+}
+
+int gem_costmap_update_origin(gem_map *m, gem_costmap_window *w, double new_origin_x, double new_origin_y, unsigned char fill,
+                              unsigned char *cost_device)
+{
+    if (!m || !cost_device) return fail(m, GEM_ERR_INVALID, "gem_costmap_update_origin: bad argument");
+    if (!cost_window_ok(w)) return fail(m, GEM_ERR_INVALID, "gem_costmap_update_origin: bad window");
+    // Costmap2D::updateOrigin: cell_ox = (int)((new_ox - origin_x) / resolution), truncating toward zero.  DEFINED: a shift
+    // that is not finite or does not fit an int (where the cast is undefined) is an error.
+    const double qx = (new_origin_x - w->origin_x) / w->resolution, qy = (new_origin_y - w->origin_y) / w->resolution;
+    if (!(std::fabs(qx) < 2147483648.0) || !(std::fabs(qy) < 2147483648.0))
+        return fail(m, GEM_ERR_INVALID, "gem_costmap_update_origin: the shift in cells is not finite or does not fit an int");
+    const int cell_ox = (int)qx, cell_oy = (int)qy;
+    if (cell_ox == 0 && cell_oy == 0) return GEM_OK; // nothing to update: the origin stays
+    Lock lk(m->mu);
+    SetDev sd(m->dev);
+    const size_t ncells = (size_t)w->size_x * w->size_y;
+    int rc;
+    if ((rc = cost_grow(m, ncells))) return rc;
+    // the copy, then the gather of k_costmap_roll, both ordered on the stream
+    GEM_CUDA(m, cudaMemcpyAsync(m->cost_scratch.p, cost_device, ncells, cudaMemcpyDefault, m->stream));
+    // |cell_ox| >= size_x leaves nothing of the old grid: clamp, so that the kernel's index sums cannot overflow
+    const int cx = std::max(-w->size_x, std::min(w->size_x, cell_ox)), cy = std::max(-w->size_y, std::min(w->size_y, cell_oy));
+    GEM_LAUNCH(m, GEM_PROF_OTHER, k_costmap_roll<<<(unsigned)((ncells + COST_BLOCK - 1) / COST_BLOCK), COST_BLOCK, 0, m->stream>>>(
+                                      m->cost_scratch.as<unsigned char>(), cost_device, w->size_x, w->size_y, cx, cy, fill));
+    GEM_CUDA(m, cudaGetLastError());
+    // the new origin is grid-aligned: origin + cell_o * resolution (an int times a double, then the sum)
+    const double dx = (double)cell_ox * w->resolution, dy = (double)cell_oy * w->resolution;
+    w->origin_x = w->origin_x + dx;
+    w->origin_y = w->origin_y + dy;
+    return GEM_OK;
+}
+
+int gem_costmap_combine(gem_map *m, int mode, const unsigned char *layer_device, unsigned char *master_device, int size_x, int size_y,
+                        int min_i, int min_j, int max_i, int max_j)
+{
+    if (!m || !layer_device || !master_device || (mode != GEM_COSTMAP_MAX && mode != GEM_COSTMAP_OVERWRITE))
+        return fail(m, GEM_ERR_INVALID, "gem_costmap_combine: bad argument");
+    if (!cost_sizes_ok(size_x, size_y)) return fail(m, GEM_ERR_INVALID, "gem_costmap_combine: bad grid size");
+    const int i0 = std::max(min_i, 0), i1 = std::min(max_i, size_x), j0 = std::max(min_j, 0), j1 = std::min(max_j, size_y);
+    if (i0 >= i1 || j0 >= j1) return GEM_OK;
+    Lock lk(m->mu);
+    SetDev sd(m->dev);
+    const int vec = (((uintptr_t)layer_device - (uintptr_t)master_device) & 15u) == 0 ? 1 : 0;
+    const long long blocks_x = ((long long)(i1 - i0) / 16 + 2 + COST_BLOCK - 1) / COST_BLOCK;
+    const dim3 grid((unsigned)std::min<long long>(blocks_x, 1024), (unsigned)std::min(j1 - j0, 65535));
+    GEM_LAUNCH(m, GEM_PROF_OTHER, k_costmap_combine<<<grid, COST_BLOCK, 0, m->stream>>>(layer_device, master_device, size_x, i0, i1, j0, j1,
+                                                                                    mode, vec));
+    GEM_CUDA(m, cudaGetLastError());
     return GEM_OK;
 }
 

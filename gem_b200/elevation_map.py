@@ -510,6 +510,77 @@ class ElevationMap:
         obstacle_stream, _ = self.color_octree(obstacle, obstacle_resolution)
         return road_stream, obstacle_stream, stats
 
+    # -- navigation costmaps (GEM's layers/ package, DESIGN.md f8) -------------------------------------------------------
+    # A window is (origin_x, origin_y, resolution, size_x, size_y); a grid is a contiguous uint8 CUDA tensor of
+    # size_x * size_y cells, cell (mx, my) at my * size_x + mx.  The library works on its own stream: each call first waits
+    # for the current torch stream, and update_origin / combine leave their writes on the library's stream (torch_stream()).
+    @staticmethod
+    def _cost_window(window):
+        ox, oy, res, sx, sy = window
+        return _lib.GemCostmapWindow(float(ox), float(oy), float(res), int(sx), int(sy))
+
+    def _cost_grid(self, grid, size_x: int, size_y: int, what: str):
+        """the device address of a costmap grid after checking it against the size the call is given: the library only
+        sees a pointer, so a tensor smaller than size_x * size_y cells would be read and written past its end"""
+        import torch
+        if not (_is_device(grid) and grid.dtype == torch.uint8 and grid.is_contiguous()):
+            raise ValueError(f"{what}: the grid must be a contiguous uint8 CUDA tensor")
+        if grid.device.index != self._device_index():
+            raise ValueError(f"{what}: the grid is on {grid.device}, the map on cuda:{self._device_index()}")
+        if grid.numel() != int(size_x) * int(size_y):
+            raise ValueError(f"{what}: the grid holds {grid.numel()} cells, the window {int(size_x)} x {int(size_y)}")
+        torch.cuda.current_stream(grid.device).synchronize()
+        return _ptr(grid)
+
+    @staticmethod
+    def _cost_marks(mk) -> dict:
+        return {k: getattr(mk, k) for k, _ in _lib.GemCostmapMarks._fields_}
+
+    def costmap_mark_map(self, window, cost, travers_thresh: float = 0.7, source: str = "shown", mark_unknown: bool = True) -> dict:
+        """ElevationMapLayer::updateBounds over show()'s grid_map ("shown": the live map after compute_features, or
+        "snapshot") into the layer grid `cost`; returns the marks {marked, lethal, min_x, min_y, max_x, max_y}"""
+        w = self._cost_window(window)
+        p = self._cost_grid(cost, w.size_x, w.size_y, "costmap_mark_map")
+        mk = _lib.GemCostmapMarks()
+        check(self._lib.gem_costmap_mark_map(self._h, _lib.GRID_SOURCES[source], C.byref(w),
+                                             float(travers_thresh), 1 if mark_unknown else 0, p, C.byref(mk)), self._h,
+              "gem_costmap_mark_map")
+        return self._cost_marks(mk)
+
+    def costmap_mark_points(self, points, window, cost, travers_thresh: float = 0.7) -> dict:
+        """PointMapLayer::updateBounds over `points`, an (n, 8) float32 CUDA tensor of PointXYZRGBICT records, into the
+        layer grid `cost`; returns the marks as costmap_mark_map does"""
+        import torch
+        if not (_is_device(points) and points.dtype == torch.float32 and points.dim() == 2 and points.shape[1] == 8
+                and points.is_contiguous()):
+            raise ValueError("costmap_mark_points: points must be a contiguous (n, 8) float32 CUDA tensor")
+        if points.device.index != self._device_index():
+            raise ValueError(f"costmap_mark_points: the points are on {points.device}, the map on cuda:{self._device_index()}")
+        w = self._cost_window(window)
+        p = self._cost_grid(cost, w.size_x, w.size_y, "costmap_mark_points")
+        mk = _lib.GemCostmapMarks()
+        n = int(points.shape[0])
+        check(self._lib.gem_costmap_mark_points(self._h, _ptr(points) if n else None, n, C.byref(w),
+                                                float(travers_thresh), p, C.byref(mk)), self._h, "gem_costmap_mark_points")
+        return self._cost_marks(mk)
+
+    def costmap_update_origin(self, window, new_origin_x: float, new_origin_y: float, fill: int, cost):
+        """Costmap2D::updateOrigin of the grid `cost` in place; returns the new window (the grid-aligned origin)"""
+        w = self._cost_window(window)
+        check(self._lib.gem_costmap_update_origin(self._h, C.byref(w), float(new_origin_x), float(new_origin_y), int(fill),
+                                                  self._cost_grid(cost, w.size_x, w.size_y, "costmap_update_origin")), self._h,
+              "gem_costmap_update_origin")
+        return (w.origin_x, w.origin_y, w.resolution, w.size_x, w.size_y)
+
+    def costmap_combine(self, mode: str, layer, master, size_x: int, size_y: int, rect):
+        """updateWithMax (mode "max") or PointMapLayer's overwrite ("overwrite") of `layer` into `master` over
+        rect = (min_i, min_j, max_i, max_j), clamped to the grid"""
+        i0, j0, i1, j1 = (int(v) for v in rect)
+        pl = self._cost_grid(layer, size_x, size_y, "costmap_combine")
+        pm = self._cost_grid(master, size_x, size_y, "costmap_combine")
+        check(self._lib.gem_costmap_combine(self._h, _lib.COSTMAP_MODES[mode], pl, pm, int(size_x), int(size_y), i0, j0, i1, j1),
+              self._h, "gem_costmap_combine")
+
     def harvest_to_local_map(self, current_xy, shift_xy, records: bool = False):
         """the harvest of harvest_scrolled_out, upserted into the device-resident localMap_ (ElevationMapping.cpp:740-747).
         Returns the number of harvested records, or (records (n, 8) float32 host array, n) with records=True"""

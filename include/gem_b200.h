@@ -327,6 +327,62 @@ typedef struct gem_octree {
 int gem_color_octree(gem_map *m, const void *points32_device, int n, double resolution, gem_octree *info);
 int gem_color_octree_read(gem_map *m, void *out, long long capacity);
 
+/* ---- navigation costmaps: the costmap_2d layers of GEM's layers/ package (DESIGN.md f8) ----
+ * ElevationMapLayer (layers/src/elevationMap_layer.cpp:42-87) and PointMapLayer (layers/src/pointMap_layer.cpp:45-100), with
+ * the costmap_2d functions they use restated from navigation 1.14 (unpinned):
+ *   - costs: FREE_SPACE 0, LETHAL_OBSTACLE 254, NO_INFORMATION 255;
+ *   - a grid is caller-owned device memory uint8[size_y][size_x], cell (mx, my) at my * size_x + mx (getIndex);
+ *   - worldToMap(wx, wy), in double: false if wx < origin_x || wy < origin_y, else mx = (int)((wx - origin_x) / resolution)
+ *     (same for my), accepted iff mx < size_x && my < size_y.  DEFINED: a non-finite coordinate is rejected, and so is a
+ *     quotient >= 2^31;
+ *   - touch: min_x = min(min_x, wx) etc. over every element written, not only over the cells that keep its value.  A zero
+ *     bound is reported as +0.
+ * gem_costmap_mark_map: ElevationMapLayer::updateBounds (:56-84) over the grid_map show() publishes, source GEM_GRID_SHOWN
+ *   (the live map after gem_compute_features) or GEM_GRID_SNAPSHOT.  Per cell in GridMapIterator order (ix + iy * L): the
+ *   value is show()'s traver (the feature output where the cell is shown, NaN elsewhere), the position the grid_map cell
+ *   centre in double (grid_resolution), the cost LETHAL if (double)value < travers_thresh, else FREE.  mark_unknown = 1 is
+ *   the reference (NaN compares false: a cleared cell is FREE); mark_unknown = 0 writes nothing for cleared cells.  Tiled
+ *   handles and a missing snapshot are errors.
+ * gem_costmap_mark_points: PointMapLayer::updateBounds (:54-81) over n 32-byte PointXYZRGBICT records in device memory, in
+ *   order: (double)x, (double)y through worldToMap, cost FREE if (double)travers > travers_thresh, else LETHAL (NaN and
+ *   equality give LETHAL).  n = 0 is valid.
+ *   In both mark calls the LAST element in order wins a costmap cell several elements fall into; cells nothing writes
+ *   keep their value (the layer grid persists).  *out receives the elements written and the touch bounds (+inf / -inf
+ *   when none was).  Host-synchronous.  They use a handle-owned scratch of 4 bytes per costmap cell, grown on demand (a
+ *   failed growth is GEM_ERR_NOMEM and writes nothing).
+ * gem_costmap_update_origin: Costmap2D::updateOrigin in place: cell_ox = (int)((new_origin_x - origin_x) / resolution)
+ *   (truncating toward zero; same for y); nothing happens when both are 0; else new cell n holds old cell n + cell_ox (and
+ *   n + cell_oy) when that is inside the grid, else `fill`, and the origin becomes origin_x + cell_ox * resolution, written
+ *   to *w.  A rolling layer calls it with robot - getSizeInMetersX() / 2, getSizeInMetersX() = (size_x - 1 + 0.5) *
+ *   resolution.  fill is the layer's default_value_: FREE_SPACE for the elevation layer; NO_INFORMATION for the point
+ *   layer (DEFINED: the reference never sets it).  DEFINED: a shift that is not finite or does not fit an int is an error.
+ * gem_costmap_combine: over the rect [min_i, max_i) x [min_j, max_j), clamped to the grid (an empty rect does nothing),
+ *   GEM_COSTMAP_MAX = CostmapLayer::updateWithMax (a NO_INFORMATION layer cell is skipped; otherwise written when the
+ *   master is NO_INFORMATION or less than the layer), GEM_COSTMAP_OVERWRITE = PointMapLayer::updateCosts (:86-100; every
+ *   layer cell that is not NO_INFORMATION is copied).  layer and master are grids of size_x * size_y.
+ * update_origin and combine are asynchronous on the handle's stream and, like mark_points, work on any handle.  No call
+ * modifies the map.  Every call rejects a bad window (size <= 0, size_x * size_y >= 2^31, a resolution that is <= 0 or not
+ * finite); a rejected call writes nothing.  Out of scope: footprint clearing (footprint_clearing_enabled false),
+ * InflationLayer (inflation_radius 0 in GEM's configs), publishing, and the elevation_map_available_ subscription gate. */
+enum { GEM_COST_FREE = 0, GEM_COST_LETHAL = 254, GEM_COST_UNKNOWN = 255 };
+enum { GEM_COSTMAP_MAX = 0, GEM_COSTMAP_OVERWRITE = 1 };
+typedef struct gem_costmap_window {
+    double origin_x, origin_y, resolution;
+    int size_x, size_y;
+} gem_costmap_window;
+typedef struct gem_costmap_marks {
+    long long marked, lethal;          /* elements written (touch calls), of which LETHAL */
+    double min_x, min_y, max_x, max_y; /* touch bounds; +inf / -inf when marked == 0 */
+} gem_costmap_marks;
+int gem_costmap_mark_map(gem_map *m, int source, const gem_costmap_window *w, double travers_thresh, int mark_unknown,
+                         unsigned char *cost_device, gem_costmap_marks *out);
+int gem_costmap_mark_points(gem_map *m, const void *points32_device, int n, const gem_costmap_window *w, double travers_thresh,
+                            unsigned char *cost_device, gem_costmap_marks *out);
+int gem_costmap_update_origin(gem_map *m, gem_costmap_window *w, double new_origin_x, double new_origin_y, unsigned char fill,
+                              unsigned char *cost_device);
+int gem_costmap_combine(gem_map *m, int mode, const unsigned char *layer_device, unsigned char *master_device, int size_x, int size_y,
+                        int min_i, int min_j, int max_i, int max_j);
+
 /* raw layer access (row-major L*L, float or int32 for the colour ids) for tests and
  * checkpoint/restore (the dead G_get_mapinfo/G_set_mapinfo of gpu.cu:457-475). */
 int gem_get_layer(gem_map *m, int layer, void *host_out);

@@ -276,6 +276,33 @@ class ElevationMap {
         g.obstacle = colorOctree(obstacle_device, (size_t)g.split.obstacle, obstacleResolution, &g.obstacleInfo);
         return g;
     }
+    // The costmap_2d layers of GEM's layers/ package (DESIGN.md f8) on caller-owned device grids uint8[size_y][size_x]:
+    // ElevationMapLayer::updateBounds over show()'s grid_map, PointMapLayer::updateBounds over PointXYZRGBICT records,
+    // Costmap2D::updateOrigin (writes the grid-aligned origin back into w) and updateWithMax / PointMapLayer's overwrite.
+    gem_costmap_marks costmapMarkMap(const gem_costmap_window &w, unsigned char *cost_device, double traversThresh = 0.7,
+                                     int source = GEM_GRID_SHOWN, bool markUnknown = true)
+    {
+        gem_costmap_marks mk{};
+        check(gem_costmap_mark_map(h_, source, &w, traversThresh, markUnknown ? 1 : 0, cost_device, &mk), "gem_costmap_mark_map");
+        return mk;
+    }
+    gem_costmap_marks costmapMarkPoints(const void *points32_device, size_t n, const gem_costmap_window &w, unsigned char *cost_device,
+                                        double traversThresh = 0.7)
+    {
+        if (n > (size_t)std::numeric_limits<int>::max()) throw std::runtime_error("costmapMarkPoints: more than INT_MAX points");
+        gem_costmap_marks mk{};
+        check(gem_costmap_mark_points(h_, points32_device, (int)n, &w, traversThresh, cost_device, &mk), "gem_costmap_mark_points");
+        return mk;
+    }
+    void costmapUpdateOrigin(gem_costmap_window &w, double newOriginX, double newOriginY, unsigned char fill, unsigned char *cost_device)
+    {
+        check(gem_costmap_update_origin(h_, &w, newOriginX, newOriginY, fill, cost_device), "gem_costmap_update_origin");
+    }
+    void costmapCombine(int mode, const unsigned char *layer_device, unsigned char *master_device, int sizeX, int sizeY, int minI,
+                        int minJ, int maxI, int maxJ)
+    {
+        check(gem_costmap_combine(h_, mode, layer_device, master_device, sizeX, sizeY, minI, minJ, maxI, maxJ), "gem_costmap_combine");
+    }
     int harvestToLocalMap(const float current[2], const float shift[2], std::vector<PointXYZRGBICT> *visual = nullptr)
     {
         int n = 0;
