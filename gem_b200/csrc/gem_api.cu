@@ -1111,6 +1111,9 @@ int gem_add_points_multi(gem_map *m, const void *xyzi, const void *rgba, int n_s
     for (int s = 0; s < n_segments; s++) hf[s] = make_frame(&frames[s]);
     GEM_CUDA(m, cudaMemcpyAsync(df, hf, (size_t)n_segments * sizeof(FrameParams), cudaMemcpyHostToDevice, m->stream));
     GEM_CUDA(m, cudaEventRecord(m->ev_frames[slot], m->stream));
+    // GEM_B200_PIPE=stream: the steady-state bin runs on the front stream, which waits only for the fold that last used
+    // its scratch (recorded before this copy was queued): it must not read the table before the copy lands
+    if (m->pipe_mode == 1 && m->front_stream) GEM_CUDA(m, cudaStreamWaitEvent(m->front_stream, m->ev_frames[slot], 0));
     const BinSource in = xyzi_source(xyzi, rgba, 0);
     const FoldSrc fs{in.xyzi ? (const char *)in.xyzi + 12 : nullptr, 16};
     // pipelined like gem_add_points_stream: consecutive multi-sensor steps overlap bin(i+1) with fold(i)

@@ -1,0 +1,246 @@
+"""The call scripts of tests/sequence_cases.py on the device map and the oracle side by side, under every schedule the
+add path has: one CUDA graph per call (the default), the bin on a second stream ordered by events, fully serial,
+profiling on (serial, with per-kernel event timing), the padded shared-memory launch of GEM_B200_EXCLUSIVE and a small
+GEM_B200_FOLD_BLOCKS cap.  At every reader and at the end of a script everything observable is compared bit for bit:
+all layers, the state after each move, map_feature, the exports, the orthomosaic, the visual cloud, harvested records,
+process_points outputs and stats().  A difference names the script, the step and the schedule."""
+import ctypes as C
+
+import numpy as np
+import pytest
+
+import gem_b200
+import sequence_cases as sc
+
+pytestmark = pytest.mark.gpu
+
+SCHEDULES = {
+    "graph": {},
+    "stream": {"GEM_B200_PIPE": "stream"},
+    "off": {"GEM_B200_PIPE": "off"},
+    "profile": {},
+    "exclusive": {"GEM_B200_EXCLUSIVE": "1"},
+    "fold_blocks_8": {"GEM_B200_FOLD_BLOCKS": "8"},
+}
+ENV = ("GEM_B200_PIPE", "GEM_B200_EXCLUSIVE", "GEM_B200_FOLD_BLOCKS", "GEM_B200_LONG_BLOCKS")
+_ORACLE = {}
+
+
+def _oracle_trace(name):
+    """the oracle's outputs of a script (the same under every schedule)"""
+    if name not in _ORACLE:
+        _ORACLE[name] = sc.run_oracle(sc.script_by_name(name))
+    return _ORACLE[name]
+
+
+def _same(a, b):
+    a, b = np.asarray(a), np.asarray(b)
+    if a.shape != b.shape:
+        return f"shape {a.shape} != {b.shape}"
+    if a.dtype.kind == "f":
+        a32, b32 = a.astype(np.float32), b.astype(np.float32)
+        ok = (a32.view(np.uint32) == b32.view(np.uint32)) | (np.isnan(a32) & np.isnan(b32))
+    else:
+        ok = a == b
+    if ok.all():
+        return None
+    bad = np.argwhere(~ok)
+    i = tuple(bad[0])
+    return f"{bad.shape[0]} values differ, first at {i}: device={a[i]!r} oracle={b[i]!r}"
+
+
+class DeviceRun:
+    def __init__(self, script, schedule):
+        self.s = script
+        self.schedule = schedule
+        self.g = gem_b200.ElevationMap(script.L, script.res, compat_box_filter=False, max_points=sc.MAX_POINTS)
+        if schedule == "profile":
+            self.g.profile_enable()
+        self.keep = []           # device and pinned inputs stay alive until the map is closed
+        self.proc = None
+        self.last_move = None
+
+    def check(self, where, what, got, want):
+        d = _same(got, want)
+        assert d is None, f"{self.s.name} step {where} [{self.schedule}]: {what}: {d}"
+
+    def _device(self, a):
+        import torch
+        t = torch.from_numpy(np.ascontiguousarray(a)).cuda()
+        torch.cuda.synchronize()                         # the library works on its own stream
+        self.keep.append(t)
+        return t
+
+    def _pinned(self, a):
+        import torch
+        t = torch.from_numpy(np.ascontiguousarray(a)).pin_memory()
+        self.keep.append(t)
+        return t
+
+    def _add(self, variant, c, f):
+        g = self.g
+        n = c["xyzi"].shape[0]
+        if variant == "host":
+            g.add(c["xyzi"], c["rgba"], f)
+        elif variant == "dev":
+            g.add(self._device(c["xyzi"]), self._device(c["rgba"]), f)
+        elif variant == "stream":
+            x, r = self._device(c["xyzi"]), self._device(c["rgba"])
+            g.add_stream_fast(C.c_void_p(x.data_ptr()), C.c_void_p(r.data_ptr()), n, C.byref(f))
+        elif variant == "host_async":
+            x, r = self._pinned(c["xyzi"]), self._pinned(c["rgba"])
+            g.add_host_async_fast(C.c_void_p(x.data_ptr()), C.c_void_p(r.data_ptr()), n, C.byref(f))
+        elif variant == "pcl":
+            g.add_pcl(sc.pcl_records(c), f)
+        else:
+            raise ValueError(variant)
+
+    def _empty(self, variant):
+        g, f = self.g, sc.frame(np.eye(4))
+        if variant == "host":
+            g.add(np.zeros((0, 4), np.float32), None, f)
+        elif variant == "dev":
+            g.add_fast(None, None, 0, C.byref(f))
+        elif variant == "stream":
+            g.add_stream_fast(None, None, 0, C.byref(f))
+        elif variant == "host_async":
+            g.add_host_async_fast(None, None, 0, C.byref(f))
+        elif variant == "pcl":
+            g.add_pcl(np.zeros((0, 8), np.float32), f)
+        else:
+            x = self._device(np.zeros((1, 4), np.float32))
+            g.add_multi(x, None, [0, 0], [f])
+
+    def _stats(self, where, want):
+        if want is not None:
+            got = self.g.stats()
+            assert got == want, f"{self.s.name} step {where} [{self.schedule}]: stats {got} != oracle {want}"
+
+    def _layers(self, where, want):
+        for name, b in want.items():
+            self.check(where, f"layer {name}", self.g.get_layer(name), b)
+
+    def _readouts(self, where, want):
+        g = self.g
+        f = g.map_feature()
+        for k, b in want["feature"].items():
+            self.check(where, f"map_feature {k}", f[k], b)
+        e = g.export_layers()
+        for k, b in want["export"].items():
+            self.check(where, f"export {k}", e[k], b)
+        self.check(where, "orthomosaic", g.export_orthomosaic(), want["ortho"])
+        xyz, rgb, n = g.export_visual_points()
+        self.check(where, "visual cloud xyz", xyz, want["vis_xyz"])
+        self.check(where, "visual cloud rgb", rgb, want["vis_rgb"])
+
+    def step(self, i, op, a, want):
+        g = self.g
+        where = f"{i} ({op})"
+        if op == "move":
+            got = g.move(a["pos"])
+            for k, what in enumerate(("centre", "start", "shift")):
+                self.check(where, f"move {what}", got[k], want["returned"][k])
+            c, st, z = g.state()
+            oc, ost, oz = want["state"]
+            self.check(where, "state centre", c, oc)
+            self.check(where, "state start", st, ost)
+            assert z == oz, f"{self.s.name} step {where} [{self.schedule}]: sensor z {z} != {oz}"
+            self.last_move = (got[0], got[2])
+        elif op == "add":
+            self._add(a["variant"], self.s.clouds[a["cloud"]], sc.frame(a["T"]))
+            if a["variant"] not in sc.PIPELINED:
+                self._stats(where, sc_stats(want, self.s, a))
+        elif op == "multi":
+            cl = [self.s.clouds[n] for n in a["clouds"]]
+            x = self._device(np.concatenate([c["xyzi"] for c in cl]))
+            r = self._device(np.concatenate([c["rgba"] for c in cl]))
+            off = np.concatenate([[0], np.cumsum([c["xyzi"].shape[0] for c in cl])])
+            g.add_multi(x, r, off, [sc.frame(T) for T in a["Ts"]])
+        elif op == "empty":
+            self._empty(a["variant"])
+        elif op == "var_update":
+            g.var_update(a["dv"])
+        elif op == "set_variance":
+            v = g.get_layer("variance")
+            self.check(where, "variance before set_layer", v, want["variance_in"])
+            g.set_layer("variance", sc.set_variance_values(v))
+        elif op == "opt_move":
+            self.check(where, "opt_move aligned", g.opt_move(a["p"], a["dh"]), want["aligned"])
+        elif op == "closeloop":
+            g.closeloop(a["p"], a["dh"])
+        elif op == "process":
+            c = self.s.clouds[a["cloud"]]
+            x = c["xyzi"]
+            got = g.process_points(x[:, 0], x[:, 1], x[:, 2], sc.frame(a["T"]))
+            for k, what in enumerate(("key", "var", "x", "y", "z")):
+                self.check(where, f"process_points {what}", got[k], want["process"][k])
+            self.proc = (c, got)
+        elif op == "fuse":
+            c, (key, var, _, _, zt) = self.proc
+            R, G, B = (c["rgba"][:, k].astype(np.int32) for k in range(3))
+            g.fuse_points(key, R, G, B, c["xyzi"][:, 3], zt, var)
+        elif op == "layers":
+            self._layers(where, want["layers"])
+        elif op == "observe":
+            self._layers(where, want["layers"])
+            self._readouts(where, want)
+        elif op == "export_ray":
+            f = g.map_feature()
+            for k, b in want["feature"].items():
+                self.check(where, f"map_feature {k}", f[k], b)
+            L = self.s.L
+            out = {k: self._pinned(np.zeros((L, L), np.float32)).numpy().T for k in want["export"]}   # Fortran order
+            g.export_layers_begin(out)
+            g.raytracing()                                # may run while the copies are in flight
+            g.export_layers_end()
+            for k, b in want["export"].items():
+                self.check(where, f"export_layers_begin/_end {k}", out[k], b)
+        elif op == "raytracing":
+            g.raytracing()
+        elif op == "snapshot":
+            f = g.map_feature()
+            for k, b in want["feature"].items():
+                self.check(where, f"map_feature {k}", f[k], b)
+            g.snapshot_shown()
+        elif op == "harvest":
+            centre, shift = self.last_move
+            rec, n = g.harvest_scrolled_out(centre, shift)
+            orec, on = want["harvest"]
+            assert n == on, f"{self.s.name} step {where} [{self.schedule}]: harvested {n} != {on}"
+            self.check(where, "harvested records", rec, orec)
+        elif op == "sync":
+            g.sync()
+            self._stats(where, want["stats"])
+        else:
+            raise ValueError(op)
+
+
+def sc_stats(want, s, a):
+    """stats() of a serial add: the oracle's process_points keys of the call"""
+    key = want["keys"]
+    k = key[key >= 0]
+    counts = np.bincount(k, minlength=s.L * s.L)
+    return {"points_in": int(s.clouds[a["cloud"]]["xyzi"].shape[0]), "points_binned": int(k.size),
+            "cells_touched": int((counts > 0).sum()), "max_points_per_cell": int(counts.max()) if k.size else 0}
+
+
+@pytest.mark.parametrize("schedule", sorted(SCHEDULES))
+@pytest.mark.parametrize("name", sc.SCRIPT_NAMES)
+def test_script_matches_oracle(name, schedule, monkeypatch):
+    for k in ENV:
+        monkeypatch.delenv(k, raising=False)
+    for k, v in SCHEDULES[schedule].items():
+        monkeypatch.setenv(k, v)                          # gem_create reads the schedule
+    trace = _oracle_trace(name)
+    s = sc.script_by_name(name)
+    run = DeviceRun(s, schedule)
+    try:
+        for i, (op, a, want) in enumerate(trace):
+            run.step(i, op, a, want)
+        run.g.sync()
+        if schedule == "profile":
+            pr = run.g.profile_read()
+            assert pr["count"]["bin"] > 0 and pr["count"]["fold"] > 0, f"{name} [{schedule}]: {pr}"
+            assert pr["ms"]["bin"] > 0 and pr["ms"]["fold"] > 0, f"{name} [{schedule}]: {pr}"
+    finally:
+        run.g.close()
