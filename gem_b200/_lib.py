@@ -84,8 +84,18 @@ class GemCostmapMarks(C.Structure):
                 ("max_x", C.c_double), ("max_y", C.c_double)]
 
 
+class GemVoxelGridParams(C.Structure):
+    _fields_ = [("leaf_size", C.c_float * 3), ("field", C.c_int), ("limit_min", C.c_double), ("limit_max", C.c_double),
+                ("limit_negative", C.c_int)]
+
+
+class GemVoxelGridInfo(C.Structure):
+    _fields_ = [("count", C.c_int), ("used", C.c_int), ("passthrough", C.c_int)]
+
+
 COST_FREE, COST_LETHAL, COST_UNKNOWN = 0, 254, 255           # GEM_COST_*
 COSTMAP_MODES = {"max": 0, "overwrite": 1}                  # GEM_COSTMAP_MAX / GEM_COSTMAP_OVERWRITE
+VOXEL_FIELDS = {None: -1, "x": 0, "y": 1, "z": 2, "intensity": 3}  # GEM_VOXEL_FIELD_*
 
 PROF_CLASSES = ["bin", "fold_long", "unused", "fold", "clear_floor", "features", "raytrace", "other", "route"]
 
@@ -151,6 +161,7 @@ SYMBOLS = {
                                           C.POINTER(GemCostmapMarks)]),
     "gem_costmap_update_origin": (C.c_int, [_P, C.POINTER(GemCostmapWindow), C.c_double, C.c_double, C.c_ubyte, _P]),
     "gem_costmap_combine": (C.c_int, [_P, C.c_int, _P, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int]),
+    "gem_voxel_grid": (C.c_int, [_P, _P, C.c_int, C.POINTER(GemVoxelGridParams), _P, C.c_int, C.POINTER(GemVoxelGridInfo)]),
     "gem_get_layer_device": (C.c_int, [_P, C.c_int, _P]),
     "gem_compute_features_tiled": (C.c_int, [_P, _P]),
     "gem_raytracing_tiled": (C.c_int, [_P, _P]),

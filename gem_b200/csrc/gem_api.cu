@@ -11,6 +11,7 @@
 #include <cuda_runtime.h>
 
 #include <algorithm>
+#include <cfloat>
 
 #include <cmath>
 #include <cstdio>
@@ -29,6 +30,7 @@
 #include "gem_octree.cuh"
 #include "gem_route.cuh"
 #include "gem_submap.cuh"
+#include "gem_voxel.cuh"
 
 using namespace gem;
 
@@ -61,10 +63,13 @@ struct TiledState { // gem_tiled_attach
     cudaGraphNode_t long_node = nullptr, fold_node = nullptr, route_node = nullptr, bin_node = nullptr;
 };
 
-struct OctBuf { // a device scratch buffer of gem_color_octree: grows on demand, never shrinks
+struct OctBuf { // a device scratch buffer (octree, costmap and voxel-grid calls): grows on demand, never shrinks
     void *p = nullptr;
     size_t cap = 0;
     template <typename T> T *as() const { return static_cast<T *>(p); }
+};
+struct VoxScratch { // gem_voxel_grid (gem_voxel.cuh): keys and input indices before / after the sort, runs, offsets
+    OctBuf key[2], idx[2], cnt, off, temp, acc;
 };
 struct OctScratch { // gem_color_octree (gem_octree.cuh); every buffer is consistent with its own capacity at all times
     OctBuf code[2], idx[2], leaf, cnt, off, level, ghead, gid, val, groups, ctr, temp, key2[2], nkey[2], nrec[2], dense;
@@ -141,6 +146,7 @@ struct gem_map {
     OctScratch oct;                // gem_color_octree: scratch and the last stream
     OctBuf cost_scratch;           // costmap calls: the winner per costmap cell (int), or the copy of a rolled grid
     CostMarksDev *cost_acc = nullptr; // costmap mark calls: counts and encoded touch bounds
+    VoxScratch vox;                // gem_voxel_grid
     unsigned long long *d_stamps = nullptr; // gem_debug_stamps
     int *d_raylist = nullptr;      // ray clean-up: cells that cast a ray + their count
     uint32_t *d_bitmap = nullptr;  // ray clean-up: validity bitmap of the lowest layer (own tile / map-wide)
@@ -867,7 +873,8 @@ int gem_destroy(gem_map *m)
         for (OctBuf *b : {&m->oct.code[0], &m->oct.code[1], &m->oct.idx[0], &m->oct.idx[1], &m->oct.leaf, &m->oct.cnt, &m->oct.off,
                           &m->oct.level, &m->oct.ghead, &m->oct.gid, &m->oct.val, &m->oct.groups, &m->oct.ctr, &m->oct.temp,
                           &m->oct.key2[0], &m->oct.key2[1], &m->oct.nkey[0], &m->oct.nkey[1], &m->oct.nrec[0], &m->oct.nrec[1],
-                          &m->oct.dense, &m->cost_scratch})
+                          &m->oct.dense, &m->cost_scratch, &m->vox.key[0], &m->vox.key[1], &m->vox.idx[0], &m->vox.idx[1],
+                          &m->vox.cnt, &m->vox.off, &m->vox.temp, &m->vox.acc})
             if (b->p) cudaFree(b->p);
         if (m->h_ctr) cudaFreeHost(m->h_ctr);
         if (m->h_ctr_ring) cudaFreeHost(m->h_ctr_ring);
@@ -1705,20 +1712,26 @@ int gem_grid_cloud_split(gem_map *m, int source, int mean_k, double stddev_mul, 
     return GEM_OK;
 }
 
-// Grow one gem_color_octree scratch buffer to at least `bytes`.  The new buffer is allocated before the old one is
-// released, so a failed growth leaves the buffer as it was.
-static int oct_grow(gem_map *m, OctBuf &b, size_t bytes)
+// Grow a device scratch buffer (octree, costmap, voxel grid) to at least `bytes`, with a quarter of slack and at least
+// 4 KiB so that slowly growing inputs do not reallocate on every call.  The new buffer is allocated before the old one is
+// released, so a failed growth leaves the buffer as it was; the stream is drained before the old buffer goes, because
+// work queued on it (an update_origin, say) may still read it.
+static int scratch_grow(gem_map *m, OctBuf &b, size_t bytes, const char *what)
 {
     if (b.cap >= bytes) return GEM_OK;
     bytes = std::max(bytes + bytes / 4, (size_t)4096);
     void *q = nullptr;
     const cudaError_t e = cudaMalloc(&q, bytes);
-    if (e != cudaSuccess) return fail(m, GEM_ERR_NOMEM, std::string("gem_color_octree: cudaMalloc: ") + cudaGetErrorString(e));
-    if (b.p) cudaFree(b.p);
+    if (e != cudaSuccess) return fail(m, GEM_ERR_NOMEM, std::string(what) + ": cudaMalloc: " + cudaGetErrorString(e));
+    if (b.p) {
+        cudaStreamSynchronize(m->stream);
+        cudaFree(b.p);
+    }
     b.p = q;
     b.cap = bytes;
     return GEM_OK;
 }
+static int oct_grow(gem_map *m, OctBuf &b, size_t bytes) { return scratch_grow(m, b, bytes, "gem_color_octree"); }
 
 // pointCloudtoOctomap's tree (ElevationMapping.cpp:1157-1174) as the ColorOcTree::writeData stream (gem_octree.cuh,
 // DESIGN.md f7)
@@ -1860,23 +1873,7 @@ static bool cost_window_ok(const gem_costmap_window *w)
 {
     return w && cost_sizes_ok(w->size_x, w->size_y) && std::isfinite(w->resolution) && w->resolution > 0.0;
 }
-// Grow the costmap scratch to at least `bytes`.  The stream is drained before the old buffer goes (an update_origin may
-// still read it), and the new buffer is allocated first, so a failed growth leaves the scratch as it was.
-static int cost_grow(gem_map *m, size_t bytes)
-{
-    OctBuf &b = m->cost_scratch;
-    if (b.cap >= bytes) return GEM_OK;
-    void *q = nullptr;
-    const cudaError_t e = cudaMalloc(&q, bytes);
-    if (e != cudaSuccess) return fail(m, GEM_ERR_NOMEM, std::string("costmap scratch: cudaMalloc: ") + cudaGetErrorString(e));
-    if (b.p) {
-        cudaStreamSynchronize(m->stream);
-        cudaFree(b.p);
-    }
-    b.p = q;
-    b.cap = bytes;
-    return GEM_OK;
-}
+static int cost_grow(gem_map *m, size_t bytes) { return scratch_grow(m, m->cost_scratch, bytes, "costmap scratch"); }
 // the last-writer scatter of both mark calls (pass 1, pass 2), then the marks back to the host
 extern "C++" {
 template <class Src> static int cost_mark(gem_map *m, const Src &src, long long nchunks, const gem_costmap_window *w, unsigned char *cost,
@@ -1991,6 +1988,134 @@ int gem_costmap_combine(gem_map *m, int mode, const unsigned char *layer_device,
     GEM_LAUNCH(m, GEM_PROF_OTHER, k_costmap_combine<<<grid, COST_BLOCK, 0, m->stream>>>(layer_device, master_device, size_x, i0, i1, j0, j1,
                                                                                     mode, vec));
     GEM_CUDA(m, cudaGetLastError());
+    return GEM_OK;
+}
+
+// ---- the VoxelGrid pre-filter of GEM's demo launches (gem_voxel.cuh, DESIGN.md f9) ------------------------------------
+int gem_voxel_grid(gem_map *m, const void *xyzi_device, int n, const gem_voxel_grid_params *p, void *out_xyzi_device, int capacity,
+                   gem_voxel_grid_info *info)
+{
+    if (!m || !p || !info || n < 0 || (n > 0 && !xyzi_device) || capacity < 0 || (capacity > 0 && !out_xyzi_device))
+        return fail(m, GEM_ERR_INVALID, "gem_voxel_grid: bad argument");
+    if (p->field < GEM_VOXEL_FIELD_NONE || p->field > GEM_VOXEL_FIELD_INTENSITY) return fail(m, GEM_ERR_INVALID, "gem_voxel_grid: bad field id");
+    for (int a = 0; a < 3; a++) // V1
+        if (!std::isfinite(p->leaf_size[a]) || !(p->leaf_size[a] > 0.0f))
+            return fail(m, GEM_ERR_INVALID, "gem_voxel_grid: every leaf size must be finite and positive");
+    // V9: input and output ranges may not overlap (chained calls alternate between two buffers)
+    const uintptr_t i0 = (uintptr_t)xyzi_device, i1 = i0 + (size_t)n * sizeof(float4);
+    const uintptr_t o0 = (uintptr_t)out_xyzi_device, o1 = o0 + (size_t)capacity * sizeof(float4);
+    if (n > 0 && capacity > 0 && i0 < o1 && o0 < i1) return fail(m, GEM_ERR_INVALID, "gem_voxel_grid: the input and output ranges overlap");
+    Lock lk(m->mu);
+    SetDev sd(m->dev);
+    gem_voxel_grid_info r{};
+    if (n == 0) { // V5
+        *info = r;
+        return GEM_OK;
+    }
+    VoxParams P{};
+    for (int a = 0; a < 3; a++) P.inv[a] = 1.0f / p->leaf_size[a];
+    P.field = p->field;
+    P.lmin = p->limit_min;
+    P.lmax = p->limit_max;
+    P.flmin = (float)p->limit_min; // getMinMax3D takes the limits as floats
+    P.flmax = (float)p->limit_max;
+    P.negative = p->limit_negative ? 1 : 0;
+    using u64 = unsigned long long;
+    const size_t N = (size_t)n;
+    cudaStream_t st = m->stream;
+    VoxScratch &S = m->vox;
+    // every buffer is sized before the first write (the sort's temporary for the widest key), so that a failed growth
+    // writes nothing
+    size_t t_sort = 0, t_rle = 0, t_scan = 0;
+    GEM_CUDA(m, cub::DeviceRadixSort::SortPairs(nullptr, t_sort, (u64 *)nullptr, (u64 *)nullptr, (int *)nullptr, (int *)nullptr, n, 0, 64, st));
+    GEM_CUDA(m, cub::DeviceRunLengthEncode::Encode(nullptr, t_rle, (u64 *)nullptr, (u64 *)nullptr, (int *)nullptr, (int *)nullptr, n, st));
+    GEM_CUDA(m, cub::DeviceScan::ExclusiveSum(nullptr, t_scan, (int *)nullptr, (int *)nullptr, n, st));
+    const char *what = "gem_voxel_grid";
+    int rc;
+    if ((rc = scratch_grow(m, S.key[0], N * 8, what)) || (rc = scratch_grow(m, S.key[1], N * 8, what)) ||
+        (rc = scratch_grow(m, S.idx[0], N * 4, what)) || (rc = scratch_grow(m, S.idx[1], N * 4, what)) ||
+        (rc = scratch_grow(m, S.cnt, N * 4, what)) || (rc = scratch_grow(m, S.off, N * 4, what)) ||
+        (rc = scratch_grow(m, S.temp, std::max(t_sort, std::max(t_rle, t_scan)), what)) || (rc = scratch_grow(m, S.acc, sizeof(VoxAcc), what)))
+        return rc;
+    const float4 *in = static_cast<const float4 *>(xyzi_device);
+    float4 *out = static_cast<float4 *>(out_xyzi_device);
+    VoxAcc *acc = S.acc.as<VoxAcc>();
+    VoxAcc h{};
+    for (int a = 0; a < 3; a++) { h.mn[a] = vg_key(FLT_MAX); h.mx[a] = vg_key(-FLT_MAX); }
+    GEM_CUDA(m, cudaMemcpyAsync(acc, &h, sizeof h, cudaMemcpyHostToDevice, st));
+    GEM_LAUNCH(m, GEM_PROF_OTHER, k_vox_bounds<<<blocks_for(N, VOX_BLOCK, NUM_SMS * 8), VOX_BLOCK, 0, st>>>(in, n, P, acc));
+    GEM_CUDA(m, cudaGetLastError());
+    // synchronisation 1: V4, V5 and the key layout are decided on the host from the counts and the bounds
+    GEM_CUDA(m, cudaMemcpyAsync(&h, acc, sizeof h, cudaMemcpyDeviceToHost, st));
+    GEM_CUDA(m, cudaStreamSynchronize(st));
+    r.used = h.used;
+    if (h.bounded == 0) { // V5
+        *info = r;
+        return GEM_OK;
+    }
+    // V4: d[a] = (int64)((max_p - min_p) * inv) + 1, the product in float.  DEFINED: a product that is not finite or a
+    // quotient >= 2^62 is an overflow; the product of the d is the mathematical one (each step below stays under 2^62)
+    float mn[3], mx[3];
+    long long d[3] = {0, 0, 0};
+    bool over = false;
+    for (int a = 0; a < 3; a++) {
+        mn[a] = vg_unkey(h.mn[a]);
+        mx[a] = vg_unkey(h.mx[a]);
+        const float q = (mx[a] - mn[a]) * P.inv[a];
+        if (!std::isfinite(q) || q >= 4611686018427387904.0f) over = true;
+        else d[a] = (long long)q + 1;
+    }
+    over = over || d[0] > INT32_MAX || d[1] > INT32_MAX || d[2] > INT32_MAX || d[0] * d[1] > INT32_MAX || d[0] * d[1] * d[2] > INT32_MAX;
+    if (over) { // the input unchanged: PCL's output = *input_
+        const size_t k = std::min(N, (size_t)capacity);
+        if (k) GEM_CUDA(m, cudaMemcpyAsync(out, in, k * sizeof(float4), cudaMemcpyDeviceToDevice, st));
+        GEM_CUDA(m, cudaStreamSynchronize(st)); // synchronisation 2: the call is host-synchronous
+        r.count = n;
+        r.passthrough = 1;
+        *info = r;
+        return GEM_OK;
+    }
+    if (h.used == 0) {
+        *info = r;
+        return GEM_OK;
+    }
+    // V6: min_b, max_b as floor values of float products (exact in either overload), div from their exact difference; the
+    // mixed-radix key ijk0 + ijk1 div0 + ijk2 div0 div1 in 64 bits is PCL's idx where that fits an int and the DEFINED
+    // lexicographic order where it does not
+    VoxGrid G{};
+    u64 div[3];
+    for (int a = 0; a < 3; a++) {
+        G.minb[a] = std::floor((double)(mn[a] * P.inv[a]));
+        div[a] = (u64)(std::floor((double)(mx[a] * P.inv[a])) - G.minb[a]) + 1;
+    }
+    // with V4 passed the voxel count stays far below 2^62 (each div[a] is within a few times d[a]); guarded all the same
+    if (!((double)div[0] * (double)div[1] * (double)div[2] < 4.0e18))
+        return fail(m, GEM_ERR_INVALID, "gem_voxel_grid: the voxel grid needs keys wider than 62 bits");
+    G.div0 = div[0];
+    G.div01 = div[0] * div[1];
+    G.cut_key = G.div01 * div[2]; // one past the largest voxel key: the cut points' run sorts last
+    int bits = 1;
+    while ((1ull << bits) <= G.cut_key) bits++;
+    u64 *key0 = S.key[0].as<u64>(), *key1 = S.key[1].as<u64>();
+    int *idx0 = S.idx[0].as<int>(), *idx1 = S.idx[1].as<int>(), *cnt = S.cnt.as<int>(), *off = S.off.as<int>();
+    size_t tcap = S.temp.cap;
+    // the run-length encoding writes nruns <= n counts; the scan runs over all n, so the rest must be defined
+    GEM_CUDA(m, cudaMemsetAsync(cnt, 0, N * sizeof(int), st));
+    GEM_LAUNCH(m, GEM_PROF_OTHER, k_vox_keys<<<(unsigned)((N + VOX_BLOCK - 1) / VOX_BLOCK), VOX_BLOCK, 0, st>>>(in, n, P, G, key0, idx0));
+    GEM_CUDA(m, cudaGetLastError());
+    // V7: the stable sort keeps each voxel's points in input order
+    GEM_CUDA(m, cub::DeviceRadixSort::SortPairs(S.temp.p, tcap, key0, key1, idx0, idx1, n, 0, bits, st));
+    GEM_CUDA(m, cub::DeviceRunLengthEncode::Encode(S.temp.p, tcap, key1, key0, cnt, &acc->nruns, n, st));
+    GEM_CUDA(m, cub::DeviceScan::ExclusiveSum(S.temp.p, tcap, cnt, off, n, st));
+    const int drop = h.used < n ? 1 : 0;
+    GEM_LAUNCH(m, GEM_PROF_OTHER, k_vox_centroids<<<(unsigned)(((size_t)h.used + VOX_BLOCK - 1) / VOX_BLOCK), VOX_BLOCK, 0, st>>>(
+                                      in, idx1, cnt, off, acc, drop, out, capacity));
+    GEM_CUDA(m, cudaGetLastError());
+    // synchronisation 2: the voxel count
+    GEM_CUDA(m, cudaMemcpyAsync(&h.nruns, &acc->nruns, sizeof(int), cudaMemcpyDeviceToHost, st));
+    GEM_CUDA(m, cudaStreamSynchronize(st));
+    r.count = h.nruns - drop;
+    *info = r;
     return GEM_OK;
 }
 

@@ -581,6 +581,40 @@ class ElevationMap:
         check(self._lib.gem_costmap_combine(self._h, _lib.COSTMAP_MODES[mode], pl, pm, int(size_x), int(size_y), i0, j0, i1, j1),
               self._h, "gem_costmap_combine")
 
+    # -- the VoxelGrid pre-filter of GEM's demo launches (DESIGN.md f9) ---------------------------------------------------
+    def voxel_grid(self, xyzi, leaf_size, field=None, limits=(-3.4028234663852886e38, 3.4028234663852886e38), negative=False,
+                   out=None):
+        """pcl_ros's VoxelGrid nodelet over `xyzi`, a contiguous (n, 4) float32 CUDA tensor {x, y, z, intensity}: leaf_size
+        is a number or three; field None, "x", "y", "z" or "intensity" with the double limits (lo, hi) and the negative
+        flag.  The centroids go to `out` (a contiguous (k, 4) float32 CUDA tensor, k = 0 being a size query) or to a new
+        (n, 4) tensor.  Returns (out[:min(count, k)], {count, used, passthrough}); the two may not overlap"""
+        import torch
+
+        def cloud(t, what):
+            if not (_is_device(t) and t.dtype == torch.float32 and t.dim() == 2 and t.shape[1] == 4 and t.is_contiguous()):
+                raise ValueError(f"voxel_grid: {what} must be a contiguous (n, 4) float32 CUDA tensor")
+            if t.device.index != self._device_index():
+                raise ValueError(f"voxel_grid: {what} is on {t.device}, the map on cuda:{self._device_index()}")
+
+        cloud(xyzi, "xyzi")
+        n = int(xyzi.shape[0])
+        if out is None:
+            out = torch.empty((n, 4), dtype=torch.float32, device=xyzi.device)
+        cloud(out, "out")
+        leaf = [float(leaf_size)] * 3 if np.ndim(leaf_size) == 0 else [float(v) for v in leaf_size]
+        if len(leaf) != 3:
+            raise ValueError("voxel_grid: leaf_size is one number or three")
+        if field not in _lib.VOXEL_FIELDS:
+            raise ValueError(f"voxel_grid: field must be one of {list(_lib.VOXEL_FIELDS)}")
+        lo, hi = (float(v) for v in limits)
+        p = _lib.GemVoxelGridParams((C.c_float * 3)(*leaf), _lib.VOXEL_FIELDS[field], lo, hi, 1 if negative else 0)
+        info = _lib.GemVoxelGridInfo()
+        cap = int(out.shape[0])
+        torch.cuda.current_stream(xyzi.device).synchronize()   # the library reads and writes on its own stream
+        check(self._lib.gem_voxel_grid(self._h, _ptr(xyzi) if n else None, n, C.byref(p), _ptr(out) if cap else None, cap,
+                                       C.byref(info)), self._h, "gem_voxel_grid")
+        return out[:min(info.count, cap)], {k: getattr(info, k) for k, _ in _lib.GemVoxelGridInfo._fields_}
+
     def harvest_to_local_map(self, current_xy, shift_xy, records: bool = False):
         """the harvest of harvest_scrolled_out, upserted into the device-resident localMap_ (ElevationMapping.cpp:740-747).
         Returns the number of harvested records, or (records (n, 8) float32 host array, n) with records=True"""

@@ -383,6 +383,48 @@ int gem_costmap_update_origin(gem_map *m, gem_costmap_window *w, double new_orig
 int gem_costmap_combine(gem_map *m, int mode, const unsigned char *layer_device, unsigned char *master_device, int size_x, int size_y,
                         int min_i, int min_j, int max_i, int max_j);
 
+/* ---- the VoxelGrid pre-filter of GEM's demo launches (filter.launch, filter_kitti.launch; DESIGN.md f9) ----
+ * gem_voxel_grid: pcl_ros's VoxelGrid nodelet, i.e. pcl::VoxelGrid<pcl::PCLPointCloud2> of PCL 1.8 with downsample_all_data_
+ *   true, over n x float4 {x, y, z, intensity} in device memory (the layout the add calls take).  Unpinned: restated, PCL
+ *   is not available.
+ *   V1 leaf: float leaf_size[3], inv[a] = 1.0f / leaf_size[a] in float; a leaf that is not finite or is <= 0 is an error.
+ *   V2 used points: with a field selected (x, y, z or intensity), its float value v is cut when (double)v > limit_max ||
+ *      (double)v < limit_min (limit_negative = 0), or when (double)v < limit_max && (double)v > limit_min (limit_negative = 1);
+ *      a NaN v passes.  A point that passes (every point without a field) is then cut when x, y or z is not finite; is_dense
+ *      is not read.
+ *   V3 bounds (getMinMax3D): the same two tests against (float)limit_min, (float)limit_max compared in float; min_p / max_p
+ *      are the per-axis float min / max over the survivors, from FLT_MAX / -FLT_MAX.  Every V2 survivor survives V3.
+ *   V4 overflow: d[a] = (int64)((max_p[a] - min_p[a]) * inv[a]) + 1, the product in float; if d[0] d[1] d[2] > INT32_MAX the
+ *      output is the input unchanged (all n points in order, bit for bit) and passthrough = 1.  DEFINED: a product that is
+ *      not finite, or a quotient >= 2^62, also counts as overflow (PCL's cast is undefined there).
+ *   V5 no V3 survivor (n = 0 included): count 0.  DEFINED: PCL casts -inf to int64 there.
+ *   V6 min_b[a] = floor(min_p[a] * inv[a]), max_b[a] likewise, ijk[a] = floor(p[a] * inv[a]) - min_b[a], idx = ijk0 + ijk1 div0
+ *      + ijk2 div0 div1 with div[a] = max_b[a] - min_b[a] + 1; output in ascending idx, i.e. lexicographic in (ijk2, ijk1,
+ *      ijk0).  The float and the double floor are both exact, so the overload changes nothing.  DEFINED: where div0 div1
+ *      div2 exceeds 2^31 although V4 passed (PCL's int idx overflows) the order is still lexicographic in (ijk2, ijk1, ijk0).
+ *   V7 DEFINED: inside a voxel, ascending input index (PCL's std::sort is not stable).
+ *   V8 centroid: the four components start at +0.0f, c += p in float in V7 order, then c /= (float)count, one IEEE division
+ *      per component.  Intensity is averaged like x, y, z (a lone -0.0 comes out +0.0); no other field is carried.
+ *   V9 min(count, capacity) float4 go to out_xyzi_device; *info always receives count (output points), used (V2 survivors)
+ *      and passthrough.  capacity = 0 is a size query.
+ *   Host-synchronous; works on any handle, tiled ones included; neither reads nor modifies the map and does not issue the
+ *   deferred fold.  A bad leaf, n < 0, NULL points with n > 0, capacity < 0, NULL out with capacity > 0, a bad field id
+ *   and overlapping input and output ranges are GEM_ERR_INVALID (chain calls, as the KITTI launch does, through two
+ *   buffers).  Uses a handle-owned scratch of about 32 bytes per input point, grown on demand: a failed growth is
+ *   GEM_ERR_NOMEM.  A rejected call writes nothing.  min_points_per_voxel (0 in GEM's launches) is not exposed. */
+enum { GEM_VOXEL_FIELD_NONE = -1, GEM_VOXEL_FIELD_X = 0, GEM_VOXEL_FIELD_Y = 1, GEM_VOXEL_FIELD_Z = 2, GEM_VOXEL_FIELD_INTENSITY = 3 };
+typedef struct gem_voxel_grid_params {
+    float leaf_size[3];
+    int field;                    /* GEM_VOXEL_FIELD_*                                       */
+    double limit_min, limit_max;  /* the nodelet's filter_limit_min / _max                   */
+    int limit_negative;           /* the nodelet's filter_limit_negative                     */
+} gem_voxel_grid_params;
+typedef struct gem_voxel_grid_info {
+    int count, used, passthrough; /* output points, V2 survivors, V4 taken                   */
+} gem_voxel_grid_info;
+int gem_voxel_grid(gem_map *m, const void *xyzi_device, int n, const gem_voxel_grid_params *p,
+                   void *out_xyzi_device, int capacity, gem_voxel_grid_info *info);
+
 /* raw layer access (row-major L*L, float or int32 for the colour ids) for tests and
  * checkpoint/restore (the dead G_get_mapinfo/G_set_mapinfo of gpu.cu:457-475). */
 int gem_get_layer(gem_map *m, int layer, void *host_out);

@@ -303,6 +303,17 @@ class ElevationMap {
     {
         check(gem_costmap_combine(h_, mode, layer_device, master_device, sizeX, sizeY, minI, minJ, maxI, maxJ), "gem_costmap_combine");
     }
+    // pcl_ros's VoxelGrid nodelet (GEM's filter.launch / filter_kitti.launch; DESIGN.md f9) over n float4 {x, y, z, intensity}
+    // in device memory: min(count, capacity) centroids go to out_device, which must not overlap the input (capacity 0 is
+    // a size query).  Chain calls through two buffers.
+    gem_voxel_grid_info voxelGrid(const void *xyzi_device, size_t n, const gem_voxel_grid_params &p, void *out_device, size_t capacity)
+    {
+        if (n > (size_t)std::numeric_limits<int>::max() || capacity > (size_t)std::numeric_limits<int>::max())
+            throw std::runtime_error("voxelGrid: more than INT_MAX points");
+        gem_voxel_grid_info info{};
+        check(gem_voxel_grid(h_, xyzi_device, (int)n, &p, out_device, (int)capacity, &info), "gem_voxel_grid");
+        return info;
+    }
     int harvestToLocalMap(const float current[2], const float shift[2], std::vector<PointXYZRGBICT> *visual = nullptr)
     {
         int n = 0;
