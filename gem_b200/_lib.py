@@ -93,9 +93,20 @@ class GemVoxelGridInfo(C.Structure):
     _fields_ = [("count", C.c_int), ("used", C.c_int), ("passthrough", C.c_int)]
 
 
+class GemMlsParams(C.Structure):
+    _fields_ = [("search_radius", C.c_double), ("sqr_gauss_param", C.c_double), ("polynomial_fit", C.c_int), ("order", C.c_int),
+                ("upsampling", C.c_int), ("point_density", C.c_int), ("seed", C.c_ulonglong)]
+
+
+class GemMlsInfo(C.Structure):
+    _fields_ = [("count", C.c_longlong), ("processed", C.c_int), ("fitted", C.c_int), ("skipped", C.c_int),
+                ("max_neighbours", C.c_int)]
+
+
 COST_FREE, COST_LETHAL, COST_UNKNOWN = 0, 254, 255           # GEM_COST_*
 COSTMAP_MODES = {"max": 0, "overwrite": 1}                  # GEM_COSTMAP_MAX / GEM_COSTMAP_OVERWRITE
 VOXEL_FIELDS = {None: -1, "x": 0, "y": 1, "z": 2, "intensity": 3}  # GEM_VOXEL_FIELD_*
+MLS_UPSAMPLING = {"none": 0, "random_uniform_density": 1}  # GEM_MLS_*
 
 PROF_CLASSES = ["bin", "fold_long", "unused", "fold", "clear_floor", "features", "raytrace", "other", "route"]
 
@@ -162,6 +173,7 @@ SYMBOLS = {
     "gem_costmap_update_origin": (C.c_int, [_P, C.POINTER(GemCostmapWindow), C.c_double, C.c_double, C.c_ubyte, _P]),
     "gem_costmap_combine": (C.c_int, [_P, C.c_int, _P, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int]),
     "gem_voxel_grid": (C.c_int, [_P, _P, C.c_int, C.POINTER(GemVoxelGridParams), _P, C.c_int, C.POINTER(GemVoxelGridInfo)]),
+    "gem_mls_upsample": (C.c_int, [_P, _P, C.c_int, C.POINTER(GemMlsParams), _P, C.c_longlong, C.POINTER(GemMlsInfo)]),
     "gem_get_layer_device": (C.c_int, [_P, C.c_int, _P]),
     "gem_compute_features_tiled": (C.c_int, [_P, _P]),
     "gem_raytracing_tiled": (C.c_int, [_P, _P]),

@@ -27,6 +27,7 @@
 #include "gem_costmap.cuh"
 #include "gem_kernels.cuh"
 #include "gem_global.cuh"
+#include "gem_mls.cuh"
 #include "gem_octree.cuh"
 #include "gem_route.cuh"
 #include "gem_submap.cuh"
@@ -70,6 +71,10 @@ struct OctBuf { // a device scratch buffer (octree, costmap and voxel-grid calls
 };
 struct VoxScratch { // gem_voxel_grid (gem_voxel.cuh): keys and input indices before / after the sort, runs, offsets
     OctBuf key[2], idx[2], cnt, off, temp, acc;
+};
+struct MlsScratch { // gem_mls_upsample (gem_mls.cuh): cell keys and indices before / after the sort, the points in cell
+                   // order, the distinct cells, neighbour and output counts, output offsets, the long lists and their keys
+    OctBuf key[2], idx[2], spts, ukey, ucnt, uoff, nbr, ocnt, ooff, longs, lkeys, temp, acc;
 };
 struct OctScratch { // gem_color_octree (gem_octree.cuh); every buffer is consistent with its own capacity at all times
     OctBuf code[2], idx[2], leaf, cnt, off, level, ghead, gid, val, groups, ctr, temp, key2[2], nkey[2], nrec[2], dense;
@@ -147,6 +152,7 @@ struct gem_map {
     OctBuf cost_scratch;           // costmap calls: the winner per costmap cell (int), or the copy of a rolled grid
     CostMarksDev *cost_acc = nullptr; // costmap mark calls: counts and encoded touch bounds
     VoxScratch vox;                // gem_voxel_grid
+    MlsScratch mls;                // gem_mls_upsample
     unsigned long long *d_stamps = nullptr; // gem_debug_stamps
     int *d_raylist = nullptr;      // ray clean-up: cells that cast a ray + their count
     uint32_t *d_bitmap = nullptr;  // ray clean-up: validity bitmap of the lowest layer (own tile / map-wide)
@@ -874,7 +880,9 @@ int gem_destroy(gem_map *m)
                           &m->oct.level, &m->oct.ghead, &m->oct.gid, &m->oct.val, &m->oct.groups, &m->oct.ctr, &m->oct.temp,
                           &m->oct.key2[0], &m->oct.key2[1], &m->oct.nkey[0], &m->oct.nkey[1], &m->oct.nrec[0], &m->oct.nrec[1],
                           &m->oct.dense, &m->cost_scratch, &m->vox.key[0], &m->vox.key[1], &m->vox.idx[0], &m->vox.idx[1],
-                          &m->vox.cnt, &m->vox.off, &m->vox.temp, &m->vox.acc})
+                          &m->vox.cnt, &m->vox.off, &m->vox.temp, &m->vox.acc, &m->mls.key[0], &m->mls.key[1], &m->mls.idx[0],
+                          &m->mls.idx[1], &m->mls.spts, &m->mls.ukey, &m->mls.ucnt, &m->mls.uoff, &m->mls.nbr, &m->mls.ocnt,
+                          &m->mls.ooff, &m->mls.longs, &m->mls.lkeys, &m->mls.temp, &m->mls.acc})
             if (b->p) cudaFree(b->p);
         if (m->h_ctr) cudaFreeHost(m->h_ctr);
         if (m->h_ctr_ring) cudaFreeHost(m->h_ctr_ring);
@@ -2115,6 +2123,135 @@ int gem_voxel_grid(gem_map *m, const void *xyzi_device, int n, const gem_voxel_g
     GEM_CUDA(m, cudaMemcpyAsync(&h.nruns, &acc->nruns, sizeof(int), cudaMemcpyDeviceToHost, st));
     GEM_CUDA(m, cudaStreamSynchronize(st));
     r.count = h.nruns - drop;
+    *info = r;
+    return GEM_OK;
+}
+
+// ---- the MLS densification of the dense_mapping signal (gem_mls.cuh, DESIGN.md f10) -----------------------------------
+int gem_mls_upsample(gem_map *m, const void *points32_device, int n, const gem_mls_params *p, void *out_points32_device,
+                     long long capacity, gem_mls_info *info)
+{
+    if (!m || !p || !info || n < 0 || (n > 0 && !points32_device) || capacity < 0 || (capacity > 0 && !out_points32_device))
+        return fail(m, GEM_ERR_INVALID, "gem_mls_upsample: bad argument");
+    if (!std::isfinite(p->search_radius) || !(p->search_radius > 0.0) || !std::isfinite(p->sqr_gauss_param) || !(p->sqr_gauss_param > 0.0))
+        return fail(m, GEM_ERR_INVALID, "gem_mls_upsample: the search radius and the Gauss parameter must be finite and positive");
+    if (p->order < 1 || p->order > 5) return fail(m, GEM_ERR_INVALID, "gem_mls_upsample: the polynomial order must lie in 1..5");
+    if (p->upsampling != GEM_MLS_NONE && p->upsampling != GEM_MLS_RANDOM_UNIFORM_DENSITY)
+        return fail(m, GEM_ERR_INVALID, "gem_mls_upsample: unknown upsampling method");
+    if (p->point_density < 0) return fail(m, GEM_ERR_INVALID, "gem_mls_upsample: point_density < 0");
+    const uintptr_t i0 = (uintptr_t)points32_device, i1 = i0 + (size_t)n * 32;
+    const uintptr_t o0 = (uintptr_t)out_points32_device, o1 = o0 + (size_t)capacity * 32;
+    if (n > 0 && capacity > 0 && i0 < o1 && o0 < i1) return fail(m, GEM_ERR_INVALID, "gem_mls_upsample: the input and output ranges overlap");
+    Lock lk(m->mu);
+    SetDev sd(m->dev);
+    gem_mls_info r{};
+    if (n == 0) {
+        r.fitted = capacity == 0 ? -1 : 0; // M8: a size query reports no fit count
+        *info = r;
+        return GEM_OK;
+    }
+    MlsParams P{};
+    P.r = p->search_radius;
+    P.r2q = P.r * P.r / 4.0;
+    P.gauss = p->sqr_gauss_param;
+    P.edge = P.r * (1.0 + 1.0 / 1024.0); // the search grid (gem_mls.cuh): a neighbour is always less than one edge away
+    P.r2f = (float)(P.r * P.r);
+    P.hi = (float)(P.r / 2.0);
+    P.lo = -P.hi;
+    P.fit = p->polynomial_fit ? 1 : 0;
+    P.order = p->order;
+    P.nc = (p->order + 1) * (p->order + 2) / 2;
+    P.upsampling = p->upsampling;
+    P.density = p->point_density;
+    P.seed = p->seed;
+    using u64 = unsigned long long;
+    const size_t N = (size_t)n;
+    cudaStream_t st = m->stream;
+    MlsScratch &S = m->mls;
+    // every buffer the first synchronisation needs is sized before the first launch, so that a failed growth writes nothing
+    size_t t_sort = 0, t_rle = 0, t_scan = 0, t_scan64 = 0;
+    GEM_CUDA(m, cub::DeviceRadixSort::SortPairs(nullptr, t_sort, (u64 *)nullptr, (u64 *)nullptr, (int *)nullptr, (int *)nullptr, n, 0, 64, st));
+    GEM_CUDA(m, cub::DeviceRunLengthEncode::Encode(nullptr, t_rle, (u64 *)nullptr, (u64 *)nullptr, (int *)nullptr, (int *)nullptr, n, st));
+    GEM_CUDA(m, cub::DeviceScan::ExclusiveSum(nullptr, t_scan, (int *)nullptr, (int *)nullptr, n, st));
+    GEM_CUDA(m, cub::DeviceScan::ExclusiveSum(nullptr, t_scan64, (long long *)nullptr, (long long *)nullptr, n, st));
+    const char *what = "gem_mls_upsample";
+    int rc;
+    if ((rc = scratch_grow(m, S.key[0], N * 8, what)) || (rc = scratch_grow(m, S.key[1], N * 8, what)) ||
+        (rc = scratch_grow(m, S.idx[0], N * 4, what)) || (rc = scratch_grow(m, S.idx[1], N * 4, what)) ||
+        (rc = scratch_grow(m, S.spts, N * 16, what)) || (rc = scratch_grow(m, S.ukey, N * 8, what)) ||
+        (rc = scratch_grow(m, S.ucnt, N * 4, what)) || (rc = scratch_grow(m, S.uoff, N * 4, what)) ||
+        (rc = scratch_grow(m, S.nbr, N * 4, what)) || (rc = scratch_grow(m, S.ocnt, N * 8, what)) ||
+        (rc = scratch_grow(m, S.ooff, N * 8, what)) || (rc = scratch_grow(m, S.longs, N * 4, what)) ||
+        (rc = scratch_grow(m, S.temp, std::max(std::max(t_sort, t_rle), std::max(t_scan, t_scan64)), what)) ||
+        (rc = scratch_grow(m, S.acc, sizeof(MlsAcc), what)))
+        return rc;
+    const float4 *in = static_cast<const float4 *>(points32_device);
+    float4 *out = static_cast<float4 *>(out_points32_device);
+    MlsAcc *acc = S.acc.as<MlsAcc>();
+    u64 *key0 = S.key[0].as<u64>(), *key1 = S.key[1].as<u64>(), *ukey = S.ukey.as<u64>();
+    int *idx0 = S.idx[0].as<int>(), *idx1 = S.idx[1].as<int>(), *ucnt = S.ucnt.as<int>(), *uoff = S.uoff.as<int>();
+    int *nbr = S.nbr.as<int>(), *longs = S.longs.as<int>();
+    long long *ocnt = S.ocnt.as<long long>(), *ooff = S.ooff.as<long long>();
+    float4 *spts = S.spts.as<float4>();
+    size_t tcap = S.temp.cap;
+    MlsAcc h{};
+    h.mn[0] = h.mn[1] = h.mn[2] = 0xffffffffu;
+    GEM_CUDA(m, cudaMemcpyAsync(acc, &h, sizeof h, cudaMemcpyHostToDevice, st));
+    // the run-length encoding writes nruns <= n counts; the scan runs over all n, so the rest must be defined
+    GEM_CUDA(m, cudaMemsetAsync(ucnt, 0, N * sizeof(int), st));
+    const unsigned gb = (unsigned)((N + VOX_BLOCK - 1) / VOX_BLOCK), gq = (unsigned)((N + MLS_WARPS - 1) / MLS_WARPS);
+    GEM_LAUNCH(m, GEM_PROF_OTHER, k_mls_bounds<<<blocks_for(N, VOX_BLOCK, NUM_SMS * 8), VOX_BLOCK, 0, st>>>(in, n, acc));
+    GEM_LAUNCH(m, GEM_PROF_OTHER, k_mls_keys<<<gb, VOX_BLOCK, 0, st>>>(in, n, P, acc, key0, idx0));
+    GEM_CUDA(m, cudaGetLastError());
+    GEM_CUDA(m, cub::DeviceRadixSort::SortPairs(S.temp.p, tcap, key0, key1, idx0, idx1, n, 0, 64, st));
+    GEM_CUDA(m, cub::DeviceRunLengthEncode::Encode(S.temp.p, tcap, key1, ukey, ucnt, &acc->nruns, n, st));
+    GEM_CUDA(m, cub::DeviceScan::ExclusiveSum(S.temp.p, tcap, ucnt, uoff, n, st));
+    GEM_LAUNCH(m, GEM_PROF_OTHER, k_mls_stage<<<gb, VOX_BLOCK, 0, st>>>(in, n, idx1, spts));
+    GEM_LAUNCH(m, GEM_PROF_OTHER, k_mls_count<<<gq, MLS_BLOCK, 0, st>>>(in, n, P, acc, spts, ukey, uoff, ucnt, nbr, ocnt, longs));
+    GEM_CUDA(m, cudaGetLastError());
+    GEM_CUDA(m, cub::DeviceScan::ExclusiveSum(S.temp.p, tcap, ocnt, ooff, n, st));
+    // synchronisation 1: the output count (last offset + last count), the longest list and the number of long lists
+    long long tail[2] = {0, 0};
+    GEM_CUDA(m, cudaMemcpyAsync(&tail[0], ooff + (N - 1), sizeof(long long), cudaMemcpyDeviceToHost, st));
+    GEM_CUDA(m, cudaMemcpyAsync(&tail[1], ocnt + (N - 1), sizeof(long long), cudaMemcpyDeviceToHost, st));
+    GEM_CUDA(m, cudaMemcpyAsync(&h, acc, sizeof h, cudaMemcpyDeviceToHost, st));
+    GEM_CUDA(m, cudaStreamSynchronize(st));
+    r.count = tail[0] + tail[1];
+    // the long lists: persistent warps, each sorting in its own global slice of a power of two >= the longest list; as
+    // many warps as fit in 256 MiB, at least one block's worth
+    int slice = 32, lwarps = 0;
+    if (h.nlong > 0) {
+        while (slice < h.max_nb) slice <<= 1;
+        const size_t per = (size_t)slice * 8;
+        size_t w = std::max((size_t)MLS_WARPS, ((size_t)256 << 20) / per / MLS_WARPS * MLS_WARPS);
+        w = std::min(w, (size_t)NUM_SMS * 16);
+        w = std::min(w, ((size_t)h.nlong + MLS_WARPS - 1) / MLS_WARPS * MLS_WARPS);
+        lwarps = (int)w;
+        if ((rc = scratch_grow(m, S.lkeys, w * per, what))) return rc;
+    }
+    if (capacity == 0) { // a size query stops here: the fits are not run
+        r.processed = h.processed;
+        r.fitted = -1;
+        r.skipped = h.skipped;
+        r.max_neighbours = h.max_nb;
+        *info = r;
+        return GEM_OK;
+    }
+    if (r.count > 0) {
+        GEM_LAUNCH(m, GEM_PROF_OTHER, k_mls_fit<false><<<gq, MLS_BLOCK, 0, st>>>(in, n, P, acc, spts, ukey, uoff, ucnt, nbr, ooff, longs,
+                                                                                 nullptr, 0, out, capacity));
+        if (lwarps)
+            GEM_LAUNCH(m, GEM_PROF_OTHER, k_mls_fit<true><<<lwarps / MLS_WARPS, MLS_BLOCK, 0, st>>>(
+                                              in, n, P, acc, spts, ukey, uoff, ucnt, nbr, ooff, longs, S.lkeys.as<u64>(), slice, out, capacity));
+        GEM_CUDA(m, cudaGetLastError());
+    }
+    // synchronisation 2: the info
+    GEM_CUDA(m, cudaMemcpyAsync(&h, acc, sizeof h, cudaMemcpyDeviceToHost, st));
+    GEM_CUDA(m, cudaStreamSynchronize(st));
+    r.processed = h.processed;
+    r.fitted = h.fitted;
+    r.skipped = h.skipped;
+    r.max_neighbours = h.max_nb;
     *info = r;
     return GEM_OK;
 }

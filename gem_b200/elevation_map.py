@@ -615,6 +615,43 @@ class ElevationMap:
                                        C.byref(info)), self._h, "gem_voxel_grid")
         return out[:min(info.count, cap)], {k: getattr(info, k) for k, _ in _lib.GemVoxelGridInfo._fields_}
 
+    # -- the MLS densification of the dense_mapping signal (DESIGN.md f10) ------------------------------------------------
+    GEM_MLS = {"search_radius": 0.5, "sqr_gauss_param": 0.25, "polynomial_fit": True, "order": 5,
+               "upsampling": "random_uniform_density", "point_density": 1000, "seed": 0}   # pointcloudinterpolation's settings
+
+    def mls_upsample(self, points, params=None, out=None, info: bool = False):
+        """pointcloudinterpolation's pcl::MovingLeastSquares (ElevationMapping.cpp:1072-1118) over `points`, a contiguous
+        (n, 8) float32 CUDA tensor of PointXYZRGBICT records: the points MLS produces, which the node appends to the
+        submap.  params: a dict overriding GEM_MLS's entries (upsampling "none" or "random_uniform_density").  The records
+        go to `out` (a contiguous (k, 8) float32 CUDA tensor that must hold them all) or to a new tensor.  Returns the
+        (m, 8) tensor, or (tensor, {count, processed, fitted, skipped, max_neighbours}) with info=True"""
+        import torch
+        if not (_is_device(points) and points.dtype == torch.float32 and points.dim() == 2 and points.shape[1] == 8
+                and points.is_contiguous()):
+            raise ValueError("mls_upsample: points must be a contiguous (n, 8) float32 CUDA tensor")
+        if points.device.index != self._device_index():
+            raise ValueError(f"mls_upsample: the points are on {points.device}, the map on cuda:{self._device_index()}")
+        q = dict(self.GEM_MLS)
+        for k, v in (params or {}).items():
+            if k not in q:
+                raise ValueError(f"mls_upsample: unknown parameter {k!r}")
+            q[k] = v
+        if q["upsampling"] not in _lib.MLS_UPSAMPLING:
+            raise ValueError(f"mls_upsample: upsampling must be one of {list(_lib.MLS_UPSAMPLING)}")
+        p = _lib.GemMlsParams(float(q["search_radius"]), float(q["sqr_gauss_param"]), 1 if q["polynomial_fit"] else 0,
+                              int(q["order"]), _lib.MLS_UPSAMPLING[q["upsampling"]], int(q["point_density"]),
+                              int(q["seed"]) & 0xFFFFFFFFFFFFFFFF)
+        n = int(points.shape[0])
+        pin = _ptr(points) if n else None
+        torch.cuda.current_stream(points.device).synchronize()   # the library reads and writes on its own stream
+        st = _lib.GemMlsInfo()
+        check(self._lib.gem_mls_upsample(self._h, pin, n, C.byref(p), None, 0, C.byref(st)), self._h, "gem_mls_upsample")
+        rec = self._records_out(st.count, out, "mls_upsample")
+        if st.count:
+            check(self._lib.gem_mls_upsample(self._h, pin, n, C.byref(p), _ptr(rec), st.count, C.byref(st)), self._h,
+                  "gem_mls_upsample")
+        return (rec, {k: getattr(st, k) for k, _ in _lib.GemMlsInfo._fields_}) if info else rec
+
     def harvest_to_local_map(self, current_xy, shift_xy, records: bool = False):
         """the harvest of harvest_scrolled_out, upserted into the device-resident localMap_ (ElevationMapping.cpp:740-747).
         Returns the number of harvested records, or (records (n, 8) float32 host array, n) with records=True"""
@@ -648,9 +685,20 @@ class ElevationMap:
         """room for `records` harvested records now, so that later harvests do not allocate"""
         check(self._lib.gem_local_map_reserve(self._h, int(records)), self._h, "gem_local_map_reserve")
 
-    def cut_submap(self, out=None):
+    def cut_submap(self, out=None, dense: bool = False, seed: int = 0):
         """the submap of a keyframe cut (ElevationMapping.cpp:653-661): local_map_take() followed by
-        export_grid_cloud("shown"), in one (n, 8) float32 CUDA tensor; the local map is empty afterwards"""
+        export_grid_cloud("shown"), in one (n, 8) float32 CUDA tensor; the local map is empty afterwards.  With dense=True
+        (the dense_mapping signal, :656-657) the MLS points of the taken local map (mls_upsample with GEM's settings and
+        `seed`) come between the two: [local map, its MLS points, grid cloud], i.e. *out_pc + *grid_pc after
+        *input += dense; `out` is then not accepted (the size is known only after the fit)"""
+        if dense:
+            import torch
+            if out is not None:
+                raise ValueError("cut_submap: out is not accepted with dense=True")
+            local = self.local_map_take()
+            extra = self.mls_upsample(local, {"seed": seed})
+            grid = self.export_grid_cloud("shown")
+            return torch.cat([local, extra, grid])
         nl, ng = self.local_map_size(), self.grid_cloud_count("shown")
         rec = self._records_out(nl + ng, out, "cut_submap")
         self.local_map_take(out=rec[:nl])

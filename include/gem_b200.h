@@ -425,6 +425,64 @@ typedef struct gem_voxel_grid_info {
 int gem_voxel_grid(gem_map *m, const void *xyzi_device, int n, const gem_voxel_grid_params *p,
                    void *out_xyzi_device, int capacity, gem_voxel_grid_info *info);
 
+/* ---- the MLS densification of GEM's dense_mapping signal (pointcloudinterpolation, ElevationMapping.cpp:1072-1118;
+ *      DESIGN.md f10) ----
+ * gem_mls_upsample: pcl::MovingLeastSquares<PointXYZRGB, PointXYZRGB>::process of PCL 1.7.2 (performProcessing /
+ *   computeMLSPointNormal, KdTreeFLANN radius search, single-threaded) over n 32-byte PointXYZRGBICT records in device
+ *   memory (the layout of gem_local_map_take).  The output holds only the points MLS produces (mls.process's cloud); the
+ *   node appends them to the submap (*input += dense).  Unpinned: restated, PCL is not available.  DEFINED: fixed here
+ *   where the reference leaves it open.
+ *   M1 only x, y, z and the bgra word of a record are read.  DEFINED: a record whose x, y or z is not finite is nobody's
+ *      neighbour and produces nothing; it counts in skipped.
+ *   M2 neighbours: d2 = ((dx dx) + dy dy) + dz dz in float; j is a neighbour iff d2 <= (float)(r r) (DEFINED inclusive),
+ *      the query included, sorted by ascending d2, ties by ascending index (DEFINED), no cap; with fewer than 3
+ *      neighbours the point produces nothing.
+ *   M3 plane, in double and neighbour order: centroid (sequential sums, then / n), the non-normalised covariance in PCL's
+ *      update order, eigen33's smallest eigenvector (scaling, computeRoots with the computeRoots2 fallback, three row
+ *      cross products, the largest squared norm in PCL's if-chain order), d = -(n . centroid) with the dot
+ *      (a0b0 + a2b2) + (a1b1 + a3b3), point = q - (q . n + d) n.  3-vector dots left to right (DEFINED).  atan2, sin, cos
+ *      and exp are the library's own double functions (gem_mathd.h), within 2 ulp of glibc's.
+ *   M4 fit when polynomial_fit and n >= nr_coeff = (order + 1)(order + 2) / 2: de = p_j - point, d2f = (float)(de . de),
+ *      w = exp(-d2f / sqr_gauss_param), v_axis = n.unitOrthogonal(), u_axis = n x v_axis, (u, v, f) = de . (u_axis, v_axis,
+ *      n), monomials u^a v^b with the u power outer; A(a,b) = sum ((P(a) w) P(b)) (a >= b), rhs(a) = sum ((P(a) w) f),
+ *      sequential in neighbour order (DEFINED); left-looking Cholesky, forward and back substitution (DEFINED orders,
+ *      DESIGN.md f10).  DEFINED: a pivot that is not finite or not > 0, or a non-finite c0, fails the fit.  The Darboux
+ *      axes are set only when the fit is attempted (as in 1.7.2); otherwise they are zero.
+ *   M5 GEM_MLS_NONE: one output per processed point, point + c0 n when fitted, else point.
+ *   M6 GEM_MLS_RANDOM_UNIFORM_DENSITY: k = (int)floor(point_density / 2.0 / n); k <= 0: M5's output; else k samples, u
+ *      then v drawn as floats in [-r/2, r/2), again while u u + v v > r r / 4 (double); sample = point + u u_axis +
+ *      v v_axis (+ height(u, v) n when fitted).  DEFINED generator: draw j of input point i is splitmix64(seed ^ (i << 32)
+ *      ^ j), the float lo + (float)(x >> 40) 2^-24 (hi - lo) in float, hi = (float)(r / 2), lo = -hi; a rejected pair
+ *      consumes its two draws.  (The reference seeds boost::mt19937 with time(0), so it differs from run to run.)
+ *   M7 records {(float)x, (float)y, (float)z, 1, the query's b g r with a = 0xff, the query's covariance, intensity and
+ *      travers} (DEFINED: the alpha and the last three, uninitialised in the reference), in input order, samples in
+ *      draw order.
+ *   M8 info: count (output records; min(count, capacity) are written), processed (n >= 3), fitted, skipped (n < 3 or
+ *      non-finite), max_neighbours (the longest list).
+ *   capacity = 0 is a size query: it stops before the fits and reports fitted = -1, the other fields as a full call.
+ *   Host-synchronous (two synchronisations); works on any handle; neither reads nor modifies the map.  Errors, which
+ *   return GEM_ERR_INVALID and write nothing: overlapping input and output, n < 0, capacity < 0, NULL pointers with a
+ *   non-zero size, a radius or Gauss parameter that is not finite or not > 0, an order outside 1..5, an unknown upsampling
+ *   id, point_density < 0.  Scratch (about 90 bytes per input point, plus the sort slices of lists longer than 512) is
+ *   handle-owned and grown on demand before anything is written: a failed growth is GEM_ERR_NOMEM.  sqr_gauss_param and
+ *   search_radius are separate, as in PCL (GEM sets sqr_gauss_param = search_radius^2). */
+enum { GEM_MLS_NONE = 0, GEM_MLS_RANDOM_UNIFORM_DENSITY = 1 };
+typedef struct gem_mls_params {
+    double search_radius;        /* 0.5 in GEM                                   */
+    double sqr_gauss_param;      /* 0.25 = search_radius^2                        */
+    int polynomial_fit;          /* 1                                             */
+    int order;                   /* 5; 1..5 accepted                              */
+    int upsampling;              /* GEM_MLS_*                                     */
+    int point_density;           /* desired_num_points_in_radius, 1000 in GEM     */
+    unsigned long long seed;     /* the random draws, item M6                     */
+} gem_mls_params;
+typedef struct gem_mls_info {
+    long long count;             /* output records (min(count, capacity) written) */
+    int processed, fitted, skipped, max_neighbours;
+} gem_mls_info;
+int gem_mls_upsample(gem_map *m, const void *points32_device, int n, const gem_mls_params *p,
+                     void *out_points32_device, long long capacity, gem_mls_info *info);
+
 /* raw layer access (row-major L*L, float or int32 for the colour ids) for tests and
  * checkpoint/restore (the dead G_get_mapinfo/G_set_mapinfo of gpu.cu:457-475). */
 int gem_get_layer(gem_map *m, int layer, void *host_out);

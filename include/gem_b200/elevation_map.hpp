@@ -314,6 +314,29 @@ class ElevationMap {
         check(gem_voxel_grid(h_, xyzi_device, (int)n, &p, out_device, (int)capacity, &info), "gem_voxel_grid");
         return info;
     }
+    // pointcloudinterpolation's MovingLeastSquares (GEM's dense_mapping signal, ElevationMapping.cpp:1072-1118; DESIGN.md
+    // f10) over n PointXYZRGBICT records in device memory: min(count, capacity) new records go to out_device, which must
+    // not overlap the input (capacity 0 is a size query).  gemMlsParams() is GEM's setting.
+    static gem_mls_params gemMlsParams(unsigned long long seed = 0)
+    {
+        gem_mls_params p{};
+        p.search_radius = 0.5;
+        p.sqr_gauss_param = 0.25;
+        p.polynomial_fit = 1;
+        p.order = 5;
+        p.upsampling = GEM_MLS_RANDOM_UNIFORM_DENSITY;
+        p.point_density = 1000;
+        p.seed = seed;
+        return p;
+    }
+    gem_mls_info mlsUpsample(const void *points32_device, size_t n, const gem_mls_params &p, void *out_device, size_t capacity)
+    {
+        if (n > (size_t)std::numeric_limits<int>::max() || capacity > (size_t)std::numeric_limits<long long>::max())
+            throw std::runtime_error("mlsUpsample: more than INT_MAX points");
+        gem_mls_info info{};
+        check(gem_mls_upsample(h_, points32_device, (int)n, &p, out_device, (long long)capacity, &info), "gem_mls_upsample");
+        return info;
+    }
     int harvestToLocalMap(const float current[2], const float shift[2], std::vector<PointXYZRGBICT> *visual = nullptr)
     {
         int n = 0;
@@ -337,6 +360,24 @@ class ElevationMap {
         localMapTake(points32_device, (size_t)nl);
         gridCloud(GEM_GRID_SHOWN, (char *)points32_device + (size_t)nl * sizeof(PointXYZRGBICT), (size_t)ng);
         return nl + ng;
+    }
+    // cutSubmap with the dense_mapping signal (:656-661): [local map, its MLS points (mlsUpsample with p), grid cloud] in
+    // one device buffer.  The local map is taken into the front of the buffer and densified from there, so `capacity` must
+    // hold the result: when it does not, nothing more is written, the local map stays taken (it is at the front of the
+    // buffer) and the size the buffer needs is returned.
+    long long cutSubmap(void *points32_device, size_t capacity, bool dense, const gem_mls_params &p = gemMlsParams())
+    {
+        if (!dense) return cutSubmap(points32_device, capacity);
+        const int nl = localMapTake(nullptr, 0), ng = gridCloud(GEM_GRID_SHOWN, nullptr, 0);
+        if ((size_t)nl > capacity) return (long long)nl + ng; // nothing taken
+        localMapTake(points32_device, (size_t)nl);
+        char *base = (char *)points32_device;
+        const size_t rest = capacity - (size_t)nl;
+        const gem_mls_info info = mlsUpsample(base, (size_t)nl, p, base + (size_t)nl * sizeof(PointXYZRGBICT), rest);
+        const long long total = (long long)nl + info.count + ng;
+        if ((unsigned long long)total > capacity) return total;
+        gridCloud(GEM_GRID_SHOWN, base + ((size_t)nl + (size_t)info.count) * sizeof(PointXYZRGBICT), (size_t)ng);
+        return total;
     }
     // Loop closure (ElevationMapping::updateGlobalMap, ElevationMapping.cpp:773-905), on device-resident submaps of
     // PointXYZRGBICT records: re-pose a submap (:805), and one pass of the pairwise fuse loop (:847-883) -- both clouds
