@@ -314,6 +314,11 @@ __device__ __forceinline__ void bin_one(Cell *cells, const BinScratch &sc, int k
 
 constexpr int BIN_PEER_MAX_BLOCKS = NUM_SMS * 8; // one wave of 256-thread blocks; a block takes sub-buckets blockIdx.x + q * gridDim.x
 constexpr int BIN_PEER_MAX_PER_BLOCK = 32;
+// k_bin_peer stages a block's sub-bucket counts in one round of BIN_PEER_MAX_PER_BLOCK.  What bounds nsub = world * nblk is
+// gem_tiled_attach's world * cap <= max_points, and gem_create caps max_points at the fold's 2^22 point indices: at most
+// 2^22 / 256 = 16384 sub-buckets, 16 per block.  A wider fold index must stage the counts in rounds first.
+static_assert((1 << FOLD_INDEX_BITS) / ROUTE_BLOCK <= BIN_PEER_MAX_BLOCKS * BIN_PEER_MAX_PER_BLOCK,
+              "k_bin_peer: more sub-buckets than one round of staged counts holds");
 
 __global__ void __launch_bounds__(ROUTE_BLOCK)
 k_bin_peer(MapGeom g, MapLayers ml, BinScratch sc, const uint4 *rec, const float *inten, const int *cnt, int nsub, const int *flags,
@@ -330,7 +335,7 @@ k_bin_peer(MapGeom g, MapLayers ml, BinScratch sc, const uint4 *rec, const float
         } while (v < step);
     }
     __syncthreads();
-    const int nmine = (nsub - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x; // <= BIN_PEER_MAX_PER_BLOCK (host)
+    const int nmine = (nsub - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x; // <= BIN_PEER_MAX_PER_BLOCK (static_assert above)
     if ((int)threadIdx.x < nmine) s_cnt[threadIdx.x] = cnt[blockIdx.x + threadIdx.x * gridDim.x];
     __syncthreads();
     for (int q = 0; q < nmine; q++) {
