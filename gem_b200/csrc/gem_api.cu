@@ -2610,8 +2610,8 @@ int gem_refuse_submaps(gem_map *m, void *new_points32, int *n_new, void *old_poi
     SubPoint *pn = (SubPoint *)new_points32, *po = (SubPoint *)old_points32;
     if (nn) GEM_LAUNCH(m, GEM_PROF_OTHER, k_hash_insert<<<blocks_for((size_t)nn, 256, 1 << 30), 256, 0, m->stream>>>(pn, nn, resolution, kn, fn, (unsigned)(cn - 1)));
     if (no) GEM_LAUNCH(m, GEM_PROF_OTHER, k_hash_insert<<<blocks_for((size_t)no, 256, 1 << 30), 256, 0, m->stream>>>(po, no, resolution, ko, fo, (unsigned)(co - 1)));
-    const int nmax = nn > no ? nn : no;
-    if (nmax) GEM_LAUNCH(m, GEM_PROF_OTHER, k_refuse_pair<<<blocks_for((size_t)nmax, 256, 1 << 30), 256, 0, m->stream>>>(pn, nn, po, no, resolution, kn, fn, (unsigned)(cn - 1), ko, fo, (unsigned)(co - 1), keepn, keepo, compat, cnts));
+    if (no) GEM_LAUNCH(m, GEM_PROF_OTHER, k_refuse_keep<<<blocks_for((size_t)no, 256, 1 << 30), 256, 0, m->stream>>>(po, no, resolution, ko, fo, (unsigned)(co - 1), keepo));
+    if (nn) GEM_LAUNCH(m, GEM_PROF_OTHER, k_refuse_pair<<<blocks_for((size_t)nn, 256, 1 << 30), 256, 0, m->stream>>>(pn, nn, po, resolution, kn, fn, (unsigned)(cn - 1), ko, fo, (unsigned)(co - 1), keepn, compat, cnts));
     GEM_LAUNCH(m, GEM_PROF_OTHER, k_compact_points<<<1, 1024, 0, m->stream>>>(pn, keepn, nn, outn, cnts + 1));
     GEM_LAUNCH(m, GEM_PROF_OTHER, k_compact_points<<<1, 1024, 0, m->stream>>>(po, keepo, no, outo, cnts + 2));
     int h[4] = {0, 0, 0, 0};

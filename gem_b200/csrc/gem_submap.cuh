@@ -74,25 +74,36 @@ __device__ __forceinline__ int hash_find(const unsigned long long *keys, const i
     }
 }
 
-// One thread per point of the NEW submap (the neighbour, "out_new"); `old` is submap i ("out_old").  keep_*[i] = 1 iff
-// point i is the first of its cell (those are the points the hash maps hold and localHashtoPointCloud emits).
+// One thread per point of the OLD submap (submap i, "out_old"), launched before k_refuse_pair: keep_o[i] = 1 iff point i
+// is the first of its cell (the point the hash map holds and localHashtoPointCloud emits); its position becomes the
+// cell's (:1129-1130).  A launch of its own because k_refuse_pair overwrites whole old records with the cell's position,
+// and a cell centre does not always key to its own cell: with res = 2^m, the coordinate 2^(m+23) + res is the only float
+// of its cell, and its centre rounds (a tie, to even) to 2^(m+23), which lies in the cell below.  So the old side reads
+// only unmodified positions.
+__global__ void __launch_bounds__(256)
+k_refuse_keep(SubPoint *po, int no, double res, const unsigned long long *ko, const int *fo, unsigned mo, unsigned char *keep_o)
+{
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= no) return;
+    float rx, ry;
+    const unsigned long long k = cell_key(po[i].x, po[i].y, res, rx, ry);
+    const bool nan = rx != rx || ry != ry;
+    const bool first = nan || hash_find(ko, fo, mo, k) == i;
+    keep_o[i] = first ? 1 : 0;
+    if (first) { po[i].x = rx; po[i].y = ry; po[i].w = 1.0f; }
+}
+
+// One thread per point of the NEW submap (the neighbour, "out_new"); `old` is submap i ("out_old"), its keep flags and
+// positions already set by k_refuse_keep.  keep_n[i] = 1 iff point i is the first of its cell.
 // ElevationMapping.cpp:847-870, with every cell present in both maps fused exactly ONCE (DEFINITION: the reference
 // erases and re-inserts while iterating, so what it visits twice depends on libstdc++'s bucket order).
 // compat != 0: the fused values as the reference's expression evaluates (C operator precedence, :862-863);
 // compat == 0: the weighting the expression was written for.
 __global__ void __launch_bounds__(256)
-k_refuse_pair(SubPoint *pn, int nn, SubPoint *po, int no, double res, const unsigned long long *kn, const int *fn, unsigned mn,
-              const unsigned long long *ko, const int *fo, unsigned mo, unsigned char *keep_n, unsigned char *keep_o, int compat, int *count)
+k_refuse_pair(SubPoint *pn, int nn, SubPoint *po, double res, const unsigned long long *kn, const int *fn, unsigned mn,
+              const unsigned long long *ko, const int *fo, unsigned mo, unsigned char *keep_n, int compat, int *count)
 {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < no) { // old map: which points it holds; their position becomes the cell's (localHashtoPointCloud :1129-1130)
-        float rx, ry;
-        const unsigned long long k = cell_key(po[i].x, po[i].y, res, rx, ry);
-        const bool nan = rx != rx || ry != ry;
-        const bool first = nan || hash_find(ko, fo, mo, k) == i;
-        keep_o[i] = first ? 1 : 0;
-        if (first) { po[i].x = rx; po[i].y = ry; po[i].w = 1.0f; }
-    }
     if (i >= nn) return;
     float rx, ry;
     const unsigned long long k = cell_key(pn[i].x, pn[i].y, res, rx, ry);
