@@ -13,6 +13,8 @@ ERR_NAMES = {0: "GEM_OK", 1: "GEM_ERR_INVALID", 2: "GEM_ERR_CUDA", 3: "GEM_ERR_N
 
 SENSOR_LASER = 0
 SENSOR_STRUCTURED_LIGHT = 1
+SENSOR_STEREO = 2
+SENSOR_PERFECT = 3
 
 GRID_SOURCES = {"shown": 0, "snapshot": 1}   # GEM_GRID_SHOWN / GEM_GRID_SNAPSHOT
 
@@ -39,6 +41,7 @@ class GemSensorModel(C.Structure):
         ("normal_factor_a", C.c_double), ("normal_factor_b", C.c_double), ("normal_factor_c", C.c_double),
         ("normal_factor_d", C.c_double), ("normal_factor_e", C.c_double), ("lateral_factor", C.c_double),
         ("cutoff_min_depth", C.c_double), ("cutoff_max_depth", C.c_double),
+        ("stereo_p", C.c_double * 5), ("depth_to_disparity_factor", C.c_double), ("cloud_width", C.c_int),
     ]
 
 

@@ -155,6 +155,8 @@ __device__ __forceinline__ int next_chunk(const uint4 *chunk) { return (int)chun
 // point sources of the bin kernel
 // ---------------------------------------------------------------------------------------
 enum { SRC_XYZI = 0, SRC_SOA = 1, SRC_PCL32 = 2, SRC_KEYS = 3, SRC_RECORDS = 4 };
+// or-ed into SRC_XYZI / SRC_SOA / SRC_PCL32: the instantiation that runs every sensor model (transform_point<true>)
+constexpr int SRC_ANY_MODEL = 8;
 
 struct RouteRec { // 20 bytes on the wire between tiles (gem_route.cuh)
     int gkey;     // global geographic linear index gx*L+gy
@@ -195,11 +197,21 @@ template <int SRC>
 __device__ __forceinline__ PointOut bin_source_point(const MapGeom &g, const FrameParams &f, const BinSource &in, int i,
                                                      const SegTable *segs, const FrameParams *frames)
 {
+    constexpr bool ANY = (SRC & SRC_ANY_MODEL) != 0;
+    constexpr int S = SRC & ~SRC_ANY_MODEL;
     PointOut o;
     o.key = -1; o.geo = -1; o.h = -1.0f; o.hv = -1.0f; o.rgbf = 0u;
-    if (SRC == SRC_XYZI) {
+    if (S == SRC_XYZI) {
         const float4 p = ld_stream_f4(in.xyzi + i);
-        const PtRes r = segs ? transform_point(g, frames[find_segment(*segs, i)], p.x, p.y, p.z) : transform_point(g, f, p.x, p.y, p.z);
+        PtRes r;
+        if (!ANY) {
+            r = segs ? transform_point(g, frames[find_segment(*segs, i)], p.x, p.y, p.z) : transform_point(g, f, p.x, p.y, p.z);
+        } else if (segs) { // the index restarts with every segment's cloud (idx0 = -offsets[s])
+            const FrameParams &fs = frames[find_segment(*segs, i)];
+            r = transform_point<true>(g, fs, p.x, p.y, p.z, fs.idx0 + i);
+        } else {
+            r = transform_point<true>(g, f, p.x, p.y, p.z, f.idx0 + i);
+        }
         if (r.ingrid) { o.key = local_key(g, r.gx, r.gy); o.geo = g.tiled ? o.key : r.gx * g.L + r.gy; }
         o.h = r.h; o.hv = r.hv;
         uint32_t rgb = 0u;
@@ -208,23 +220,23 @@ __device__ __forceinline__ PointOut bin_source_point(const MapGeom &g, const Fra
             rgb = pack_rgb(c.x, c.y, c.z);
         }
         o.rgbf = with_colour_flag(rgb, p.w);
-    } else if (SRC == SRC_PCL32) {
+    } else if (S == SRC_PCL32) {
         const float4 p = ld_stream_f4(in.pcl + 2 * (size_t)i);
         const float4 q = ld_stream_f4(in.pcl + 2 * (size_t)i + 1); // {rgb(b,g,r,a bytes), covariance, intensity, travers}
-        const PtRes r = transform_point(g, f, p.x, p.y, p.z);
+        const PtRes r = transform_point<ANY>(g, f, p.x, p.y, p.z, f.idx0 + i);
         if (r.ingrid) { o.key = local_key(g, r.gx, r.gy); o.geo = g.tiled ? o.key : r.gx * g.L + r.gy; }
         o.h = r.h; o.hv = r.hv;
         const uint32_t bgra = __float_as_uint(q.x);
         o.rgbf = with_colour_flag(pack_rgb((bgra >> 16) & 255, (bgra >> 8) & 255, bgra & 255), q.z);
-    } else if (SRC == SRC_SOA) {
-        const PtRes r = transform_point(g, f, in.x[i], in.y[i], in.z[i]);
+    } else if (S == SRC_SOA) {
+        const PtRes r = transform_point<ANY>(g, f, in.x[i], in.y[i], in.z[i], f.idx0 + i);
         if (r.ingrid) { o.key = local_key(g, r.gx, r.gy); o.geo = g.tiled ? o.key : r.gx * g.L + r.gy; }
         o.h = r.h; o.hv = r.hv;
         if (in.key_out) in.key_out[i] = o.key;
         if (in.h_out) in.h_out[i] = r.h;
         if (in.hv_out) in.hv_out[i] = r.hv;
         if (in.xt_out) { in.xt_out[i] = r.xt; in.yt_out[i] = r.yt; }
-    } else if (SRC == SRC_KEYS) {
+    } else if (S == SRC_KEYS) {
         int key = in.key_in[i];
         if (key < 0 || key >= in.ncells) key = -1; // no G_fuse thread has such a map_index
         o.key = key;

@@ -62,6 +62,7 @@ struct TiledState { // gem_tiled_attach
     cudaGraph_t graph = nullptr;
     cudaGraphExec_t exec = nullptr;
     cudaGraphNode_t long_node = nullptr, fold_node = nullptr, route_node = nullptr, bin_node = nullptr;
+    const void *route_func = nullptr; // the route kernel the graph was built with (k_route_peer or k_route_peer_any)
 };
 
 struct OctBuf { // a device scratch buffer (octree, costmap and voxel-grid calls): grows on demand, never shrinks
@@ -309,7 +310,16 @@ FrameParams make_frame(const gem_frame *f)
     p.lat = f->sensor.lateral_factor;
     p.cut_lo = (float)f->sensor.cutoff_min_depth; // pcl::PassThrough::setFilterLimits takes floats
     p.cut_hi = (float)f->sensor.cutoff_max_depth;
+    for (int i = 0; i < 5; i++) p.sp[i] = f->sensor.stereo_p[i];
+    p.dtd = f->sensor.depth_to_disparity_factor;
+    p.width = f->sensor.cloud_width;
+    p.idx0 = 0;
     return p;
+}
+// a sensor model the kernels implement: an unknown type must not run as a laser
+bool sensor_ok(const gem_sensor_model &s)
+{
+    return s.type >= GEM_SENSOR_LASER && s.type <= GEM_SENSOR_PERFECT && s.cloud_width >= 0;
 }
 
 size_t region_cells(const gem_map *m, const RegionOp &r)
@@ -481,8 +491,12 @@ void pend_all_floor(gem_map *m)
 inline int points_per_thread(int n) { return n >= 600000 ? 4 : (n >= 250000 ? 2 : 1); }
 
 typedef void (*BinKernel)(MapGeom, MapLayers, FrameParams, BinSource, int, BinScratch, const RegionOps, int, const SegTable, const FrameParams *);
-template <int SRC> BinKernel bin_kernel(int U)
+// any: a frame uses the stereo or perfect model -> the every-model instantiation, one point per thread
+template <int SRC> BinKernel bin_kernel(int U, bool any)
 {
+    if constexpr (SRC == SRC_XYZI || SRC == SRC_SOA || SRC == SRC_PCL32) {
+        if (any) return k_bin<SRC | SRC_ANY_MODEL, 1>;
+    }
     if (SRC == SRC_XYZI || SRC == SRC_RECORDS) {
         if (U == 4) return k_bin<SRC, 4>;
         if (U == 2) return k_bin<SRC, 2>;
@@ -607,9 +621,10 @@ int launch_frame_graph(gem_map *m, BinKernel bk, void **bin_args, int bin_grid, 
 // on the handle's stream.  pipelined == true: the bin kernel of this call is issued together with the FOLD OF THE
 // PREVIOUS pipelined call (which also carries the row / column clears this call's Move decided), and this call's
 // fold stays pending until the next call or until anything observes the map (drain).
+// any_segment: some segment of a multi-cloud call uses the stereo or perfect model (fp is segment 0's frame)
 template <int SRC>
 int enqueue_add(gem_map *m, const BinSource &in, const FoldSrc &fsrc, int n, const FrameParams &fp, const SegTable *segs,
-                const FrameParams *frames, bool pipelined, bool do_fuse, bool do_lowest)
+                const FrameParams *frames, bool pipelined, bool do_fuse, bool do_lowest, bool any_segment = false)
 {
     int rc;
     if (m->profiling || m->pipe_mode == 0) pipelined = false; // per-kernel event timing needs the serial schedule
@@ -627,8 +642,9 @@ int enqueue_add(gem_map *m, const BinSource &in, const FoldSrc &fsrc, int n, con
     sc.ctr_next = m->ctr[(c + 1) % 3];
     sc.par = par;
     sc.stamps = m->d_stamps;
-    const int U = points_per_thread(n);
-    BinKernel bk = bin_kernel<SRC>(U);
+    const bool any = any_segment || any_model(fp);
+    const int U = any ? 1 : points_per_thread(n);
+    BinKernel bk = bin_kernel<SRC>(U, any);
     const int pb = blocks_for((size_t)(n + U - 1) / U, ADD_BLOCK, NUM_SMS * 16);
     SegTable st{};
     if (segs) st = *segs;
@@ -1043,16 +1059,17 @@ static BinSource xyzi_source(const void *xyzi, const void *rgba, int off)
 
 int gem_add_points(gem_map *m, const void *xyzi, const void *rgba, int n, const gem_frame *frame)
 {
-    if (!m || !frame || n < 0 || (n > 0 && !xyzi)) return fail(m, GEM_ERR_INVALID, "gem_add_points: bad argument");
+    if (!m || !frame || n < 0 || (n > 0 && !xyzi) || !sensor_ok(frame->sensor)) return fail(m, GEM_ERR_INVALID, "gem_add_points: bad argument");
     Lock lk(m->mu);
     SetDev sd(m->dev);
     int rc = GEM_OK;
-    const FrameParams fp = make_frame(frame);
+    FrameParams fp = make_frame(frame);
     memset(&m->stats, 0, sizeof m->stats);
     if (n == 0) return flush_all_pending(m);
     for (int off = 0; off < n; off += m->P) {
         const int cn = (n - off < m->P) ? (n - off) : m->P;
         const BinSource in = xyzi_source(xyzi, rgba, off);
+        fp.idx0 = off; // the stereo model indexes the caller's cloud
         const FoldSrc fs{in.xyzi ? (const char *)in.xyzi + 12 : nullptr, 16};
         if ((rc = enqueue_add<SRC_XYZI>(m, in, fs, cn, fp, nullptr, nullptr, false, true, true))) return rc;
         if (n > m->P && (rc = read_counters(m, cn, true))) return rc; // chunked: keep totals
@@ -1063,17 +1080,18 @@ int gem_add_points(gem_map *m, const void *xyzi, const void *rgba, int n, const 
 
 int gem_add_points_host(gem_map *m, const void *xyzi, const void *rgba, int n, const gem_frame *frame)
 {
-    if (!m || !frame || n < 0 || (n > 0 && !xyzi)) return fail(m, GEM_ERR_INVALID, "gem_add_points_host: bad argument");
+    if (!m || !frame || n < 0 || (n > 0 && !xyzi) || !sensor_ok(frame->sensor)) return fail(m, GEM_ERR_INVALID, "gem_add_points_host: bad argument");
     Lock lk(m->mu);
     SetDev sd(m->dev);
     int rc = ensure_host_staging(m);
     if (rc) return rc;
-    const FrameParams fp = make_frame(frame);
+    FrameParams fp = make_frame(frame);
     memset(&m->stats, 0, sizeof m->stats);
     if (n == 0) { if ((rc = flush_all_pending(m))) return rc; return gem_sync(m); }
     if ((rc = drain(m))) return rc; // the staging buffers may still feed a deferred fold
     for (int off = 0; off < n; off += m->P) {
         const int cn = (n - off < m->P) ? (n - off) : m->P;
+        fp.idx0 = off;
         GEM_CUDA(m, cudaMemcpyAsync(m->d_xyzi, (const float4 *)xyzi + off, (size_t)cn * 16, cudaMemcpyHostToDevice, m->stream));
         if (rgba)
             GEM_CUDA(m, cudaMemcpyAsync(m->d_rgba, (const uchar4 *)rgba + off, (size_t)cn * 4, cudaMemcpyHostToDevice, m->stream));
@@ -1087,7 +1105,7 @@ int gem_add_points_host(gem_map *m, const void *xyzi, const void *rgba, int n, c
 
 int gem_add_points_stream(gem_map *m, const void *xyzi, const void *rgba, int n, const gem_frame *frame)
 {
-    if (!m || !frame || n < 0 || (n > 0 && !xyzi)) return fail(m, GEM_ERR_INVALID, "gem_add_points_stream: bad argument");
+    if (!m || !frame || n < 0 || (n > 0 && !xyzi) || !sensor_ok(frame->sensor)) return fail(m, GEM_ERR_INVALID, "gem_add_points_stream: bad argument");
     if (n > m->P) return fail(m, GEM_ERR_INVALID, "gem_add_points_stream: n exceeds max_points (use gem_add_points)");
     Lock lk(m->mu);
     SetDev sd(m->dev);
@@ -1111,6 +1129,11 @@ int gem_add_points_multi(gem_map *m, const void *xyzi, const void *rgba, int n_s
     if (offsets[0] != 0 || n < 0 || n > m->P) return fail(m, GEM_ERR_INVALID, "gem_add_points_multi: offsets must start at 0 and n <= max_points");
     for (int s = 0; s < n_segments; s++)
         if (offsets[s + 1] < offsets[s]) return fail(m, GEM_ERR_INVALID, "gem_add_points_multi: offsets not monotone");
+    bool any = false;
+    for (int s = 0; s < n_segments; s++) {
+        if (!sensor_ok(frames[s].sensor)) return fail(m, GEM_ERR_INVALID, "gem_add_points_multi: bad sensor model");
+        any = any || frames[s].sensor.type == GEM_SENSOR_STEREO || frames[s].sensor.type == GEM_SENSOR_PERFECT;
+    }
     Lock lk(m->mu);
     SetDev sd(m->dev);
     int rc = GEM_OK;
@@ -1125,7 +1148,10 @@ int gem_add_points_multi(gem_map *m, const void *xyzi, const void *rgba, int n_s
     SegTable st{};
     st.n = n_segments;
     for (int s = 0; s <= n_segments; s++) st.off[s] = offsets[s];
-    for (int s = 0; s < n_segments; s++) hf[s] = make_frame(&frames[s]);
+    for (int s = 0; s < n_segments; s++) {
+        hf[s] = make_frame(&frames[s]);
+        hf[s].idx0 = -offsets[s]; // every segment is a cloud of its own
+    }
     GEM_CUDA(m, cudaMemcpyAsync(df, hf, (size_t)n_segments * sizeof(FrameParams), cudaMemcpyHostToDevice, m->stream));
     GEM_CUDA(m, cudaEventRecord(m->ev_frames[slot], m->stream));
     // GEM_B200_PIPE=stream: the steady-state bin runs on the front stream, which waits only for the fold that last used
@@ -1134,7 +1160,7 @@ int gem_add_points_multi(gem_map *m, const void *xyzi, const void *rgba, int n_s
     const BinSource in = xyzi_source(xyzi, rgba, 0);
     const FoldSrc fs{in.xyzi ? (const char *)in.xyzi + 12 : nullptr, 16};
     // pipelined like gem_add_points_stream: consecutive multi-sensor steps overlap bin(i+1) with fold(i)
-    if ((rc = enqueue_add<SRC_XYZI>(m, in, fs, n, hf[0], &st, df, true, true, true))) return rc;
+    if ((rc = enqueue_add<SRC_XYZI>(m, in, fs, n, hf[0], &st, df, true, true, true, any))) return rc;
     memset(&m->stats, 0, sizeof m->stats);
     m->stats.points_in = n;
     return GEM_OK;
@@ -1142,7 +1168,7 @@ int gem_add_points_multi(gem_map *m, const void *xyzi, const void *rgba, int n_s
 
 int gem_add_points_host_async(gem_map *m, const void *xyzi, const void *rgba, int n, const gem_frame *frame)
 {
-    if (!m || !frame || n < 0 || (n > 0 && !xyzi)) return fail(m, GEM_ERR_INVALID, "gem_add_points_host_async: bad argument");
+    if (!m || !frame || n < 0 || (n > 0 && !xyzi) || !sensor_ok(frame->sensor)) return fail(m, GEM_ERR_INVALID, "gem_add_points_host_async: bad argument");
     if (n > m->P) return fail(m, GEM_ERR_INVALID, "gem_add_points_host_async: n exceeds max_points (use gem_add_points_host)");
     Lock lk(m->mu);
     SetDev sd(m->dev);
@@ -1188,17 +1214,18 @@ int gem_add_points_host_async(gem_map *m, const void *xyzi, const void *rgba, in
 
 int gem_add_cloud_pcl_host(gem_map *m, const void *pts, int n, const gem_frame *frame)
 {
-    if (!m || !frame || n < 0 || (n > 0 && !pts)) return fail(m, GEM_ERR_INVALID, "gem_add_cloud_pcl_host: bad argument");
+    if (!m || !frame || n < 0 || (n > 0 && !pts) || !sensor_ok(frame->sensor)) return fail(m, GEM_ERR_INVALID, "gem_add_cloud_pcl_host: bad argument");
     Lock lk(m->mu);
     SetDev sd(m->dev);
     int rc = ensure_pcl_staging(m);
     if (rc) return rc;
-    const FrameParams fp = make_frame(frame);
+    FrameParams fp = make_frame(frame);
     memset(&m->stats, 0, sizeof m->stats);
     if (n == 0) { if ((rc = flush_all_pending(m))) return rc; return gem_sync(m); }
     if ((rc = drain(m))) return rc;
     for (int off = 0; off < n; off += m->P) {
         const int cn = (n - off < m->P) ? (n - off) : m->P;
+        fp.idx0 = off;
         GEM_CUDA(m, cudaMemcpyAsync(m->d_pcl, (const char *)pts + (size_t)off * 32, (size_t)cn * 32, cudaMemcpyHostToDevice, m->stream));
         BinSource in{};
         in.pcl = (const float4 *)m->d_pcl;
@@ -1213,14 +1240,14 @@ int gem_add_cloud_pcl_host(gem_map *m, const void *pts, int n, const gem_frame *
 int gem_process_points(gem_map *m, int *map_index, const float *x, const float *y, const float *z, float *var,
                        float *x_ts, float *y_ts, float *z_ts, int n, const gem_frame *frame)
 {
-    if (!m || !frame || n < 0 || (n > 0 && (!x || !y || !z)))
+    if (!m || !frame || n < 0 || (n > 0 && (!x || !y || !z)) || !sensor_ok(frame->sensor))
         return fail(m, GEM_ERR_INVALID, "gem_process_points: bad argument");
     if (m->geom.tiled) return fail(m, GEM_ERR_INVALID, "gem_process_points: not available on tiled handles");
     Lock lk(m->mu);
     SetDev sd(m->dev);
     int rc = ensure_compat_staging(m);
     if (rc) return rc;
-    const FrameParams fp = make_frame(frame);
+    FrameParams fp = make_frame(frame);
     memset(&m->stats, 0, sizeof m->stats);
     if ((rc = drain(m))) return rc;
     // Process_points does not fuse: clears/floors stay pending (they are handed to the bin kernel only by fusing calls)
@@ -1229,6 +1256,7 @@ int gem_process_points(gem_map *m, int *map_index, const float *x, const float *
     for (int off = 0; off < n && rc == GEM_OK; off += m->P) {
         const int cn = (n - off < m->P) ? (n - off) : m->P;
         const size_t b = (size_t)cn * 4;
+        fp.idx0 = off;
         cudaError_t e = cudaMemcpyAsync(m->d_x, x + off, b, cudaMemcpyHostToDevice, m->stream);
         if (e == cudaSuccess) e = cudaMemcpyAsync(m->d_y, y + off, b, cudaMemcpyHostToDevice, m->stream);
         if (e == cudaSuccess) e = cudaMemcpyAsync(m->d_z, z + off, b, cudaMemcpyHostToDevice, m->stream);
@@ -2511,7 +2539,7 @@ int gem_host_free(void *p) { return cudaFreeHost(p) == cudaSuccess ? GEM_OK : GE
 int gem_route_points(gem_map *m, const void *xyzi, const void *rgba, int n, const gem_frame *frame, int tiles_r,
                      int tiles_c, void *rec_out, int *counts_out, int bucket_stride)
 {
-    if (!m || !frame || n < 0 || tiles_r < 1 || tiles_c < 1 || !rec_out || !counts_out || (n > 0 && !xyzi))
+    if (!m || !frame || n < 0 || tiles_r < 1 || tiles_c < 1 || !rec_out || !counts_out || (n > 0 && !xyzi) || !sensor_ok(frame->sensor))
         return fail(m, GEM_ERR_INVALID, "gem_route_points: bad argument");
     if (n > m->P) return fail(m, GEM_ERR_INVALID, "gem_route_points: n exceeds max_points");
     if (tiles_r * tiles_c > ROUTE_MAX_OWNERS) return fail(m, GEM_ERR_INVALID, "gem_route_points: too many tiles");
@@ -2548,7 +2576,7 @@ int gem_route_points_peer(gem_map *m, const void *xyzi, const void *rgba, int n,
 {
     const int no = tiles_r * tiles_c;
     if (!m || !frame || n < 0 || tiles_r < 1 || tiles_c < 1 || !peer_recv || !peer_counts || (n > 0 && !xyzi) || bucket_stride < n ||
-        my_rank < 0 || my_rank >= no)
+        my_rank < 0 || my_rank >= no || !sensor_ok(frame->sensor))
         return fail(m, GEM_ERR_INVALID, "gem_route_points_peer: bad argument (bucket_stride must be >= n)");
     if (n > m->P) return fail(m, GEM_ERR_INVALID, "gem_route_points_peer: n exceeds max_points");
     if (no > ROUTE_MAX_OWNERS) return fail(m, GEM_ERR_INVALID, "gem_route_points_peer: too many tiles");
@@ -2669,7 +2697,7 @@ int gem_tiled_attach(gem_map *m, const gem_tiled_peers *p)
 // GEM_B200_PIPE=stream and off route and bin each step inside its own call, whatever the depth.
 int gem_tiled_step(gem_map *m, const void *xyzi, const void *rgba, int n, const gem_frame *frame)
 {
-    if (!m || !frame || n < 0 || (n > 0 && !xyzi)) return fail(m, GEM_ERR_INVALID, "gem_tiled_step: bad argument");
+    if (!m || !frame || n < 0 || (n > 0 && !xyzi) || !sensor_ok(frame->sensor)) return fail(m, GEM_ERR_INVALID, "gem_tiled_step: bad argument");
     Lock lk(m->mu);
     SetDev sd(m->dev);
     TiledState &ts = m->tiled;
@@ -2692,9 +2720,11 @@ int gem_tiled_step(gem_map *m, const void *xyzi, const void *rgba, int n, const 
     int nn = n, tiles_c = ts.tiles_c, my_rank = ts.my_rank, nblk = ts.nblk, cap = ts.cap, bufv = ts.step % PEER_BUFS, stepv = ts.step, worldv = world;
     int *ticket = ts.d_ticket;
     PeerBufs pb = ts.pb;
+    // stereo / perfect frames take the every-model instantiation (gem_route.cuh)
+    auto *route_kernel = any_model(fp) ? k_route_peer_any : k_route_peer;
     void *route_args[] = {&gg, &fp, &px, &pr, &nn, &th, &tw, &tiles_c, &worldv, &my_rank, &nblk, &cap, &bufv, &stepv, &pb, &ticket};
     auto launch_route = [&]() -> int {
-        GEM_LAUNCH(m, GEM_PROF_ROUTE, k_route_peer<<<nblk, ROUTE_BLOCK, 0, m->stream>>>(gg, fp, px, pr, nn, th, tw, tiles_c, worldv, my_rank, nblk, cap, bufv, stepv, pb, ticket));
+        GEM_LAUNCH(m, GEM_PROF_ROUTE, route_kernel<<<nblk, ROUTE_BLOCK, 0, m->stream>>>(gg, fp, px, pr, nn, th, tw, tiles_c, worldv, my_rank, nblk, cap, bufv, stepv, pb, ticket));
         GEM_CUDA(m, cudaGetLastError());
         return GEM_OK;
     };
@@ -2739,9 +2769,13 @@ int gem_tiled_step(gem_map *m, const void *xyzi, const void *rgba, int n, const 
     cudaKernelNodeParams kl{}, kf{}, kr{}, kb{};
     kl.func = (void *)k_fold_long; kl.gridDim = dim3((unsigned)long_blocks_for(m, prev.n / world)); kl.blockDim = dim3(LONG_BLOCK); kl.sharedMemBytes = (unsigned)m->long_smem; kl.kernelParams = long_args;
     kf.func = (void *)k_fold; kf.gridDim = dim3((unsigned)fb); kf.blockDim = dim3(ADD_BLOCK); kf.sharedMemBytes = (unsigned)m->fold_smem; kf.kernelParams = fold_args;
-    kr.func = (void *)k_route_peer; kr.gridDim = dim3((unsigned)nblk); kr.blockDim = dim3(ROUTE_BLOCK); kr.sharedMemBytes = 0; kr.kernelParams = route_args;
+    kr.func = (void *)route_kernel; kr.gridDim = dim3((unsigned)nblk); kr.blockDim = dim3(ROUTE_BLOCK); kr.sharedMemBytes = 0; kr.kernelParams = route_args;
     kb.func = (void *)k_bin_peer; kb.gridDim = dim3((unsigned)bin_peer_blocks(b.nsub)); kb.blockDim = dim3(ROUTE_BLOCK); kb.sharedMemBytes = 0; kb.kernelParams = bin_args;
+    if (ts.exec && ts.route_func != kr.func) { // a sensor model of the other kind: a node's kernel cannot be swapped
+        cudaGraphExecDestroy(ts.exec); cudaGraphDestroy(ts.graph); ts.exec = nullptr; ts.graph = nullptr;
+    }
     if (!ts.exec) {
+        ts.route_func = kr.func;
         GEM_CUDA(m, cudaGraphCreate(&ts.graph, 0));
         GEM_CUDA(m, cudaGraphAddKernelNode(&ts.long_node, ts.graph, nullptr, 0, &kl));
         GEM_CUDA(m, cudaGraphAddKernelNode(&ts.route_node, ts.graph, nullptr, 0, &kr));

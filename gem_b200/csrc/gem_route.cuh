@@ -14,10 +14,11 @@ namespace gem {
 constexpr int ROUTE_MAX_OWNERS = 64;
 constexpr int ROUTE_BLOCK = 256;
 
-// pass 1: transform, owner id, per-block owner histogram
-__global__ void __launch_bounds__(ROUTE_BLOCK)
-k_route_count(MapGeom g, FrameParams f, const float4 *xyzi, int n, int tile_h, int tile_w, int tiles_c,
-              int n_owners, int *owner_out, int *gkey_out, float *h_out, float *hv_out, int *blockCounts /* [owners][blocks] */)
+// pass 1: transform, owner id, per-block owner histogram.  ANY: every sensor model (k_route_count_any)
+template <bool ANY>
+__device__ __forceinline__ void route_count(const MapGeom &g, const FrameParams &f, const float4 *xyzi, int n, int tile_h, int tile_w,
+                                            int tiles_c, int n_owners, int *owner_out, int *gkey_out, float *h_out, float *hv_out,
+                                            int *blockCounts)
 {
     __shared__ int s_cnt[ROUTE_MAX_OWNERS];
     for (int o = threadIdx.x; o < n_owners; o += blockDim.x) s_cnt[o] = 0;
@@ -26,7 +27,7 @@ k_route_count(MapGeom g, FrameParams f, const float4 *xyzi, int n, int tile_h, i
     int owner = -1;
     if (i < n) {
         const float4 p = ld_stream_f4(xyzi + i);
-        const PtRes r = transform_point(g, f, p.x, p.y, p.z);
+        const PtRes r = transform_point<ANY>(g, f, p.x, p.y, p.z, i);
         int gkey = -1;
         if (r.ingrid) {
             owner = (r.gx / tile_h) * tiles_c + (r.gy / tile_w);
@@ -40,6 +41,18 @@ k_route_count(MapGeom g, FrameParams f, const float4 *xyzi, int n, int tile_h, i
     if (owner >= 0) atomicAdd(&s_cnt[owner], 1);
     __syncthreads();
     for (int o = threadIdx.x; o < n_owners; o += blockDim.x) blockCounts[o * gridDim.x + blockIdx.x] = s_cnt[o];
+}
+__global__ void __launch_bounds__(ROUTE_BLOCK)
+k_route_count(MapGeom g, FrameParams f, const float4 *xyzi, int n, int tile_h, int tile_w, int tiles_c,
+              int n_owners, int *owner_out, int *gkey_out, float *h_out, float *hv_out, int *blockCounts /* [owners][blocks] */)
+{
+    route_count<false>(g, f, xyzi, n, tile_h, tile_w, tiles_c, n_owners, owner_out, gkey_out, h_out, hv_out, blockCounts);
+}
+__global__ void __launch_bounds__(ROUTE_BLOCK)
+k_route_count_any(MapGeom g, FrameParams f, const float4 *xyzi, int n, int tile_h, int tile_w, int tiles_c,
+                  int n_owners, int *owner_out, int *gkey_out, float *h_out, float *hv_out, int *blockCounts)
+{
+    route_count<true>(g, f, xyzi, n, tile_h, tile_w, tiles_c, n_owners, owner_out, gkey_out, h_out, hv_out, blockCounts);
 }
 
 // pass 2: one block scans blockCounts owner-major -> exclusive offsets; owner totals
@@ -176,8 +189,8 @@ inline cudaError_t route_points(cudaStream_t st, const MapGeom &g, const FramePa
     const int nblocks = n > 0 ? (n + ROUTE_BLOCK - 1) / ROUTE_BLOCK : 1;
     if ((size_t)n_owners * nblocks > sc.blockCounts_capacity) return cudaErrorInvalidValue;
     const int tile_h = (g.L + tiles_r - 1) / tiles_r, tile_w = (g.L + tiles_c - 1) / tiles_c;
-    k_route_count<<<nblocks, ROUTE_BLOCK, 0, st>>>(g, fp, xyzi, n, tile_h, tile_w, tiles_c, n_owners, sc.owner, sc.gkey,
-                                                  sc.h, sc.hv, sc.blockCounts);
+    (any_model(fp) ? k_route_count_any : k_route_count)<<<nblocks, ROUTE_BLOCK, 0, st>>>(
+        g, fp, xyzi, n, tile_h, tile_w, tiles_c, n_owners, sc.owner, sc.gkey, sc.h, sc.hv, sc.blockCounts);
     k_route_scan<<<1, 1024, 0, st>>>(sc.blockCounts, n_owners, nblocks, counts_out);
     if (peer)
         k_route_write_peer<<<nblocks, ROUTE_BLOCK, 0, st>>>(xyzi, rgba, n, n_owners, sc.owner, sc.gkey, sc.h, sc.hv, sc.blockCounts,
@@ -219,9 +232,10 @@ struct PeerBufs { // device addresses valid on THIS device (own memory or peer m
     unsigned long long flag[ROUTE_MAX_OWNERS];  // int   [world]: flag[o][r] = last step rank r has delivered to rank o
 };
 
-__global__ void __launch_bounds__(ROUTE_BLOCK)
-k_route_peer(MapGeom g, FrameParams f, const float4 *xyzi, const uchar4 *rgba, int n, int tile_h, int tile_w, int tiles_c, int world,
-             int my_rank, int nblk, int cap, int buf, int step, const __grid_constant__ PeerBufs pb, int *ticket)
+template <bool ANY>
+__device__ __forceinline__ void route_peer(const MapGeom &g, const FrameParams &f, const float4 *xyzi, const uchar4 *rgba, int n, int tile_h,
+                                           int tile_w, int tiles_c, int world, int my_rank, int nblk, int cap, int buf, int step,
+                                           const PeerBufs &pb, int *ticket)
 {
     __shared__ int s_wcnt[ROUTE_BLOCK / 32][ROUTE_MAX_OWNERS];
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -234,7 +248,7 @@ k_route_peer(MapGeom g, FrameParams f, const float4 *xyzi, const uchar4 *rgba, i
     uint32_t rgb = 0u;
     if (i < n) {
         const float4 p = ld_stream_f4(xyzi + i);
-        const PtRes r = transform_point(g, f, p.x, p.y, p.z);
+        const PtRes r = transform_point<ANY>(g, f, p.x, p.y, p.z, i);
         if (r.ingrid) {
             owner = (r.gx / tile_h) * tiles_c + (r.gy / tile_w);
             gkey = r.gx * g.L + r.gy;
@@ -276,6 +290,18 @@ k_route_peer(MapGeom g, FrameParams f, const float4 *xyzi, const uchar4 *rgba, i
                 asm volatile("st.relaxed.sys.global.s32 [%0], %1;" ::"l"(reinterpret_cast<int *>(pb.flag[o]) + my_rank), "r"(step) : "memory");
         }
     }
+}
+__global__ void __launch_bounds__(ROUTE_BLOCK)
+k_route_peer(MapGeom g, FrameParams f, const float4 *xyzi, const uchar4 *rgba, int n, int tile_h, int tile_w, int tiles_c, int world,
+             int my_rank, int nblk, int cap, int buf, int step, const __grid_constant__ PeerBufs pb, int *ticket)
+{
+    route_peer<false>(g, f, xyzi, rgba, n, tile_h, tile_w, tiles_c, world, my_rank, nblk, cap, buf, step, pb, ticket);
+}
+__global__ void __launch_bounds__(ROUTE_BLOCK) // every sensor model
+k_route_peer_any(MapGeom g, FrameParams f, const float4 *xyzi, const uchar4 *rgba, int n, int tile_h, int tile_w, int tiles_c, int world,
+                 int my_rank, int nblk, int cap, int buf, int step, const __grid_constant__ PeerBufs pb, int *ticket)
+{
+    route_peer<true>(g, f, xyzi, rgba, n, tile_h, tile_w, tiles_c, world, my_rank, nblk, cap, buf, step, pb, ticket);
 }
 
 // one point of the bin kernel, U = 1 (see bin_points for the argument why the waits cannot deadlock)

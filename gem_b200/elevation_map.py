@@ -57,6 +57,49 @@ class StructuredLightSensorProcessor:
                               self.normal_factor_e, self.lateral_factor, self.cutoff_min_depth, self.cutoff_max_depth)
 
 
+@dataclass
+class StereoSensorProcessor:
+    """sensor_processor/type: stereo (StereoSensorProcessor.cpp:23-34, aslam.yaml).  Every parameter defaults to the
+    node's 0.0.  cloud_width: pointCloud->width of the organised cloud the calls receive (0 = unorganised); the
+    model reads each point's pixel row and column from its index in that cloud."""
+    p_1: float = 0.0
+    p_2: float = 0.0
+    p_3: float = 0.0
+    p_4: float = 0.0
+    p_5: float = 0.0
+    lateral_factor: float = 0.0
+    depth_to_disparity_factor: float = 0.0
+    cloud_width: int = 0
+    ignore_points_above: float = float("inf")
+    ignore_points_below: float = float("-inf")
+
+    def model(self) -> GemSensorModel:
+        m = GemSensorModel(_lib.SENSOR_STEREO)
+        m.lateral_factor = self.lateral_factor
+        m.stereo_p[:] = [self.p_1, self.p_2, self.p_3, self.p_4, self.p_5]
+        m.depth_to_disparity_factor = self.depth_to_disparity_factor
+        m.cloud_width = int(self.cloud_width)
+        return m
+
+
+@dataclass
+class PerfectSensorProcessor:
+    """sensor_processor/type: perfect (PerfectSensorProcessor.cpp, perfect.yaml): zero sensor variance.  Its
+    readParameters does not call the base class (:36-39), so the height window is always the constructor's +-inf
+    (SensorProcessorBase.cpp:39-40): there are no ignore_points_* to set."""
+
+    @property
+    def ignore_points_above(self) -> float:
+        return float("inf")
+
+    @property
+    def ignore_points_below(self) -> float:
+        return float("-inf")
+
+    def model(self) -> GemSensorModel:
+        return GemSensorModel(_lib.SENSOR_PERFECT)
+
+
 def make_frame(T, sensor, base_z: float = 0.0, rotation_variance=None, C_SB_transpose=None,
                P_mul_C_BM_transpose=None, B_r_BS_skew=None, sensor_jacobian=None) -> GemFrame:
     """Per-frame constants as SensorProcessorBase::GPUPointCloudprocess derives them.

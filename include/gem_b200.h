@@ -68,11 +68,27 @@ typedef struct gem_config {
     double grid_resolution;
 } gem_config;
 
-enum { GEM_SENSOR_LASER = 0, GEM_SENSOR_STRUCTURED_LIGHT = 1 };
+enum { GEM_SENSOR_LASER = 0, GEM_SENSOR_STRUCTURED_LIGHT = 1, GEM_SENSOR_STEREO = 2, GEM_SENSOR_PERFECT = 3 };
 
 /* Sensor noise model: laser = gpu.cu:410-411 (C_min_r, C_beam_a, C_beam_c);
  * structured light = StructuredLightSensorProcessor.cpp:129-139 (doubles), plus the depth
- * pass-through of its cleanPointCloud (:51-66). */
+ * pass-through of its cleanPointCloud (:51-66);
+ * stereo = StereoSensorProcessor.cpp:78-90 (doubles; PARITY UNPINNED, restated: the reference's CPU code needs
+ * kindr and PCL).  With (x, y, z) the sensor-frame point, idx its index in the cloud the caller passes and
+ * w = cloud_width (0: unorganised, one row), row = w ? idx / w : 0 and col = w ? idx % w : idx (getI / getJ,
+ * :109-117; the library removes no points, so idx is the position removeNaNFromPointCloud records), and
+ *     disp = dtd / (double)z                       dtd = depth_to_disparity_factor
+ *     a    = dtd / (disp * disp)
+ *     s    = ((p3 * disp) + p4) - (double)col      p1..p5 = stereo_p[0..4]
+ *     r    = (double)(240 - row)                   the reference's hard-coded principal row
+ *     vN   = (float)((a * a) * ((((p5 * disp) + p2) * sqrt(s * s + r * r)) + p1))
+ *     vL   = (float)(l * l),  l = lateral_factor * (double)sqrtf((x * x + y * y) + z * z)
+ * pow(v, 2) is DEFINED as v * v, rounded once.  vN and vL are variances (not deviations), fed to the same
+ * height-variance expression as every model; z = +-0, subnormal or negative give what the expression gives
+ * (inf, NaN, negative values), unclamped.  Its cleanPointCloud only removes non-finite points (:37-48);
+ * perfect = PerfectSensorProcessor.cpp:84-101: vN = vL = 0.  Its readParameters skips the base class (:36-39),
+ * so its height window is always +-inf: the helpers in gem_b200/elevation_map.hpp ignore ignore_points_* for it.
+ * A type outside 0..3 or cloud_width < 0 makes every call that takes a frame return GEM_ERR_INVALID. */
 typedef struct gem_sensor_model {
     int type;
     float min_radius, beam_angle, beam_constant;
@@ -86,6 +102,12 @@ typedef struct gem_sensor_model {
      * cleanPointCloud only removes non-finite points (LaserSensorProcessor.cpp:50-59) -- those never pass the
      * height window of gpu.cu:397 anyway. */
     double cutoff_min_depth, cutoff_max_depth;
+    /* stereo only: p_1..p_5, depth_to_disparity_factor (StereoSensorProcessor.cpp:26-32; the node's defaults
+     * are 0) and pointCloud->width of the organised cloud, 0 = unorganised (the stereo model reads
+     * lateral_factor too) */
+    double stereo_p[5];
+    double depth_to_disparity_factor;
+    int cloud_width;
 } gem_sensor_model;
 
 /* Per-frame constants = the by-value arguments of Process_points (gpu.cu:1085), derived by
