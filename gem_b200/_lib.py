@@ -180,9 +180,6 @@ SYMBOLS = {
     "gem_get_layer_device": (C.c_int, [_P, C.c_int, _P]),
     "gem_compute_features_tiled": (C.c_int, [_P, _P]),
     "gem_raytracing_tiled": (C.c_int, [_P, _P]),
-    "gem_route_points_peer": (C.c_int, [_P, _P, _P, C.c_int, C.POINTER(GemFrame), C.c_int, C.c_int,
-                                        C.POINTER(C.c_ulonglong), C.POINTER(C.c_ulonglong), C.c_int, C.c_int]),
-    "gem_fuse_records_counted": (C.c_int, [_P, _P, _P, C.c_int, C.c_int]),
     "gem_transform_cloud": (C.c_int, [_P, _P, C.c_int, _FP]),
     "gem_refuse_submaps": (C.c_int, [_P, _P, _IP, _P, _IP, C.c_double, C.c_int, _IP]),
     "gem_tiled_attach": (C.c_int, [_P, C.POINTER(GemTiledPeers)]),

@@ -179,11 +179,8 @@ struct BinSource {
     const int *key_in, *R, *G, *B;
     const float *h_in, *hv_in, *inten_in;
     int ncells;
-    // SRC_RECORDS (tiled maps): records received from the other tiles, buckets of `stride` slots filled up to
-    // src_counts[bucket] (src_counts == nullptr: all n slots are records; gkey < 0 = padding)
+    // SRC_RECORDS (tiled maps): records received from the other tiles (gkey < 0 = padding)
     const RouteRec *rec;
-    const int *src_counts;
-    int stride;
 };
 
 struct PointOut {
@@ -248,21 +245,14 @@ __device__ __forceinline__ PointOut bin_source_point(const MapGeom &g, const Fra
                                       (b != 0 && (b & 255) == 0) ? 255 : b);
         o.rgbf = with_colour_flag(rgb, in.inten_in ? in.inten_in[i] : 0.0f);
     } else { // SRC_RECORDS
-        bool valid = true;
-        if (in.src_counts) {
-            const int s = i / in.stride;
-            valid = (i - s * in.stride) < in.src_counts[s];
+        const RouteRec r = in.rec[i];
+        if (r.gkey >= 0) {
+            const int gx = r.gkey / g.L, gy = r.gkey - gx * g.L;
+            o.key = local_key(g, gx, gy);
+            o.geo = g.tiled ? o.key : r.gkey;
         }
-        if (valid) {
-            const RouteRec r = in.rec[i];
-            if (r.gkey >= 0) {
-                const int gx = r.gkey / g.L, gy = r.gkey - gx * g.L;
-                o.key = local_key(g, gx, gy);
-                o.geo = g.tiled ? o.key : r.gkey;
-            }
-            o.h = r.h; o.hv = r.var;
-            o.rgbf = with_colour_flag(r.rgb, r.intensity);
-        }
+        o.h = r.h; o.hv = r.var;
+        o.rgbf = with_colour_flag(r.rgb, r.intensity);
     }
     return o;
 }

@@ -123,10 +123,7 @@ struct gem_map {
     // GEM_B200_EXCLUSIVE=1 pads the kernels' shared memory so that k_fold_long's blocks get SMs of their own
     int fold_max_blocks = NUM_SMS * 2, long_blocks = LONG_BLOCKS;
     size_t bin_smem = 0, fold_smem = FOLD_SMEM_USED, long_smem = (LONG_BLOCK / 32) * sizeof(WarpScratch);
-    int pipe_mode = 2;               // 0: never defer the fold; 1: two streams + events; 2: CUDA graph per call
     std::map<const void *, FrameGraph> graphs; // keyed by the bin kernel function
-    cudaStream_t front_stream = nullptr;      // pipe_mode 1: the bin kernels run here
-    cudaEvent_t ev_bin[2] = {nullptr, nullptr}, ev_fold[2] = {nullptr, nullptr}, ev_mark = nullptr;
     // deferred region operations (scroll clears of Move, the every-cell variance floor of
     // G_fuse): executed by the next add/fuse launch, or flushed before anything observes the map
     std::vector<RegionOp> pending;
@@ -136,7 +133,6 @@ struct gem_map {
     int *d_keyin = nullptr, *d_keyout = nullptr, *d_R = nullptr, *d_G = nullptr, *d_B = nullptr;
     float *d_int = nullptr, *d_h = nullptr, *d_hv = nullptr;
     float *d_out = nullptr; // 9 * nc floats read-out staging
-    int *d_owner_cnt = nullptr;
     RouteScratch route_sc{};
     float2 *prev_ev = nullptr;     // gem_snapshot_shown: prevMap_ (ElevationMapping.cpp:422) on the device
     uint2 *prev_ci = nullptr;
@@ -223,21 +219,20 @@ cudaEvent_t prof_event(gem_map *m)
     return e;
 }
 // every kernel launch of the library goes through this macro: counts the launch and, when
-// profiling is on, brackets it with CUDA events on the stream it is launched on
-#define GEM_LAUNCH_ON(m, st, cls, ...)                           \
+// profiling is on, brackets it with CUDA events on the handle's stream
+#define GEM_LAUNCH(m, cls, ...)                                  \
     do {                                                         \
         (m)->launches++;                                         \
         if ((m)->profiling) {                                    \
             gem_map::Span sp__{(cls), prof_event(m), prof_event(m)}; \
-            cudaEventRecord(sp__.e0, (st));                      \
+            cudaEventRecord(sp__.e0, (m)->stream);               \
             __VA_ARGS__;                                         \
-            cudaEventRecord(sp__.e1, (st));                      \
+            cudaEventRecord(sp__.e1, (m)->stream);               \
             (m)->spans.push_back(sp__);                          \
         } else {                                                 \
             __VA_ARGS__;                                         \
         }                                                        \
     } while (0)
-#define GEM_LAUNCH(m, cls, ...) GEM_LAUNCH_ON(m, (m)->stream, cls, __VA_ARGS__)
 
 #define GEM_CUDA(m, expr)                                                                      \
     do {                                                                                       \
@@ -343,7 +338,7 @@ int launch_regions(gem_map *m, const RegionOp *ops, int count)
 }
 
 // ---- the fold of a pipelined add call is issued with the NEXT call, or here ------------------------------------
-int launch_fold(gem_map *m, cudaStream_t st, const PendingFold &p, const RegionOps &ro, int region_blocks, bool do_fuse, bool do_lowest)
+int launch_fold(gem_map *m, const PendingFold &p, const RegionOps &ro, int region_blocks, bool do_fuse, bool do_lowest)
 {
     const int fb = fold_blocks_for(m, p.n);
     const int slice = fold_slice(p.n, fb);
@@ -351,8 +346,8 @@ int launch_fold(gem_map *m, cudaStream_t st, const PendingFold &p, const RegionO
     // (disjoint cells, so the order is free) -- the frame graph of the pipelined mode runs them side by side.  Both get
     // the next call's clears `ro`: a long list inside a cleared band must store the cleared value itself, because
     // k_fold's region blocks may clear the cell before k_fold_long writes it (cell_end)
-    GEM_LAUNCH_ON(m, st, GEM_PROF_FOLD_LONG, k_fold_long<<<long_blocks_for(m, p.n), LONG_BLOCK, m->long_smem, st>>>(p.geom, m->ml, p.sc, p.src, ro, do_fuse ? 1 : 0, do_lowest ? 1 : 0));
-    GEM_LAUNCH_ON(m, st, GEM_PROF_FOLD, k_fold<<<fb + region_blocks, ADD_BLOCK, m->fold_smem, st>>>(p.geom, m->ml, p.sc, p.src, ro, p.n, fb, slice, do_fuse ? 1 : 0, do_lowest ? 1 : 0, p.n_dev));
+    GEM_LAUNCH(m, GEM_PROF_FOLD_LONG, k_fold_long<<<long_blocks_for(m, p.n), LONG_BLOCK, m->long_smem, m->stream>>>(p.geom, m->ml, p.sc, p.src, ro, do_fuse ? 1 : 0, do_lowest ? 1 : 0));
+    GEM_LAUNCH(m, GEM_PROF_FOLD, k_fold<<<fb + region_blocks, ADD_BLOCK, m->fold_smem, m->stream>>>(p.geom, m->ml, p.sc, p.src, ro, p.n, fb, slice, do_fuse ? 1 : 0, do_lowest ? 1 : 0, p.n_dev));
     GEM_CUDA(m, cudaGetLastError());
     return GEM_OK;
 }
@@ -415,15 +410,13 @@ int drain(gem_map *m)
     RegionOps none{};
     int rc;
     if (m->pend.active) {
-        if (m->pipe_mode == 1) GEM_CUDA(m, cudaStreamWaitEvent(m->stream, m->ev_bin[m->pend.sc.par], 0));
-        if ((rc = launch_fold(m, m->stream, m->pend, none, 0, true, true))) return rc;
-        if (m->pipe_mode == 1) GEM_CUDA(m, cudaEventRecord(m->ev_fold[m->pend.sc.par], m->stream));
+        if ((rc = launch_fold(m, m->pend, none, 0, true, true))) return rc;
         m->pend.active = false;
     }
     if (m->tiled.routed.active) { // a tiled step that is routed but not binned: bin it, fold it
         const TiledBin b = tiled_bin_of(m, m->tiled.routed.step, m->tiled.routed.buf);
         m->tiled.routed.active = false;
-        if ((rc = launch_tiled_bin(m, b)) || (rc = launch_fold(m, m->stream, b.fold, none, 0, true, true))) return rc;
+        if ((rc = launch_tiled_bin(m, b)) || (rc = launch_fold(m, b.fold, none, 0, true, true))) return rc;
     }
     return GEM_OK;
 }
@@ -577,23 +570,8 @@ int ensure_route_scratch(gem_map *m)
     return GEM_OK;
 }
 
-int pipe_setup(gem_map *m)
-{
-    if (m->pipe_mode != 1) return GEM_OK;
-    if (!m->front_stream) GEM_CUDA(m, cudaStreamCreateWithFlags(&m->front_stream, cudaStreamNonBlocking));
-    for (int i = 0; i < 2; i++) {
-        if (!m->ev_bin[i]) GEM_CUDA(m, cudaEventCreateWithFlags(&m->ev_bin[i], cudaEventDisableTiming));
-        if (!m->ev_fold[i]) {
-            GEM_CUDA(m, cudaEventCreateWithFlags(&m->ev_fold[i], cudaEventDisableTiming));
-            GEM_CUDA(m, cudaEventRecord(m->ev_fold[i], m->stream));
-        }
-    }
-    if (!m->ev_mark) GEM_CUDA(m, cudaEventCreateWithFlags(&m->ev_mark, cudaEventDisableTiming));
-    return GEM_OK;
-}
-
 // {long lists, other lists of the previous call || bin of this call} as a three-node graph, built once per bin kernel; per
-// call only the node parameters change.  One cudaGraphLaunch replaces three launches, two event records and two stream waits.
+// call only the node parameters change.  One cudaGraphLaunch runs the three side by side on the handle's stream.
 int launch_frame_graph(gem_map *m, BinKernel bk, void **bin_args, int bin_grid, void **fold_args, int fold_grid, void **long_args, int long_grid)
 {
     FrameGraph &fg = m->graphs[(const void *)bk];
@@ -627,8 +605,7 @@ int enqueue_add(gem_map *m, const BinSource &in, const FoldSrc &fsrc, int n, con
                 const FrameParams *frames, bool pipelined, bool do_fuse, bool do_lowest, bool any_segment = false)
 {
     int rc;
-    if (m->profiling || m->pipe_mode == 0) pipelined = false; // per-kernel event timing needs the serial schedule
-    if (pipelined && (rc = pipe_setup(m))) return rc;
+    if (m->profiling) pipelined = false; // per-kernel event timing needs the serial schedule
     if (pipelined && m->pend.active) {
         // operations other than "clear + floor of a row / column band" cannot ride on a running fold
         bool mergeable = (int)m->pending.size() <= MAX_REGION_OPS;
@@ -660,19 +637,12 @@ int enqueue_add(gem_map *m, const BinSource &in, const FoldSrc &fsrc, int n, con
     if (!pipelined || !m->pend.active) {
         // nothing in flight: the bin kernel carries the deferred region operations in spare blocks
         if ((rc = take_region_ops(m, ro, rb))) return rc;
-        cudaStream_t st_bin = m->stream;
-        if (pipelined && m->pipe_mode == 1) { // later bins of the pipeline run on the front stream: order it behind everything issued so far
-            GEM_CUDA(m, cudaEventRecord(m->ev_mark, m->stream));
-            GEM_CUDA(m, cudaStreamWaitEvent(m->front_stream, m->ev_mark, 0));
-            st_bin = m->front_stream;
-        }
-        GEM_LAUNCH_ON(m, st_bin, GEM_PROF_BIN, bk<<<pb + rb, ADD_BLOCK, m->bin_smem, st_bin>>>(g, ml, f, bin, nn, sc, ro, pb, st, frames));
+        GEM_LAUNCH(m, GEM_PROF_BIN, bk<<<pb + rb, ADD_BLOCK, m->bin_smem, m->stream>>>(g, ml, f, bin, nn, sc, ro, pb, st, frames));
         GEM_CUDA(m, cudaGetLastError());
         commit_region_ops(m);
-        if (pipelined && m->pipe_mode == 1) GEM_CUDA(m, cudaEventRecord(m->ev_bin[par], st_bin));
         if (!pipelined) {
             RegionOps none{};
-            if ((rc = launch_fold(m, m->stream, cur, none, 0, do_fuse, do_lowest))) return rc;
+            if ((rc = launch_fold(m, cur, none, 0, do_fuse, do_lowest))) return rc;
         } else {
             m->pend = cur;
         }
@@ -683,20 +653,11 @@ int enqueue_add(gem_map *m, const BinSource &in, const FoldSrc &fsrc, int n, con
         const int fb = fold_blocks_for(m, prev.n);
         int slice = fold_slice(prev.n, fb);
         RegionOps none{};
-        if (m->pipe_mode == 2) {
-            int pbk = pb, one = 1, fbk = fb;
-            void *bin_args[] = {&g, &ml, &f, &bin, &nn, &sc, &none, &pbk, &st, (void *)&frames};
-            void *fold_args[] = {&prev.geom, &ml, &prev.sc, &prev.src, &ro, &prev.n, &fbk, &slice, &one, &one, (void *)&prev.n_dev};
-            void *long_args[] = {&prev.geom, &ml, &prev.sc, &prev.src, &ro, &one, &one}; // the clears, like k_fold (launch_fold)
-            if ((rc = launch_frame_graph(m, bk, bin_args, pb, fold_args, fb + rb, long_args, long_blocks_for(m, prev.n)))) return rc;
-        } else {
-            GEM_CUDA(m, cudaStreamWaitEvent(m->front_stream, m->ev_fold[par], 0)); // the fold that last used this parity's scratch
-            GEM_LAUNCH_ON(m, m->front_stream, GEM_PROF_BIN, bk<<<pb, ADD_BLOCK, m->bin_smem, m->front_stream>>>(g, ml, f, bin, nn, sc, none, pb, st, frames));
-            GEM_CUDA(m, cudaEventRecord(m->ev_bin[par], m->front_stream));
-            GEM_CUDA(m, cudaStreamWaitEvent(m->stream, m->ev_bin[prev.sc.par], 0));
-            if ((rc = launch_fold(m, m->stream, prev, ro, rb, true, true))) return rc;
-            GEM_CUDA(m, cudaEventRecord(m->ev_fold[prev.sc.par], m->stream));
-        }
+        int pbk = pb, one = 1, fbk = fb;
+        void *bin_args[] = {&g, &ml, &f, &bin, &nn, &sc, &none, &pbk, &st, (void *)&frames};
+        void *fold_args[] = {&prev.geom, &ml, &prev.sc, &prev.src, &ro, &prev.n, &fbk, &slice, &one, &one, (void *)&prev.n_dev};
+        void *long_args[] = {&prev.geom, &ml, &prev.sc, &prev.src, &ro, &one, &one}; // the clears, like k_fold (launch_fold)
+        if ((rc = launch_frame_graph(m, bk, bin_args, pb, fold_args, fb + rb, long_args, long_blocks_for(m, prev.n)))) return rc;
         commit_region_ops(m);
         m->pend = cur;
     }
@@ -806,9 +767,6 @@ int gem_create(const gem_config *cfg, gem_map **out)
     // the fold's sort key packs the point index of a launch into 22 bits; larger calls are chunked
     if (m->P > (1 << FOLD_INDEX_BITS)) m->P = 1 << FOLD_INDEX_BITS;
     {
-        const char *env = getenv("GEM_B200_PIPE"); // graph (default) | stream | off
-        if (env && !strcmp(env, "stream")) m->pipe_mode = 1;
-        else if (env && !strcmp(env, "off")) m->pipe_mode = 0;
         const char *e1 = getenv("GEM_B200_FOLD_BLOCKS"), *e2 = getenv("GEM_B200_LONG_BLOCKS"), *e3 = getenv("GEM_B200_EXCLUSIVE");
         if (e1 && atoi(e1) > 0) m->fold_max_blocks = atoi(e1);
         if (e2 && atoi(e2) > 0) m->long_blocks = atoi(e2);
@@ -882,7 +840,6 @@ int gem_destroy(gem_map *m)
     {
         Lock lk(m->mu);
         SetDev sd(m->dev);
-        if (m->front_stream) cudaStreamSynchronize(m->front_stream);
         if (m->stream) cudaStreamSynchronize(m->stream);
         for (auto &kv : m->graphs) {
             if (kv.second.exec) cudaGraphExecDestroy(kv.second.exec);
@@ -905,14 +862,8 @@ int gem_destroy(gem_map *m)
         if (m->h_ctr) cudaFreeHost(m->h_ctr);
         if (m->h_ctr_ring) cudaFreeHost(m->h_ctr_ring);
         if (m->h_frames) cudaFreeHost(m->h_frames);
-        for (int i = 0; i < 2; i++) {
-            if (m->ev_bin[i]) cudaEventDestroy(m->ev_bin[i]);
-            if (m->ev_fold[i]) cudaEventDestroy(m->ev_fold[i]);
-        }
-        if (m->ev_mark) cudaEventDestroy(m->ev_mark);
         if (m->ev_export) cudaEventDestroy(m->ev_export);
         if (m->ev_export_done) cudaEventDestroy(m->ev_export_done);
-        if (m->front_stream) cudaStreamDestroy(m->front_stream);
         for (int i = 0; i < 4; i++) if (m->ev_frames[i]) cudaEventDestroy(m->ev_frames[i]);
         for (int i = 0; i < 3; i++) {
             if (m->ev_h2d[i]) cudaEventDestroy(m->ev_h2d[i]);
@@ -1154,9 +1105,6 @@ int gem_add_points_multi(gem_map *m, const void *xyzi, const void *rgba, int n_s
     }
     GEM_CUDA(m, cudaMemcpyAsync(df, hf, (size_t)n_segments * sizeof(FrameParams), cudaMemcpyHostToDevice, m->stream));
     GEM_CUDA(m, cudaEventRecord(m->ev_frames[slot], m->stream));
-    // GEM_B200_PIPE=stream: the steady-state bin runs on the front stream, which waits only for the fold that last used
-    // its scratch (recorded before this copy was queued): it must not read the table before the copy lands
-    if (m->pipe_mode == 1 && m->front_stream) GEM_CUDA(m, cudaStreamWaitEvent(m->front_stream, m->ev_frames[slot], 0));
     const BinSource in = xyzi_source(xyzi, rgba, 0);
     const FoldSrc fs{in.xyzi ? (const char *)in.xyzi + 12 : nullptr, 16};
     // pipelined like gem_add_points_stream: consecutive multi-sensor steps overlap bin(i+1) with fold(i)
@@ -1196,7 +1144,6 @@ int gem_add_points_host_async(gem_map *m, const void *xyzi, const void *rgba, in
     GEM_CUDA(m, cudaEventRecord(m->ev_h2d[b], m->copy_stream));
     // compute stream: wait for the copy, issue {fold of the previous call || bin of this one}
     GEM_CUDA(m, cudaStreamWaitEvent(m->stream, m->ev_h2d[b], 0));
-    if (m->pipe_mode == 1 && m->front_stream) GEM_CUDA(m, cudaStreamWaitEvent(m->front_stream, m->ev_h2d[b], 0));
     const FrameParams fp = make_frame(frame);
     const BinSource in = xyzi_source(m->d_axyzi[b], rgba ? m->d_argba[b] : nullptr, 0);
     const FoldSrc fs{in.xyzi ? (const char *)in.xyzi + 12 : nullptr, 16};
@@ -2485,7 +2432,6 @@ int gem_profile_read(gem_map *m, gem_profile *out, int reset)
     Lock lk(m->mu);
     SetDev sd(m->dev);
     { int rc = drain(m); if (rc) return rc; }
-    if (m->front_stream) GEM_CUDA(m, cudaStreamSynchronize(m->front_stream));
     GEM_CUDA(m, cudaStreamSynchronize(m->stream));
     for (auto &sp : m->spans) {
         float ms = 0.0f;
@@ -2560,41 +2506,24 @@ int gem_route_points(gem_map *m, const void *xyzi, const void *rgba, int n, cons
     return GEM_OK;
 }
 
-static int fuse_records_impl(gem_map *m, const void *rec, int n, const int *src_counts, int stride);
-
-int gem_fuse_records(gem_map *m, const void *rec, int n) { return fuse_records_impl(m, rec, n, nullptr, 1); }
-
-int gem_fuse_records_counted(gem_map *m, const void *rec, const int *src_counts, int n_sources, int bucket_stride)
+int gem_fuse_records(gem_map *m, const void *rec, int n)
 {
-    if (!m || !rec || !src_counts || n_sources < 1 || bucket_stride < 1) return fail(m, GEM_ERR_INVALID, "gem_fuse_records_counted: bad argument");
-    if ((long long)n_sources * bucket_stride > m->P) return fail(m, GEM_ERR_INVALID, "gem_fuse_records_counted: n_sources*bucket_stride exceeds max_points");
-    return fuse_records_impl(m, rec, n_sources * bucket_stride, src_counts, bucket_stride);
-}
-
-int gem_route_points_peer(gem_map *m, const void *xyzi, const void *rgba, int n, const gem_frame *frame, int tiles_r, int tiles_c,
-                          const unsigned long long *peer_recv, const unsigned long long *peer_counts, int my_rank, int bucket_stride)
-{
-    const int no = tiles_r * tiles_c;
-    if (!m || !frame || n < 0 || tiles_r < 1 || tiles_c < 1 || !peer_recv || !peer_counts || (n > 0 && !xyzi) || bucket_stride < n ||
-        my_rank < 0 || my_rank >= no || !sensor_ok(frame->sensor))
-        return fail(m, GEM_ERR_INVALID, "gem_route_points_peer: bad argument (bucket_stride must be >= n)");
-    if (n > m->P) return fail(m, GEM_ERR_INVALID, "gem_route_points_peer: n exceeds max_points");
-    if (no > ROUTE_MAX_OWNERS) return fail(m, GEM_ERR_INVALID, "gem_route_points_peer: too many tiles");
+    if (!m || n < 0 || (n > 0 && !rec)) return fail(m, GEM_ERR_INVALID, "gem_fuse_records: bad argument");
     Lock lk(m->mu);
     SetDev sd(m->dev);
     int rc = GEM_OK;
-    if (!m->d_owner_cnt && (rc = dev_alloc(m, &m->d_owner_cnt, ROUTE_MAX_OWNERS))) return rc;
-    const FrameParams fp = make_frame(frame);
-    MapGeom gg = m->geom;
-    gg.tiled = 0;
-    PeerTable pt;
-    memset(&pt, 0, sizeof pt);
-    for (int o = 0; o < no; o++) { pt.recv[o] = peer_recv[o]; pt.counts[o] = peer_counts[o]; }
-    if ((rc = ensure_route_scratch(m))) return rc;
-    const cudaError_t e = route_points(m->stream, gg, fp, (const float4 *)xyzi, (const uchar4 *)rgba, n, tiles_r, tiles_c,
-                                       m->route_sc, nullptr, m->d_owner_cnt, bucket_stride, &pt, my_rank);
-    m->launches += 3;
-    if (e != cudaSuccess) return fail(m, GEM_ERR_CUDA, std::string("gem_route_points_peer: ") + cudaGetErrorString(e));
+    memset(&m->stats, 0, sizeof m->stats);
+    if (n == 0) return flush_all_pending(m);
+    for (int off = 0; off < n; off += m->P) {
+        const int cn = (n - off < m->P) ? (n - off) : m->P;
+        BinSource in{};
+        in.rec = (const RouteRec *)rec + off;
+        const FoldSrc fs{(const char *)in.rec + 16, (int)sizeof(RouteRec)};
+        const FrameParams none{};
+        if ((rc = enqueue_add<SRC_RECORDS>(m, in, fs, cn, none, nullptr, nullptr, false, true, true))) return rc;
+        if (n > m->P && (rc = read_counters(m, cn, true))) return rc;
+    }
+    if (n <= m->P) m->stats.points_in = n;
     return GEM_OK;
 }
 
@@ -2671,7 +2600,7 @@ int gem_tiled_attach(gem_map *m, const gem_tiled_peers *p)
         return fail(m, GEM_ERR_INVALID, "gem_tiled_attach: world * bucket_capacity (rounded up to 256) = " + std::to_string((long long)world * cap) +
                                             " exceeds max_points = " + std::to_string(m->P) + " (at most 2^" + std::to_string(FOLD_INDEX_BITS) + ")");
     int rc = drain(m);
-    if (rc || (rc = pipe_setup(m))) return rc; // GEM_B200_PIPE=stream: the events drain() waits on
+    if (rc) return rc;
     TiledState &ts = m->tiled;
     ts.world = world; ts.my_rank = p->my_rank; ts.tiles_r = p->tiles_r; ts.tiles_c = p->tiles_c; ts.cap = cap; ts.nblk = nblk;
     for (int o = 0; o < world; o++) {
@@ -2694,7 +2623,6 @@ int gem_tiled_attach(gem_map *m, const gem_tiled_peers *p)
 // GEM_B200_TILED_DEPTH=3 pipelines three deep: four independent kernels {fold_long, fold of step j-2 || bin of step j-1
 // || route of step j}.  What is outstanding after the last call is issued by whatever reads the map next (gem_flush).
 // Every rank must make the same sequence of gem_tiled_step calls (a bin waits for every peer's flag of its step).
-// GEM_B200_PIPE=stream and off route and bin each step inside its own call, whatever the depth.
 int gem_tiled_step(gem_map *m, const void *xyzi, const void *rgba, int n, const gem_frame *frame)
 {
     if (!m || !frame || n < 0 || (n > 0 && !xyzi) || !sensor_ok(frame->sensor)) return fail(m, GEM_ERR_INVALID, "gem_tiled_step: bad argument");
@@ -2704,7 +2632,7 @@ int gem_tiled_step(gem_map *m, const void *xyzi, const void *rgba, int n, const 
     if (!ts.attached) return fail(m, GEM_ERR_INVALID, "gem_tiled_step: gem_tiled_attach first");
     if (n > ts.cap) return fail(m, GEM_ERR_INVALID, "gem_tiled_step: cloud larger than bucket_capacity");
     int rc;
-    const bool serial = m->profiling || m->pipe_mode == 0;
+    const bool serial = m->profiling;
     if (serial && (rc = drain(m))) return rc;
     if (!m->pending.empty()) { // tiled maps do not scroll: only the first-fuse floor can be pending
         if ((rc = drain(m)) || (rc = flush_all_pending(m))) return rc;
@@ -2732,17 +2660,14 @@ int gem_tiled_step(gem_map *m, const void *xyzi, const void *rgba, int n, const 
     m->stats.points_in = n;
     RegionOps none{};
     int one = 1;
-    const bool graphs = !serial && m->pipe_mode == 2;
+    const bool graphs = !serial;
     if (!graphs || ts.depth == 2) {
         // route -> bin of this step on the stream or in one graph with the previous step's folds
         if (!graphs || !m->pend.active) {
             if ((rc = drain(m)) || (rc = launch_route())) return rc;
             const TiledBin b = tiled_bin_of(m, stepv, bufv);
             if ((rc = launch_tiled_bin(m, b))) return rc;
-            if (serial) return launch_fold(m, m->stream, b.fold, none, 0, true, true);
-            // GEM_B200_PIPE=stream: drain() orders a pending fold after the event of its bin (the untiled bin runs on the
-            // front stream); this bin ran on the map's stream, so the event is recorded there
-            if (m->pipe_mode == 1) GEM_CUDA(m, cudaEventRecord(m->ev_bin[b.sc.par], m->stream));
+            if (serial) return launch_fold(m, b.fold, none, 0, true, true);
             m->pend = b.fold;
             return GEM_OK;
         }
@@ -2793,29 +2718,6 @@ int gem_tiled_step(gem_map *m, const void *xyzi, const void *rgba, int n, const 
     m->launches += 4;
     m->pend = b.fold;
     if (ts.depth != 2) { ts.routed.active = true; ts.routed.step = stepv; ts.routed.buf = bufv; }
-    return GEM_OK;
-}
-
-static int fuse_records_impl(gem_map *m, const void *rec, int n, const int *src_counts, int stride)
-{
-    if (!m || n < 0 || (n > 0 && !rec)) return fail(m, GEM_ERR_INVALID, "gem_fuse_records: bad argument");
-    Lock lk(m->mu);
-    SetDev sd(m->dev);
-    int rc = GEM_OK;
-    memset(&m->stats, 0, sizeof m->stats);
-    if (n == 0) return flush_all_pending(m);
-    for (int off = 0; off < n; off += m->P) {
-        const int cn = (n - off < m->P) ? (n - off) : m->P;
-        BinSource in{};
-        in.rec = (const RouteRec *)rec + off;
-        in.src_counts = src_counts; // counted buffers are never chunked (n <= max_points is checked by the caller)
-        in.stride = stride;
-        const FoldSrc fs{(const char *)in.rec + 16, (int)sizeof(RouteRec)};
-        const FrameParams none{};
-        if ((rc = enqueue_add<SRC_RECORDS>(m, in, fs, cn, none, nullptr, nullptr, false, true, true))) return rc;
-        if (n > m->P && (rc = read_counters(m, cn, true))) return rc;
-    }
-    if (n <= m->P) m->stats.points_in = n;
     return GEM_OK;
 }
 

@@ -125,54 +125,6 @@ k_route_write(const float4 *xyzi, const uchar4 *rgba, int n, int n_owners, const
     }
 }
 
-// ---- peer-memory routing: compute + "collective" in one kernel ------------------------------
-// Instead of bucketing locally and calling an all-to-all, every record is stored straight into the
-// OWNING rank's receive buffer through a peer mapping (NVLink / NVSwitch; torch symmetric memory
-// provides the mappings, gem_b200/tiled.py).  Rank r's records for owner o land in bucket r of o's
-// buffer, in source order, so the receiver sees (source rank, source order) exactly as with the
-// all-to-all.  The per-(source,owner) count goes to the owner's count array the same way.
-struct PeerTable {
-    unsigned long long recv[ROUTE_MAX_OWNERS];   // RouteRec* of every rank's receive buffer (current parity)
-    unsigned long long counts[ROUTE_MAX_OWNERS]; // int* of every rank's per-source count array
-};
-
-__global__ void __launch_bounds__(ROUTE_BLOCK)
-k_route_write_peer(const float4 *xyzi, const uchar4 *rgba, int n, int n_owners, const int *owner_in, const int *gkey_in,
-                   const float *h_in, const float *hv_in, const int *blockOffsets, const int *counts_local,
-                   const __grid_constant__ PeerTable pt, int my_rank, int bucket_stride)
-{
-    __shared__ int s_wcnt[ROUTE_BLOCK / 32][ROUTE_MAX_OWNERS];
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    const unsigned lane = threadIdx.x & 31u;
-    const int w = threadIdx.x >> 5;
-    if (blockIdx.x == 0 && (int)threadIdx.x < n_owners) // publish my bucket sizes to their owners
-        ((int *)pt.counts[threadIdx.x])[my_rank] = counts_local[threadIdx.x];
-    for (int o = (int)lane; o < n_owners; o += 32) s_wcnt[w][o] = 0;
-    __syncwarp();
-    const int owner = (i < n) ? owner_in[i] : -1;
-    const unsigned peers = __match_any_sync(0xffffffffu, owner);
-    const int rank_in_warp = __popc(peers & ((1u << lane) - 1u));
-    if (owner >= 0 && rank_in_warp == 0) s_wcnt[w][owner] = __popc(peers);
-    __syncthreads();
-    if (owner >= 0) {
-        int before = 0;
-        for (int ww = 0; ww < w; ww++) before += s_wcnt[ww][owner];
-        const int pos = blockOffsets[owner * gridDim.x + blockIdx.x] - blockOffsets[owner * gridDim.x] + before + rank_in_warp;
-        RouteRec r;
-        r.gkey = gkey_in[i];
-        r.h = h_in[i];
-        r.var = hv_in[i];
-        r.rgb = 0u;
-        if (rgba) {
-            const uchar4 c = rgba[i];
-            r.rgb = pack_rgb(c.x, c.y, c.z);
-        }
-        r.intensity = xyzi[i].w;
-        RouteRec *dst = (RouteRec *)pt.recv[owner] + (size_t)my_rank * bucket_stride + pos; // peer store over NVLink
-        *dst = r;
-    }
-}
-
 // per-point scratch of the routing passes
 struct RouteScratch {
     int *owner, *gkey;
@@ -182,8 +134,7 @@ struct RouteScratch {
 };
 inline cudaError_t route_points(cudaStream_t st, const MapGeom &g, const FrameParams &fp, const float4 *xyzi,
                                 const uchar4 *rgba, int n, int tiles_r, int tiles_c, const RouteScratch &sc,
-                                RouteRec *out, int *counts_out, int bucket_stride,
-                                const PeerTable *peer = nullptr, int my_rank = 0)
+                                RouteRec *out, int *counts_out, int bucket_stride)
 {
     const int n_owners = tiles_r * tiles_c;
     const int nblocks = n > 0 ? (n + ROUTE_BLOCK - 1) / ROUTE_BLOCK : 1;
@@ -192,11 +143,7 @@ inline cudaError_t route_points(cudaStream_t st, const MapGeom &g, const FramePa
     (any_model(fp) ? k_route_count_any : k_route_count)<<<nblocks, ROUTE_BLOCK, 0, st>>>(
         g, fp, xyzi, n, tile_h, tile_w, tiles_c, n_owners, sc.owner, sc.gkey, sc.h, sc.hv, sc.blockCounts);
     k_route_scan<<<1, 1024, 0, st>>>(sc.blockCounts, n_owners, nblocks, counts_out);
-    if (peer)
-        k_route_write_peer<<<nblocks, ROUTE_BLOCK, 0, st>>>(xyzi, rgba, n, n_owners, sc.owner, sc.gkey, sc.h, sc.hv, sc.blockCounts,
-                                                          counts_out, *peer, my_rank, bucket_stride);
-    else
-        k_route_write<<<nblocks, ROUTE_BLOCK, 0, st>>>(xyzi, rgba, n, n_owners, sc.owner, sc.gkey, sc.h, sc.hv, sc.blockCounts, out, bucket_stride);
+    k_route_write<<<nblocks, ROUTE_BLOCK, 0, st>>>(xyzi, rgba, n, n_owners, sc.owner, sc.gkey, sc.h, sc.hv, sc.blockCounts, out, bucket_stride);
     return cudaGetLastError();
 }
 

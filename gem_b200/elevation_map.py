@@ -759,21 +759,6 @@ class ElevationMap:
     def raytracing_tiled(self, global_lowest):
         check(self._lib.gem_raytracing_tiled(self._h, _ptr(global_lowest)), self._h, "gem_raytracing_tiled")
 
-    def route_points_peer(self, xyzi, rgba, frame: GemFrame, tiles_r: int, tiles_c: int, peer_recv, peer_counts,
-                          my_rank: int, bucket_stride: int):
-        """peer_recv / peer_counts: lists of device addresses (ints), one per rank"""
-        n = int(xyzi.shape[0])
-        no = len(peer_recv)
-        pr = (C.c_ulonglong * no)(*[int(v) for v in peer_recv])
-        pc = (C.c_ulonglong * no)(*[int(v) for v in peer_counts])
-        rc = self._lib.gem_route_points_peer(self._h, _ptr(xyzi), _ptr(rgba), n, C.byref(frame), int(tiles_r), int(tiles_c),
-                                             pr, pc, int(my_rank), int(bucket_stride))
-        check(rc, self._h, "gem_route_points_peer")
-
-    def fuse_records_counted(self, rec, src_counts, n_sources: int, bucket_stride: int):
-        rc = self._lib.gem_fuse_records_counted(self._h, _ptr(rec), _ptr(src_counts), int(n_sources), int(bucket_stride))
-        check(rc, self._h, "gem_fuse_records_counted")
-
     def transform_cloud(self, points32, T):
         """gem_transform_cloud: (n, 8) float32 device tensor of PointXYZRGBICT records, rigidly transformed in place"""
         t = (C.c_float * 16)(*[float(v) for v in np.asarray(T, np.float32).reshape(-1)])

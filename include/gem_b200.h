@@ -180,8 +180,7 @@ int gem_add_points_host(gem_map *m, const void *xyzi_host, const void *rgba_host
  * the next call of any kind that reads or changes the map, by gem_flush or by gem_sync.
  * Contract: the device inputs are read by the bin kernel of this call AND (intensities) by the
  * deferred fold: they must stay valid until two further stream calls have COMPLETED on the
- * stream, or until gem_sync.  n <= max_points.  GEM_B200_PIPE=stream selects two streams +
- * events instead of the graph, GEM_B200_PIPE=off makes this call identical to gem_add_points. */
+ * stream, or until gem_sync.  n <= max_points. */
 int gem_add_points_stream(gem_map *m, const void *xyzi_device, const void *rgba_device, int n,
                           const gem_frame *frame);
 /* Several clouds in one launch (multi-sensor rigs, BASELINE config 5): the device buffers hold
@@ -570,21 +569,6 @@ int gem_fuse_records(gem_map *m, const void *rec_device, int n);
 int gem_get_layer_device(gem_map *m, int layer, void *out_device);
 int gem_compute_features_tiled(gem_map *m, const float *padded_elevation_device);
 int gem_raytracing_tiled(gem_map *m, const float *global_lowest_device);
-
-/* Peer-memory routing (no collective library on the data path): like gem_route_points with a bucket
- * stride, but every record is stored directly into the OWNING rank's receive buffer through a peer
- * mapping (NVLink/NVSwitch): rank r's records for owner o go to peer_recv[o] + r*bucket_stride, its
- * bucket size to ((int*)peer_counts[o])[r].  peer_recv / peer_counts: n_owners device addresses
- * valid on this handle's device (host arrays).  The caller synchronises the ranks (one barrier)
- * before folding with gem_fuse_records_counted. */
-int gem_route_points_peer(gem_map *m, const void *xyzi_device, const void *rgba_device, int n,
-                          const gem_frame *frame, int tiles_r, int tiles_c,
-                          const unsigned long long *peer_recv, const unsigned long long *peer_counts,
-                          int my_rank, int bucket_stride);
-/* fold a receive buffer of n_sources buckets of bucket_stride slots, bucket s filled up to
- * src_counts_device[s] */
-int gem_fuse_records_counted(gem_map *m, const void *rec_device, const int *src_counts_device, int n_sources,
-                             int bucket_stride);
 
 /* ---- loop-closure re-fusion of submaps (ElevationMapping::updateGlobalMap, ElevationMapping.cpp:773-905; SURVEY 8f row 4) ----
  * Submaps are arrays of 32-byte PointXYZRGBICT records in device memory (what gem_harvest_scrolled_out produces).

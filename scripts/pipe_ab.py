@@ -1,5 +1,5 @@
-"""A/B of the frame pipeline of gem_add_points_stream: GEM_B200_PIPE = graph | stream | off, plus the plain
-gem_add_points call.  Prints us/frame (device, CUDA events on the handle's stream) and the host enqueue time."""
+"""A/B of the frame pipeline: gem_add_points_stream (one CUDA graph per call, `graph`) against the plain
+gem_add_points call (`plain`).  Prints us/frame (device, CUDA events on the handle's stream) and the host enqueue time."""
 import os, sys, time, ctypes as C
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np, torch
@@ -16,8 +16,7 @@ npts = [fr["xyzi"].shape[0] for fr in frames]
 pos_c = [(C.c_float * 3)(*[float(v) for v in fr["position"]]) for fr in frames]
 xp = [C.c_void_p(t.data_ptr()) for t in xd]; rp = [C.c_void_p(t.data_ptr()) for t in rd]
 fref = [C.byref(f) for f in fobjs]
-for mode in (sys.argv[1:] or ["graph", "stream", "off", "plain"]):
-    os.environ["GEM_B200_PIPE"] = mode if mode != "plain" else "off"
+for mode in (sys.argv[1:] or ["graph", "plain"]):
     m = gem_b200.ElevationMap(1024, 0.05, compat_box_filter=False)
     st = m.torch_stream()
     def step(s):

@@ -9,7 +9,7 @@ bands, and every cell after the first fuse, after a negative gem_var_update and 
 
 Every hand-written script below targets one of those decisions and is named after it; tests/test_sequence_cases.py
 checks on the oracle alone that each one reaches its hazard, tests/test_sequences_gpu.py runs every script on the
-device under each schedule (GEM_B200_PIPE, profiling, GEM_B200_EXCLUSIVE, GEM_B200_FOLD_BLOCKS) against the oracle.
+device under each schedule (the default graph, profiling, GEM_B200_EXCLUSIVE, GEM_B200_FOLD_BLOCKS) against the oracle.
 
 A script is a list of steps (op, args).  Ops:
   move pos                       gem_move; the state and the returned centre / start / shift are compared

@@ -10,53 +10,36 @@ import pytest
 from gem_b200 import build
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-EXE = os.path.join(ROOT, "tests", "cxx", "facade_smoke")
 
 
-def compile_program():
+def compile_with_shim(out_dir, name, extra_flags=()):
+    """tests/cxx/<name>.cpp + the shim, linked against libgem_b200.so, built into out_dir (the tree may be read-only)"""
     lib = build.build()
-    srcs = [os.path.join(ROOT, "tests", "cxx", "facade_smoke.cpp"), os.path.join(ROOT, "compat", "gpu_process_shim.cpp")]
-    deps = srcs + [lib, os.path.join(ROOT, "include", "gem_b200.h"), os.path.join(ROOT, "include", "gem_b200", "elevation_map.hpp")]
-    if os.path.exists(EXE) and all(os.path.getmtime(d) <= os.path.getmtime(EXE) for d in deps):
-        return EXE
-    cmd = ["g++", "-O2", "-std=c++14", "-Wall", "-I", os.path.join(ROOT, "include"), "-I", os.path.join(ROOT, "oracle", "mini_eigen"),
-           "-o", EXE] + srcs + ["-L", os.path.dirname(lib), "-lgem_b200", "-Wl,-rpath," + os.path.dirname(lib)]
+    exe = os.path.join(str(out_dir), name)
+    srcs = [os.path.join(ROOT, "tests", "cxx", name + ".cpp"), os.path.join(ROOT, "compat", "gpu_process_shim.cpp")]
+    cmd = ["g++", "-O2", "-std=c++14", "-Wall", *extra_flags, "-I", os.path.join(ROOT, "include"), "-I", os.path.join(ROOT, "oracle", "mini_eigen"),
+           "-o", exe] + srcs + ["-L", os.path.dirname(lib), "-lgem_b200", "-Wl,-rpath," + os.path.dirname(lib)]
     subprocess.run(cmd, check=True)
-    return EXE
+    return exe
 
 
-THREADS_EXE = os.path.join(ROOT, "tests", "cxx", "threads_shim")
-
-
-def compile_threads_program():
-    lib = build.build()
-    srcs = [os.path.join(ROOT, "tests", "cxx", "threads_shim.cpp"), os.path.join(ROOT, "compat", "gpu_process_shim.cpp")]
-    deps = srcs + [lib, os.path.join(ROOT, "include", "gem_b200.h")]
-    if os.path.exists(THREADS_EXE) and all(os.path.getmtime(d) <= os.path.getmtime(THREADS_EXE) for d in deps):
-        return THREADS_EXE
-    cmd = ["g++", "-O2", "-std=c++14", "-Wall", "-pthread", "-I", os.path.join(ROOT, "include"), "-I", os.path.join(ROOT, "oracle", "mini_eigen"),
-           "-o", THREADS_EXE] + srcs + ["-L", os.path.dirname(lib), "-lgem_b200", "-Wl,-rpath," + os.path.dirname(lib)]
-    subprocess.run(cmd, check=True)
-    return THREADS_EXE
-
-
-def test_three_thread_program_compiles():
-    assert os.path.exists(compile_threads_program())
+def test_three_thread_program_compiles(tmp_path):
+    assert os.path.exists(compile_with_shim(tmp_path, "threads_shim", ["-pthread"]))
 
 
 @pytest.mark.gpu
-def test_node_threading_through_the_shim():
+def test_node_threading_through_the_shim(tmp_path):
     """the node's three threads (Process_points outside MapMutex_, ElevationMapping.cpp:271-282) through the unmodified
     shim: no failures, sane map"""
-    exe = compile_threads_program()
+    exe = compile_with_shim(tmp_path, "threads_shim", ["-pthread"])
     r = subprocess.run([exe], capture_output=True, text=True, timeout=300)
     print(r.stdout, r.stderr[-2000:])
     assert r.returncode == 0 and "failures=0" in r.stdout, r.stdout + r.stderr[-2000:]
     assert "failed" not in r.stderr
 
 
-def test_facade_and_shim_compile_and_link():
-    exe = compile_program()
+def test_facade_and_shim_compile_and_link(tmp_path):
+    exe = compile_with_shim(tmp_path, "facade_smoke")
     assert os.path.exists(exe)
     out = subprocess.run(["nm", "-C", "--defined-only", exe], capture_output=True, text=True).stdout
     for sym in ("Init_GPU_elevationmap(int, float, float, float)", "Raytracing(int)", "Map_closeloop(float*, float, int, float)",
@@ -65,8 +48,8 @@ def test_facade_and_shim_compile_and_link():
 
 
 @pytest.mark.gpu
-def test_facade_and_shim_run_and_agree():
-    exe = compile_program()
+def test_facade_and_shim_run_and_agree(tmp_path):
+    exe = compile_with_shim(tmp_path, "facade_smoke")
     r = subprocess.run([exe], capture_output=True, text=True, timeout=300)
     print(r.stdout, r.stderr)
     assert r.returncode == 0, r.stdout + r.stderr

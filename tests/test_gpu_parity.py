@@ -702,7 +702,6 @@ def test_error_paths_return_codes():
     assert lib.gem_add_points(g.handle, None, None, -1, C.byref(f)) == 1
     assert lib.gem_get_layer(g.handle, 99, None) == 1
     assert lib.gem_add_points_multi(g.handle, None, None, 0, None, None) == 1
-    assert lib.gem_fuse_records_counted(g.handle, None, None, 0, 0) == 1
     t = gem_b200.ElevationMap(64, 0.1, tile=(0, 64, 0, 32))
     with pytest.raises(gem_b200.GemError):
         t.compute_features()                                                         # tiled handles: not implemented

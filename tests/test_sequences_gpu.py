@@ -1,7 +1,6 @@
 """The call scripts of tests/sequence_cases.py on the device map and the oracle side by side, under every schedule the
-add path has: one CUDA graph per call (the default), the bin on a second stream ordered by events, fully serial,
-profiling on (serial, with per-kernel event timing), the padded shared-memory launch of GEM_B200_EXCLUSIVE and a small
-GEM_B200_FOLD_BLOCKS cap.  At every reader and at the end of a script everything observable is compared bit for bit:
+add path has: one CUDA graph per call (the default), profiling on (fully serial, with per-kernel event timing), the
+padded shared-memory launch of GEM_B200_EXCLUSIVE and a small GEM_B200_FOLD_BLOCKS cap.  At every reader and at the end of a script everything observable is compared bit for bit:
 all layers, the state after each move, map_feature, the exports, the orthomosaic, the visual cloud, harvested records,
 process_points outputs and stats().  A difference names the script, the step and the schedule."""
 import ctypes as C
@@ -16,13 +15,11 @@ pytestmark = pytest.mark.gpu
 
 SCHEDULES = {
     "graph": {},
-    "stream": {"GEM_B200_PIPE": "stream"},
-    "off": {"GEM_B200_PIPE": "off"},
     "profile": {},
     "exclusive": {"GEM_B200_EXCLUSIVE": "1"},
     "fold_blocks_8": {"GEM_B200_FOLD_BLOCKS": "8"},
 }
-ENV = ("GEM_B200_PIPE", "GEM_B200_EXCLUSIVE", "GEM_B200_FOLD_BLOCKS", "GEM_B200_LONG_BLOCKS")
+ENV = ("GEM_B200_EXCLUSIVE", "GEM_B200_FOLD_BLOCKS", "GEM_B200_LONG_BLOCKS")
 _ORACLE = {}
 
 

@@ -6,7 +6,7 @@ out its symmetric-memory buffers (records int32 [5, W*cap, 4], intensities float
 zeroed, flags int32 [64] zeroed, one set per rank); their addresses go to ElevationMap.tiled_attach.
 
 * World 1: one tile owns the map.  Its bin waits only on its own flag, raised by a route ordered before it, so every
-  schedule runs: off, stream, graph at depth 2 and graph at depth 3.
+  schedule runs: serial with profiling on, graph at depth 2 and graph at depth 3.
 * One rank of a W-rank tiling, the other ranks absent: the foreign words of the rank's own flag array are preset to
   INT32_MAX and the foreign counts stay zero, so its bin never waits.  What the route stored into every owner's buffer
   (slots, counts, flags) is checked record by record against a numpy model of the routing.
@@ -27,12 +27,11 @@ from oracle_lib import OracleMap
 pytestmark = pytest.mark.gpu
 
 LAYERS = ["elevation", "variance", "intensity", "color_r", "color_g", "color_b", "lowest"]
-ENV = ("GEM_B200_PIPE", "GEM_B200_TILED_DEPTH", "GEM_B200_EXCLUSIVE", "GEM_B200_FOLD_BLOCKS", "GEM_B200_LONG_BLOCKS")
+ENV = ("GEM_B200_TILED_DEPTH", "GEM_B200_EXCLUSIVE", "GEM_B200_FOLD_BLOCKS", "GEM_B200_LONG_BLOCKS")
 SCHEDULES = {
-    "off": {"GEM_B200_PIPE": "off"},
-    "stream": {"GEM_B200_PIPE": "stream"},
-    "graph_depth2": {"GEM_B200_PIPE": "graph", "GEM_B200_TILED_DEPTH": "2"},
-    "graph_depth3": {"GEM_B200_PIPE": "graph", "GEM_B200_TILED_DEPTH": "3"},
+    "profile": {},                           # gem_profile_enable: every step routed, binned and folded inside its call
+    "graph_depth2": {"GEM_B200_TILED_DEPTH": "2"},
+    "graph_depth3": {"GEM_B200_TILED_DEPTH": "3"},
 }
 RES = 0.1
 INT32_MAX = 2**31 - 1
@@ -290,6 +289,8 @@ def test_world1_steps_match_oracle(schedule, monkeypatch):
     L = 256
     bufs = PeerBuffers(1, CAP)
     g = _tile_map(L, 0, 1, CAP)
+    if schedule == "profile":
+        g.profile_enable()
     o = OracleMap(L, RES, compat_box_filter=False)
     keep = []
     step, last_n, last_binned, stats = 0, 0, 0, None
