@@ -5,25 +5,8 @@
 #include "gem_add.cuh"
 using namespace gem;
 
-__device__ __forceinline__ void fold_chunk_inl(CellState &s, const uint4 r, int m)
-{
-    uint32_t nh = __shfl_sync(0xffffffffu, r.y, 0), nv = __shfl_sync(0xffffffffu, r.z, 0);
-    uint32_t nc = __shfl_sync(0xffffffffu, r.w, 0), nx = __shfl_sync(0xffffffffu, r.x, 0);
-    bool rare = false;
-    for (int t = 0; t < m; t++) {
-        const float h = __uint_as_float(nh), v = __uint_as_float(nv);
-        const uint32_t rgb = nc, x = nx;
-        const int tn = (t + 1) & 31;
-        nh = __shfl_sync(0xffffffffu, r.y, tn);
-        nv = __shfl_sync(0xffffffffu, r.z, tn);
-        nc = __shfl_sync(0xffffffffu, r.w, tn);
-        nx = __shfl_sync(0xffffffffu, r.x, tn);
-        rare |= fold_step_fast(s, h, v, rgb, x, __uint_as_float(x));
-    }
-    if (__any_sync(0xffffffffu, rare)) s.elev += 1.0f;
-}
-
-// mode 0: inlined chunk loop; 1: the library's noinline fold_chunk.  busy: warps 1.. of the block spin on ALU work.
+// mode 0: the general path alone (fold_chunk_general); 1: the library's fold_chunk, plain path first.  busy: warps 1..
+// of the block spin on ALU work.
 __global__ void k_micro(const uint4 *rec, int k, int mode, int busy_iters, float *out, long long *cyc)
 {
     const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -34,7 +17,7 @@ __global__ void k_micro(const uint4 *rec, int k, int mode, int busy_iters, float
         for (int c0 = 0; c0 < k; c0 += 32) {
             uint4 r = make_uint4(0, 0, 0, 0);
             if (c0 + lane < k) r = rec[c0 + lane];
-            if (mode == 0) fold_chunk_inl(s, r, min(32, k - c0));
+            if (mode == 0) { if (fold_chunk_general(s, r, min(32, k - c0))) s.elev += 1.0f; }
             else fold_chunk(s, r, min(32, k - c0), true);
         }
         const long long t1 = clock64();
@@ -67,7 +50,7 @@ int main()
                     cudaDeviceSynchronize();
                 }
                 cudaMemcpy(&hc, c, 8, cudaMemcpyDeviceToHost);
-                printf("mode %d (%s) warps/block %2d busy %6d : %6.1f cycles/record (%lld cycles for k=%d) %s\n", mode, mode ? "noinline lib fold_chunk" : "inlined", nwarps, busy,
+                printf("mode %d (%s) warps/block %2d busy %6d : %6.1f cycles/record (%lld cycles for k=%d) %s\n", mode, mode ? "fold_chunk" : "fold_chunk_general", nwarps, busy,
                        (double)hc / k, hc, k, cudaGetErrorString(cudaGetLastError()));
             }
     return 0;
