@@ -22,11 +22,18 @@ void Map_optmove(float *opt_p, float height_update, float resolution, int length
 void Mapvar_update(int length, float var_update);
 int Process_points(int *mapindex, float *point_x, float *point_y, float *point_z, float *point_var, float *point_x_ts, float *point_y_ts, float *point_z_ts, Eigen::Matrix4f Transform, int point_num, double relativeLowerThreshold, double relativeUpperThreshold, float min_r, float beam_a, float beam_c, Eigen::RowVector3f sensorJacobian, Eigen::Matrix3f rotationVariance, Eigen::Matrix3f C_SB_transpose, Eigen::RowVector3f P_mul_C_BM_transpose, Eigen::Matrix3f B_r_BS_skew);
 
-// device-global layer pointers of the reference (gpu_process.cu:20-28); needs -rdc=true
+// device-global layer pointers and scroll state of the reference (gpu_process.cu:20-33); needs -rdc=true
 extern __device__ float *map_lowest;
 extern __device__ float *map_traver;
 extern __device__ float *map_elevation;
 extern __device__ float *map_variance;
+extern __device__ float *map_intensity;
+extern __device__ int *map_colorR;
+extern __device__ int *map_colorG;
+extern __device__ int *map_colorB;
+extern __device__ float central_coordinate[2];
+extern __device__ int start_indice[2];
+extern __device__ float sensorZatLowestScan;
 
 static int g_length = 0;
 
@@ -84,23 +91,35 @@ void ref_closeloop(float p[2], float height_update, float resolution)
     Map_closeloop(p, height_update, g_length, resolution);
     cudaDeviceSynchronize();
 }
-// read / write one of the reference's device layers (0 lowest, 1 traver, 2 elevation, 3 variance)
-static float *layer_ptr(int which)
+// read / write one of the reference's device layers (0 lowest, 1 traver, 2 elevation, 3 variance, 4 intensity,
+// 5 colorR, 6 colorG, 7 colorB); every layer has 4-byte elements (float or int)
+static void *layer_ptr(int which)
 {
-    float *p = nullptr;
+    void *p = nullptr;
     if (which == 0) cudaMemcpyFromSymbol(&p, map_lowest, sizeof p);
     else if (which == 1) cudaMemcpyFromSymbol(&p, map_traver, sizeof p);
     else if (which == 2) cudaMemcpyFromSymbol(&p, map_elevation, sizeof p);
-    else cudaMemcpyFromSymbol(&p, map_variance, sizeof p);
+    else if (which == 3) cudaMemcpyFromSymbol(&p, map_variance, sizeof p);
+    else if (which == 4) cudaMemcpyFromSymbol(&p, map_intensity, sizeof p);
+    else if (which == 5) cudaMemcpyFromSymbol(&p, map_colorR, sizeof p);
+    else if (which == 6) cudaMemcpyFromSymbol(&p, map_colorG, sizeof p);
+    else cudaMemcpyFromSymbol(&p, map_colorB, sizeof p);
     return p;
 }
-void ref_get_layer(int which, float *host_out)
+void ref_get_layer(int which, void *host_out)
 {
-    cudaMemcpy(host_out, layer_ptr(which), sizeof(float) * g_length * g_length, cudaMemcpyDeviceToHost);
+    cudaMemcpy(host_out, layer_ptr(which), 4 * (size_t)g_length * g_length, cudaMemcpyDeviceToHost);
 }
-void ref_set_layer(int which, const float *host_in)
+void ref_set_layer(int which, const void *host_in)
 {
-    cudaMemcpy(layer_ptr(which), host_in, sizeof(float) * g_length * g_length, cudaMemcpyHostToDevice);
+    cudaMemcpy(layer_ptr(which), host_in, 4 * (size_t)g_length * g_length, cudaMemcpyHostToDevice);
+}
+// the scroll state Move, Map_optmove and Map_closeloop keep in device globals (gpu_process.cu:30-33)
+void ref_get_state(float centre_out[2], int start_out[2], float *sensor_z_out)
+{
+    cudaMemcpyFromSymbol(centre_out, central_coordinate, sizeof(float) * 2);
+    cudaMemcpyFromSymbol(start_out, start_indice, sizeof(int) * 2);
+    cudaMemcpyFromSymbol(sensor_z_out, sensorZatLowestScan, sizeof(float));
 }
 int ref_last_cuda_error(void) { return (int)cudaGetLastError(); }
 

@@ -78,16 +78,42 @@ class RefMap:
     def raytracing(self):
         self.lib.ref_raytracing()
 
+    def opt_move(self, opt_p, height_update):
+        """Map_optmove: returns the aligned position it moved the centre to"""
+        p = np.array(opt_p, np.float32, copy=True)
+        out = np.zeros(2, np.float32)
+        self.lib.ref_optmove(_p(p), C.c_float(height_update), C.c_float(self.res), _p(out))
+        return out
+
+    def closeloop(self, update_position, height_update):
+        p = np.array(update_position, np.float32, copy=True)
+        self.lib.ref_closeloop(_p(p), C.c_float(height_update), C.c_float(self.res))
+
+    def state(self):
+        """(central_coordinate, start_indice, [sensorZatLowestScan]) as float32[2], int32[2], float32[1]"""
+        centre, start, sz = np.zeros(2, np.float32), np.zeros(2, np.int32), np.zeros(1, np.float32)
+        self.lib.ref_get_state(_p(centre), _p(start), _p(sz))
+        return centre, start, sz
+
     def get_layer(self, name):
-        which = {"lowest": 0, "traver": 1, "elevation": 2, "variance": 3}[name]
-        out = np.empty(self.L * self.L, np.float32)
+        which, dtype = LAYERS[name]
+        out = np.empty(self.L * self.L, dtype)
         self.lib.ref_get_layer(which, _p(out))
         return out.reshape(self.L, self.L)
 
+    def layers(self, names):
+        return {n: self.get_layer(n) for n in names}
+
     def set_layer(self, name, arr):
-        which = {"lowest": 0, "traver": 1, "elevation": 2, "variance": 3}[name]
-        a = np.ascontiguousarray(arr, np.float32).reshape(-1)
+        which, dtype = LAYERS[name]
+        a = np.ascontiguousarray(arr, dtype).reshape(-1)
+        assert a.shape[0] == self.L * self.L, (name, a.shape)
         self.lib.ref_set_layer(which, _p(a))
+
+
+# the reference's device layers the harness reads and writes: name -> (harness index, element type)
+LAYERS = {"lowest": (0, np.float32), "traver": (1, np.float32), "elevation": (2, np.float32), "variance": (3, np.float32),
+          "intensity": (4, np.float32), "color_r": (5, np.int32), "color_g": (6, np.int32), "color_b": (7, np.int32)}
 
 
 def _bytes(a):
@@ -114,6 +140,41 @@ def rebuild(like, x):
     """the reference's array, bit for bit, from the oracle's array it was stored against and the stored XOR"""
     like = np.ascontiguousarray(like)
     return np.bitwise_xor(_bytes(like), x).view(like.dtype).reshape(like.shape)
+
+
+def pack(store):
+    """a recording as a few arrays instead of two per call: every stored XOR one after the other (`xor`, lengths
+    `xor_len`, in the order of `keys`) and the oracle digests as raw bytes (`oracle_sha256`, one row of 32 per key);
+    other entries are kept as they are.  Packed(np.load(...)) reads it back with the store's interface."""
+    keys = sorted(k[:-4] for k in store if k.endswith("_xor"))
+    xs = [np.asarray(store[k + "_xor"], np.uint8) for k in keys]
+    out = {k: v for k, v in store.items() if not (k.endswith("_xor") or k.endswith("_oracle_sha256"))}
+    out["keys"] = np.array(keys)
+    out["xor"] = np.concatenate(xs) if xs else np.zeros(0, np.uint8)
+    out["xor_len"] = np.array([x.size for x in xs], np.int64)
+    out["oracle_sha256"] = np.array([np.frombuffer(bytes.fromhex(str(store[k + "_oracle_sha256"])), np.uint8)
+                                     for k in keys], np.uint8).reshape(len(keys), 32)
+    return out
+
+
+class Packed:
+    """the store interface (store[tag_n + "_xor"], store[tag_n + "_oracle_sha256"]) over a packed recording"""
+
+    def __init__(self, npz):
+        keys = [str(k) for k in npz["keys"]]
+        ends = np.cumsum(npz["xor_len"])
+        self._xor = npz["xor"]
+        self._at = {k: (int(e - n), int(e)) for k, e, n in zip(keys, ends, npz["xor_len"])}
+        self._sha = {k: bytes(row).hex() for k, row in zip(keys, npz["oracle_sha256"])}
+        self._other = {k: npz[k] for k in npz.files if k not in ("keys", "xor", "xor_len", "oracle_sha256")}
+
+    def __getitem__(self, key):
+        if key.endswith("_xor"):
+            a, b = self._at[key[:-4]]
+            return self._xor[a:b]
+        if key.endswith("_oracle_sha256"):
+            return np.array(self._sha[key[:-len("_oracle_sha256")]])
+        return self._other[key]
 
 
 class PinnedRef:
@@ -148,8 +209,15 @@ class PinnedRef:
             return tuple(self._pin(a, None if out is None else b) for a, b in zip(like, out or (None,) * len(like)))
         return self._pin(like, out)
 
-    def _call(self, like, method, *args):
-        return self._pin_all(like, getattr(self.live, method)(*args) if self.live is not None else None)
+    def _call(self, like, method, *args, derive=None):
+        """derive: a function of the reference's output to pin instead of the output itself (e.g. some cells only,
+        where the reference leaves the rest uninitialised); `like` is then the same function of the oracle's output"""
+        out = None
+        if self.live is not None:
+            out = getattr(self.live, method)(*args)
+            if derive is not None:
+                out = derive(out)
+        return self._pin_all(like, out)
 
     def move(self, pos, like):
         return self._call(like, "move", pos)
@@ -157,11 +225,20 @@ class PinnedRef:
     def process_points(self, x, y, z, frame, like):
         return self._call(like, "process_points", x, y, z, frame)
 
-    def map_feature(self, like):
-        return self._call(like, "map_feature")
+    def map_feature(self, like, derive=None):
+        return self._call(like, "map_feature", derive=derive)
 
-    def get_layer(self, name, like):
-        return self._call(like, "get_layer", name)
+    def layers(self, names, like):
+        return self._call(like, "layers", names)
+
+    def get_layer(self, name, like, derive=None):
+        return self._call(like, "get_layer", name, derive=derive)
+
+    def opt_move(self, opt_p, height_update, like):
+        return self._call(like, "opt_move", opt_p, height_update)
+
+    def state(self, like):
+        return self._call(like, "state")
 
     def fuse_points(self, *args):
         if self.live is not None:
@@ -170,6 +247,14 @@ class PinnedRef:
     def raytracing(self):
         if self.live is not None:
             self.live.raytracing()
+
+    def var_update(self, dv):
+        if self.live is not None:
+            self.live.var_update(dv)
+
+    def closeloop(self, update_position, height_update):
+        if self.live is not None:
+            self.live.closeloop(update_position, height_update)
 
     def set_layer(self, name, arr):
         if self.live is not None:
