@@ -2,5 +2,5 @@
 hot path (the reference's libgpu.so).  The product is the CUDA library behind include/gem_b200.h;
 this package is its Python host mirror used by tests and benchmarks."""
 from ._lib import GemError, GemFrame, GemSensorModel, load  # noqa: F401
-from .elevation_map import (ElevationMap, LaserSensorProcessor, PerfectSensorProcessor,  # noqa: F401
-                            StereoSensorProcessor, StructuredLightSensorProcessor, make_frame)
+from .elevation_map import (CameraImage, ElevationMap, LaserSensorProcessor, PerfectSensorProcessor,  # noqa: F401
+                            PointCloud2Layout, StereoSensorProcessor, StructuredLightSensorProcessor, make_frame)

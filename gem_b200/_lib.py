@@ -106,10 +106,37 @@ class GemMlsInfo(C.Structure):
                 ("max_neighbours", C.c_int)]
 
 
+class GemPointField(C.Structure):
+    _fields_ = [("name", C.c_char * 32), ("offset", C.c_uint), ("datatype", C.c_ubyte), ("count", C.c_uint)]
+
+
+class GemPointCloud2(C.Structure):
+    _fields_ = [("width", C.c_uint), ("height", C.c_uint), ("point_step", C.c_uint), ("row_step", C.c_uint),
+                ("is_bigendian", C.c_ubyte), ("nfields", C.c_int), ("fields", C.POINTER(GemPointField))]
+
+
+class GemPc2Span(C.Structure):
+    _fields_ = [("serialized_offset", C.c_uint), ("struct_offset", C.c_uint), ("size", C.c_uint)]
+
+
+class GemPc2Mapping(C.Structure):
+    _fields_ = [("nspans", C.c_int), ("spans", GemPc2Span * 7), ("fast_path", C.c_int), ("matched", C.c_uint),
+                ("points", C.c_longlong), ("bytes", C.c_ulonglong)]
+
+
+class GemCameraImage(C.Structure):
+    _fields_ = [("T_camera", C.c_double * 12), ("T_lidar", C.c_double * 16), ("encoding", C.c_char * 32), ("width", C.c_int),
+                ("height", C.c_int), ("step", C.c_int), ("data", C.c_void_p)]
+
+
 COST_FREE, COST_LETHAL, COST_UNKNOWN = 0, 254, 255           # GEM_COST_*
 COSTMAP_MODES = {"max": 0, "overwrite": 1}                  # GEM_COSTMAP_MAX / GEM_COSTMAP_OVERWRITE
 VOXEL_FIELDS = {None: -1, "x": 0, "y": 1, "z": 2, "intensity": 3}  # GEM_VOXEL_FIELD_*
 MLS_UPSAMPLING = {"none": 0, "random_uniform_density": 1}  # GEM_MLS_*
+# sensor_msgs/PointField datatypes (GEM_PF_*) and the PointXYZRGBICT fields in registration order (GEM_PC2_*)
+POINTFIELD_TYPES = {"int8": 1, "uint8": 2, "int16": 3, "uint16": 4, "int32": 5, "uint32": 6, "float32": 7, "float64": 8}
+PC2_FIELDS = ["x", "y", "z", "rgb", "intensity", "covariance", "travers"]
+IMAGE_ENCODINGS = {"bgr8": 3, "rgb8": 3, "bgra8": 4, "rgba8": 4, "mono8": 1}   # the byte-permutation encodings: channels
 
 PROF_CLASSES = ["bin", "fold_long", "unused", "fold", "clear_floor", "features", "raytrace", "other", "route"]
 
@@ -184,6 +211,11 @@ SYMBOLS = {
     "gem_refuse_submaps": (C.c_int, [_P, _P, _IP, _P, _IP, C.c_double, C.c_int, _IP]),
     "gem_tiled_attach": (C.c_int, [_P, C.POINTER(GemTiledPeers)]),
     "gem_tiled_step": (C.c_int, [_P, _P, _P, C.c_int, C.POINTER(GemFrame)]),
+    "gem_pointcloud2_mapping": (C.c_int, [C.POINTER(GemPointCloud2), C.c_ulonglong, C.POINTER(GemPc2Mapping)]),
+    "gem_decode_pointcloud2": (C.c_int, [_P, C.POINTER(GemPointCloud2), _P, C.c_ulonglong, _P]),
+    "gem_image_to_bgr8": (C.c_int, [_P, C.c_char_p, _P, C.c_int, C.c_int, C.c_int, _P, C.c_int]),
+    "gem_add_pointcloud2_host_async": (C.c_int, [_P, C.POINTER(GemPointCloud2), _P, C.c_ulonglong, C.POINTER(GemCameraImage),
+                                                 C.POINTER(GemFrame)]),
 }
 
 _lib = None

@@ -27,6 +27,7 @@
 #include "gem_costmap.cuh"
 #include "gem_kernels.cuh"
 #include "gem_global.cuh"
+#include "gem_ingest.cuh"
 #include "gem_mls.cuh"
 #include "gem_octree.cuh"
 #include "gem_route.cuh"
@@ -163,6 +164,9 @@ struct gem_map {
     cudaEvent_t ev_h2d[3] = {nullptr, nullptr, nullptr}, ev_done[3] = {nullptr, nullptr, nullptr};
     BinCounters *h_ctr_ring = nullptr; // pinned, 2 entries
     unsigned async_calls = 0;
+    // gem_add_pointcloud2_host_async: per ring slot the message bytes and the camera image as they arrive (copy
+    // stream), and one BGR8 conversion target (handle's stream); grown on demand
+    OctBuf pc2_raw[3], pc2_img[3], pc2_bgr;
     // gem_add_points_multi: ring of per-call FrameParams tables (pinned host + device)
     FrameParams *h_frames = nullptr, *d_frames = nullptr;
     cudaEvent_t ev_frames[4] = {nullptr, nullptr, nullptr, nullptr};
@@ -857,7 +861,8 @@ int gem_destroy(gem_map *m)
                           &m->oct.dense, &m->cost_scratch, &m->vox.key[0], &m->vox.key[1], &m->vox.idx[0], &m->vox.idx[1],
                           &m->vox.cnt, &m->vox.off, &m->vox.temp, &m->vox.acc, &m->mls.key[0], &m->mls.key[1], &m->mls.idx[0],
                           &m->mls.idx[1], &m->mls.spts, &m->mls.ukey, &m->mls.ucnt, &m->mls.uoff, &m->mls.nbr, &m->mls.ocnt,
-                          &m->mls.ooff, &m->mls.longs, &m->mls.lkeys, &m->mls.temp, &m->mls.acc})
+                          &m->mls.ooff, &m->mls.longs, &m->mls.lkeys, &m->mls.temp, &m->mls.acc, &m->pc2_raw[0],
+                          &m->pc2_raw[1], &m->pc2_raw[2], &m->pc2_img[0], &m->pc2_img[1], &m->pc2_img[2], &m->pc2_bgr})
             if (b->p) cudaFree(b->p);
         if (m->h_ctr) cudaFreeHost(m->h_ctr);
         if (m->h_ctr_ring) cudaFreeHost(m->h_ctr_ring);
@@ -1114,15 +1119,11 @@ int gem_add_points_multi(gem_map *m, const void *xyzi, const void *rgba, int n_s
     return GEM_OK;
 }
 
-int gem_add_points_host_async(gem_map *m, const void *xyzi, const void *rgba, int n, const gem_frame *frame)
+// gem_add_points_host_async / gem_add_pointcloud2_host_async: lazy set-up of the shared ring (every handle created at most
+// once, also after a partial failure): copy stream, three staging sets, events, counter ring
+static int ensure_async_ring(gem_map *m)
 {
-    if (!m || !frame || n < 0 || (n > 0 && !xyzi) || !sensor_ok(frame->sensor)) return fail(m, GEM_ERR_INVALID, "gem_add_points_host_async: bad argument");
-    if (n > m->P) return fail(m, GEM_ERR_INVALID, "gem_add_points_host_async: n exceeds max_points (use gem_add_points_host)");
-    Lock lk(m->mu);
-    SetDev sd(m->dev);
     int rc = GEM_OK;
-    // lazy set-up (every handle created at most once, also after a partial failure): copy stream, three staging
-    // sets, events, counter ring
     if (!m->copy_stream) GEM_CUDA(m, cudaStreamCreateWithFlags(&m->copy_stream, cudaStreamNonBlocking));
     for (int i = 0; i < 3; i++) {
         if (!m->d_axyzi[i] && (rc = dev_alloc(m, (float4 **)&m->d_axyzi[i], (size_t)m->P))) return rc;
@@ -1134,6 +1135,37 @@ int gem_add_points_host_async(gem_map *m, const void *xyzi, const void *rgba, in
         }
     }
     if (!m->h_ctr_ring) GEM_CUDA(m, cudaHostAlloc((void **)&m->h_ctr_ring, 2 * sizeof(BinCounters), cudaHostAllocDefault));
+    return GEM_OK;
+}
+
+// the pipelined add of ring call i, whose points are in staging set i % 3 on the handle's stream
+static int async_add_slot(gem_map *m, unsigned i, int n, bool rgba, const gem_frame *frame)
+{
+    const int b = (int)(i % 3u);
+    const FrameParams fp = make_frame(frame);
+    const BinSource in = xyzi_source(m->d_axyzi[b], rgba ? m->d_argba[b] : nullptr, 0);
+    const FoldSrc fs{in.xyzi ? (const char *)in.xyzi + 12 : nullptr, 16};
+    BinCounters *prev_ctr = m->pend.active ? m->pend.sc.ctr : nullptr;
+    int rc = enqueue_add<SRC_XYZI>(m, in, fs, n, fp, nullptr, nullptr, true, true, true);
+    if (rc) return rc;
+    // the step's host-visible result: the counters of the newest call whose fold has been issued
+    GEM_CUDA(m, cudaMemcpyAsync(&m->h_ctr_ring[i & 1u], prev_ctr ? prev_ctr : m->ctr_last, sizeof(BinCounters), cudaMemcpyDeviceToHost, m->stream));
+    // staging set (i-1) % 3 was last read by the fold just issued (or by this call's own fold in the serial fallback)
+    GEM_CUDA(m, cudaEventRecord(m->ev_done[(i + 2u) % 3u], m->stream));
+    if (!m->pend.active) GEM_CUDA(m, cudaEventRecord(m->ev_done[b], m->stream));
+    memset(&m->stats, 0, sizeof m->stats);
+    m->stats.points_in = n; // the rest is fetched by gem_get_stats
+    return GEM_OK;
+}
+
+int gem_add_points_host_async(gem_map *m, const void *xyzi, const void *rgba, int n, const gem_frame *frame)
+{
+    if (!m || !frame || n < 0 || (n > 0 && !xyzi) || !sensor_ok(frame->sensor)) return fail(m, GEM_ERR_INVALID, "gem_add_points_host_async: bad argument");
+    if (n > m->P) return fail(m, GEM_ERR_INVALID, "gem_add_points_host_async: n exceeds max_points (use gem_add_points_host)");
+    Lock lk(m->mu);
+    SetDev sd(m->dev);
+    int rc = ensure_async_ring(m);
+    if (rc) return rc;
     if (n == 0) return flush_all_pending(m);
     const unsigned i = m->async_calls++;
     const int b = (int)(i % 3u);
@@ -1144,19 +1176,7 @@ int gem_add_points_host_async(gem_map *m, const void *xyzi, const void *rgba, in
     GEM_CUDA(m, cudaEventRecord(m->ev_h2d[b], m->copy_stream));
     // compute stream: wait for the copy, issue {fold of the previous call || bin of this one}
     GEM_CUDA(m, cudaStreamWaitEvent(m->stream, m->ev_h2d[b], 0));
-    const FrameParams fp = make_frame(frame);
-    const BinSource in = xyzi_source(m->d_axyzi[b], rgba ? m->d_argba[b] : nullptr, 0);
-    const FoldSrc fs{in.xyzi ? (const char *)in.xyzi + 12 : nullptr, 16};
-    BinCounters *prev_ctr = m->pend.active ? m->pend.sc.ctr : nullptr;
-    if ((rc = enqueue_add<SRC_XYZI>(m, in, fs, n, fp, nullptr, nullptr, true, true, true))) return rc;
-    // the step's host-visible result: the counters of the newest call whose fold has been issued
-    GEM_CUDA(m, cudaMemcpyAsync(&m->h_ctr_ring[i & 1u], prev_ctr ? prev_ctr : m->ctr_last, sizeof(BinCounters), cudaMemcpyDeviceToHost, m->stream));
-    // staging set (i-1) % 3 was last read by the fold just issued (or by this call's own fold in the serial fallback)
-    GEM_CUDA(m, cudaEventRecord(m->ev_done[(i + 2u) % 3u], m->stream));
-    if (!m->pend.active) GEM_CUDA(m, cudaEventRecord(m->ev_done[b], m->stream));
-    memset(&m->stats, 0, sizeof m->stats);
-    m->stats.points_in = n; // the rest is fetched by gem_get_stats
-    return GEM_OK;
+    return async_add_slot(m, i, n, rgba != nullptr, frame);
 }
 
 int gem_add_cloud_pcl_host(gem_map *m, const void *pts, int n, const gem_frame *frame)
@@ -1415,13 +1435,8 @@ int gem_closeloop(gem_map *m, const float up[2], float height_update)
     return GEM_OK;
 }
 
-int gem_colourise_points(gem_map *m, void *xyzi, int n, const double Tc[12], const double Tl[16], const unsigned char *bgr,
-                         int width, int height, int row_stride, void *rgba_out)
+static ProjParams proj_params(const double Tc[12], const double Tl[16], int width, int height, int row_stride)
 {
-    if (!m || n < 0 || (n > 0 && (!xyzi || !rgba_out)) || !Tc || !Tl || !bgr || width < 1 || height < 1 || row_stride < 3 * width)
-        return fail(m, GEM_ERR_INVALID, "gem_colourise_points: bad argument");
-    Lock lk(m->mu);
-    SetDev sd(m->dev);
     ProjParams pp;
     for (int i = 0; i < 3; i++) // P_lidar2img = Tcamera * TLidar (ElevationMapping.cpp:347), double, left-to-right sums
         for (int j = 0; j < 4; j++) {
@@ -1430,6 +1445,17 @@ int gem_colourise_points(gem_map *m, void *xyzi, int n, const double Tc[12], con
             pp.P[4 * i + j] = a;
         }
     pp.width = width; pp.height = height; pp.row_stride = row_stride;
+    return pp;
+}
+
+int gem_colourise_points(gem_map *m, void *xyzi, int n, const double Tc[12], const double Tl[16], const unsigned char *bgr,
+                         int width, int height, int row_stride, void *rgba_out)
+{
+    if (!m || n < 0 || (n > 0 && (!xyzi || !rgba_out)) || !Tc || !Tl || !bgr || width < 1 || height < 1 || row_stride < 3 * width)
+        return fail(m, GEM_ERR_INVALID, "gem_colourise_points: bad argument");
+    Lock lk(m->mu);
+    SetDev sd(m->dev);
+    const ProjParams pp = proj_params(Tc, Tl, width, height, row_stride);
     if (n > 0)
         GEM_LAUNCH(m, GEM_PROF_OTHER, k_colourise<<<blocks_for((size_t)n, 256), 256, 0, m->stream>>>((float4 *)xyzi, n, pp, bgr, (uchar4 *)rgba_out));
     GEM_CUDA(m, cudaGetLastError());
@@ -2719,6 +2745,138 @@ int gem_tiled_step(gem_map *m, const void *xyzi, const void *rgba, int n, const 
     m->pend = b.fold;
     if (ts.depth != 2) { ts.routed.active = true; ts.routed.step = stepv; ts.routed.buf = bufv; }
     return GEM_OK;
+}
+
+// ---- raw sensor messages: PointCloud2 decode, cv_bridge's 8-bit conversions, the one-call frame (gem_ingest.cuh; f12) ----
+int gem_pointcloud2_mapping(const gem_pointcloud2 *layout, unsigned long long data_bytes, gem_pc2_mapping *out)
+{
+    const char *why = pc2_map(layout, data_bytes, out);
+    return why ? fail(nullptr, GEM_ERR_INVALID, std::string("gem_pointcloud2_mapping: ") + why) : GEM_OK;
+}
+
+static bool ranges_meet(const void *a, size_t na, const void *b, size_t nb)
+{
+    const uintptr_t a0 = (uintptr_t)a, b0 = (uintptr_t)b;
+    return na > 0 && nb > 0 && a0 < b0 + nb && b0 < a0 + na;
+}
+
+static int launch_decode(gem_map *m, const gem_pointcloud2 *layout, const gem_pc2_mapping &mp, const void *data, void *xyzi_out)
+{
+    if (mp.points == 0) return GEM_OK;
+    const Pc2Params p = pc2_params(layout, mp, data, mp.bytes); // the kernel reads no byte past the last point's
+    const int blocks = p.tiles < (unsigned long long)NUM_SMS * 16 ? (int)p.tiles : NUM_SMS * 16;
+    GEM_LAUNCH(m, GEM_PROF_OTHER, k_decode_pc2<<<blocks, PC2_BLOCK, pc2_smem_bytes(p), m->stream>>>(p, (uint4 *)xyzi_out));
+    GEM_CUDA(m, cudaGetLastError());
+    return GEM_OK;
+}
+
+int gem_decode_pointcloud2(gem_map *m, const gem_pointcloud2 *layout, const void *data, unsigned long long data_bytes, void *xyzi_out)
+{
+    if (!m) return GEM_ERR_INVALID;
+    gem_pc2_mapping mp;
+    const char *why = pc2_map(layout, data_bytes, &mp);
+    if (why) return fail(m, GEM_ERR_INVALID, std::string("gem_decode_pointcloud2: ") + why);
+    if (mp.points > 0 && ((mp.bytes > 0 && !data) || !xyzi_out || ((uintptr_t)xyzi_out & 15u)))
+        return fail(m, GEM_ERR_INVALID, "gem_decode_pointcloud2: NULL pointer, or the output is not 16-byte aligned");
+    if (mp.points > 0 && ranges_meet(data, mp.bytes, xyzi_out, (size_t)mp.points * 16))
+        return fail(m, GEM_ERR_INVALID, "gem_decode_pointcloud2: the message and output ranges overlap");
+    Lock lk(m->mu);
+    SetDev sd(m->dev);
+    return launch_decode(m, layout, mp, data, xyzi_out);
+}
+
+static int launch_image(gem_map *m, int enc, const void *src, int width, int height, long long step, void *dst, long long dst_step)
+{
+    GEM_LAUNCH(m, GEM_PROF_OTHER, k_image_to_bgr8<<<blocks_for((size_t)width * height, 256), 256, 0, m->stream>>>(
+                                      (const unsigned char *)src, width, height, step, enc, (unsigned char *)dst, dst_step));
+    GEM_CUDA(m, cudaGetLastError());
+    return GEM_OK;
+}
+
+// bytes of a width x height image with `channels` bytes per pixel and rows `step` bytes apart (the last row unpadded)
+static size_t image_bytes(int width, int height, long long step, int channels)
+{
+    return (size_t)(height - 1) * (size_t)step + (size_t)channels * width;
+}
+
+int gem_image_to_bgr8(gem_map *m, const char *encoding, const void *src, int width, int height, int step, void *dst, int dst_step)
+{
+    if (!m) return GEM_ERR_INVALID;
+    const int enc = image_encoding(encoding);
+    if (enc < 0) return fail(m, GEM_ERR_INVALID, "gem_image_to_bgr8: encoding is not bgr8, rgb8, bgra8, rgba8 or mono8");
+    const int ch = image_channels(enc);
+    if (!src || !dst || width < 1 || height < 1 || (long long)step < (long long)ch * width || (long long)dst_step < 3ll * width)
+        return fail(m, GEM_ERR_INVALID, "gem_image_to_bgr8: bad argument");
+    if (ranges_meet(src, image_bytes(width, height, step, ch), dst, image_bytes(width, height, dst_step, 3)))
+        return fail(m, GEM_ERR_INVALID, "gem_image_to_bgr8: the source and destination ranges overlap");
+    Lock lk(m->mu);
+    SetDev sd(m->dev);
+    return launch_image(m, enc, src, width, height, step, dst, dst_step);
+}
+
+int gem_add_pointcloud2_host_async(gem_map *m, const gem_pointcloud2 *layout, const void *data, unsigned long long data_bytes,
+                                   const gem_camera_image *img, const gem_frame *frame)
+{
+    if (!m || !frame || !sensor_ok(frame->sensor)) return fail(m, GEM_ERR_INVALID, "gem_add_pointcloud2_host_async: bad argument");
+    gem_pc2_mapping mp;
+    const char *why = pc2_map(layout, data_bytes, &mp);
+    if (why) return fail(m, GEM_ERR_INVALID, std::string("gem_add_pointcloud2_host_async: ") + why);
+    if (mp.bytes > 0 && !data) return fail(m, GEM_ERR_INVALID, "gem_add_pointcloud2_host_async: NULL data");
+    if (mp.points > m->P) return fail(m, GEM_ERR_INVALID, "gem_add_pointcloud2_host_async: width * height exceeds max_points");
+    int enc = -1;
+    size_t img_bytes = 0;
+    if (img) {
+        char e[sizeof img->encoding + 1];
+        memcpy(e, img->encoding, sizeof img->encoding);
+        e[sizeof img->encoding] = 0;
+        if ((enc = image_encoding(e)) < 0)
+            return fail(m, GEM_ERR_INVALID, "gem_add_pointcloud2_host_async: encoding is not bgr8, rgb8, bgra8, rgba8 or mono8");
+        if (!img->data || img->width < 1 || img->height < 1 || (long long)img->step < (long long)image_channels(enc) * img->width)
+            return fail(m, GEM_ERR_INVALID, "gem_add_pointcloud2_host_async: bad image");
+        img_bytes = image_bytes(img->width, img->height, img->step, image_channels(enc));
+    }
+    const int n = (int)mp.points;
+    Lock lk(m->mu);
+    SetDev sd(m->dev);
+    int rc = ensure_async_ring(m);
+    if (rc) return rc;
+    if (n == 0) return flush_all_pending(m);
+    const unsigned i = m->async_calls;
+    const int b = (int)(i % 3u);
+    // growth before anything is enqueued: both streams drained, so no queued copy or kernel uses a buffer that goes
+    const size_t bgr_bytes = img && enc != IMG_BGR8 ? (size_t)3 * img->width * img->height : 0;
+    if (m->pc2_raw[b].cap < mp.bytes || m->pc2_img[b].cap < img_bytes || m->pc2_bgr.cap < bgr_bytes) {
+        GEM_CUDA(m, cudaStreamSynchronize(m->copy_stream));
+        GEM_CUDA(m, cudaStreamSynchronize(m->stream));
+        if ((rc = scratch_grow(m, m->pc2_raw[b], mp.bytes, "gem_add_pointcloud2_host_async")) ||
+            (rc = scratch_grow(m, m->pc2_img[b], img_bytes, "gem_add_pointcloud2_host_async")) ||
+            (rc = scratch_grow(m, m->pc2_bgr, bgr_bytes, "gem_add_pointcloud2_host_async")))
+            return rc;
+    }
+    m->async_calls++;
+    // copy stream: the slot's last reader (call i-3) is done (see gem_add_points_host_async); pageable sources are staged
+    // by CUDA before cudaMemcpyAsync returns
+    GEM_CUDA(m, cudaStreamWaitEvent(m->copy_stream, m->ev_done[b], 0));
+    if (mp.bytes > 0) GEM_CUDA(m, cudaMemcpyAsync(m->pc2_raw[b].p, data, mp.bytes, cudaMemcpyHostToDevice, m->copy_stream));
+    if (img) GEM_CUDA(m, cudaMemcpyAsync(m->pc2_img[b].p, img->data, img_bytes, cudaMemcpyHostToDevice, m->copy_stream));
+    GEM_CUDA(m, cudaEventRecord(m->ev_h2d[b], m->copy_stream));
+    GEM_CUDA(m, cudaStreamWaitEvent(m->stream, m->ev_h2d[b], 0));
+    // decode into staging set b, then (with an image) BGR8 and the colourisation of ElevationMapping.cpp:331-381
+    if ((rc = launch_decode(m, layout, mp, m->pc2_raw[b].p, m->d_axyzi[b]))) return rc;
+    if (img) {
+        const void *bgr = m->pc2_img[b].p;
+        int stride = img->step;
+        if (enc != IMG_BGR8) {
+            if ((rc = launch_image(m, enc, m->pc2_img[b].p, img->width, img->height, img->step, m->pc2_bgr.p, 3ll * img->width))) return rc;
+            bgr = m->pc2_bgr.p;
+            stride = 3 * img->width;
+        }
+        const ProjParams pp = proj_params(img->T_camera, img->T_lidar, img->width, img->height, stride);
+        GEM_LAUNCH(m, GEM_PROF_OTHER, k_colourise<<<blocks_for((size_t)n, 256), 256, 0, m->stream>>>(
+                                          (float4 *)m->d_axyzi[b], n, pp, (const unsigned char *)bgr, (uchar4 *)m->d_argba[b]));
+        GEM_CUDA(m, cudaGetLastError());
+    }
+    return async_add_slot(m, i, n, img != nullptr, frame);
 }
 
 } // extern "C"

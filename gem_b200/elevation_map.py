@@ -145,6 +145,78 @@ def _is_device(a) -> bool:
 
 
 # ------------------------------------------------------------------------------------------
+# raw sensor messages (DESIGN.md f12)
+# ------------------------------------------------------------------------------------------
+_NP_POINTFIELD = {("i", 1): 1, ("u", 1): 2, ("i", 2): 3, ("u", 2): 4, ("i", 4): 5, ("u", 4): 6, ("f", 4): 7, ("f", 8): 8}
+
+
+class PointCloud2Layout:
+    """sensor_msgs/PointCloud2's layout as gem_pointcloud2: `c` is the C struct, `fields` the (name, offset, datatype, count)
+    list it was built from (kept alive with the C array)."""
+
+    def __init__(self, fields, width: int, height: int = 1, point_step: int | None = None, row_step: int | None = None,
+                 is_bigendian: int = 0):
+        if isinstance(fields, np.dtype):
+            dt = fields
+            point_step = dt.itemsize if point_step is None else point_step
+            fields = []
+            for name in dt.names:
+                ft, off = dt.fields[name][:2]
+                base, shape = (ft.subdtype if ft.subdtype else (ft, ()))
+                key = (base.kind, base.itemsize)
+                if key not in _NP_POINTFIELD:
+                    raise ValueError(f"PointCloud2Layout: field {name!r} has no PointField datatype ({base})")
+                fields.append((name, off, _NP_POINTFIELD[key], int(np.prod(shape)) if shape else 1))
+        self.fields = [(str(n), int(o), _lib.POINTFIELD_TYPES[d] if isinstance(d, str) else int(d), int(c))
+                       for n, o, d, c in fields]
+        if point_step is None:
+            raise ValueError("PointCloud2Layout: point_step is needed with a field list")
+        self._arr = (_lib.GemPointField * max(len(self.fields), 1))()
+        for k, (n, o, d, c) in enumerate(self.fields):
+            nb = n.encode()[:32]      # 32 bytes leave no NUL: such a name matches nothing, like any longer than 31 bytes
+            C.memmove(C.addressof(self._arr[k]) + _lib.GemPointField.name.offset, nb, len(nb))
+            self._arr[k].offset, self._arr[k].datatype, self._arr[k].count = o, d, c
+        self.width, self.height, self.point_step = int(width), int(height), int(point_step)
+        self.row_step = self.width * self.point_step if row_step is None else int(row_step)
+        self.c = _lib.GemPointCloud2(self.width, self.height, self.point_step, self.row_step, int(is_bigendian),
+                                     len(self.fields), C.cast(self._arr, C.POINTER(_lib.GemPointField)))
+
+    @property
+    def points(self) -> int:
+        return self.width * self.height
+
+
+def _host_bytes(a):
+    """(pointer, bytes) of host memory: a numpy array, bytes / bytearray, or a CPU torch tensor (pinned or not)"""
+    if isinstance(a, (bytes, bytearray, memoryview)):
+        a = np.frombuffer(a, np.uint8)
+    if isinstance(a, np.ndarray):
+        if not a.flags.c_contiguous:
+            raise ValueError("host buffer must be contiguous")
+        return C.c_void_p(a.ctypes.data), int(a.nbytes)
+    if hasattr(a, "data_ptr") and not _is_device(a):
+        return C.c_void_p(a.data_ptr()), int(a.numel() * a.element_size())
+    raise TypeError(f"not a host buffer: {type(a)}")
+
+
+class CameraImage:
+    """gem_camera_image: an 8-bit image in host memory (numpy array or CPU tensor, pinned or pageable) with the
+    camera-lidar calibration of gem_colourise_points; `c` is the C struct"""
+
+    def __init__(self, T_camera, T_lidar, encoding: str, data, width: int, height: int, step: int | None = None):
+        if encoding not in _lib.IMAGE_ENCODINGS:
+            raise ValueError(f"CameraImage: encoding {encoding!r} is not one of {list(_lib.IMAGE_ENCODINGS)}")
+        self.data = data
+        ptr, _ = _host_bytes(data)
+        step = _lib.IMAGE_ENCODINGS[encoding] * int(width) if step is None else int(step)
+        self.c = _lib.GemCameraImage()
+        self.c.T_camera[:] = [float(v) for v in np.asarray(T_camera, np.float64).reshape(-1)]
+        self.c.T_lidar[:] = [float(v) for v in np.asarray(T_lidar, np.float64).reshape(-1)]
+        self.c.encoding = encoding.encode()
+        self.c.width, self.c.height, self.c.step, self.c.data = int(width), int(height), step, ptr
+
+
+# ------------------------------------------------------------------------------------------
 class ElevationMap:
     """One robot-centric elevation grid resident on one H100.
 
@@ -657,6 +729,65 @@ class ElevationMap:
         check(self._lib.gem_voxel_grid(self._h, _ptr(xyzi) if n else None, n, C.byref(p), _ptr(out) if cap else None, cap,
                                        C.byref(info)), self._h, "gem_voxel_grid")
         return out[:min(info.count, cap)], {k: getattr(info, k) for k, _ in _lib.GemVoxelGridInfo._fields_}
+
+    # -- raw sensor messages: PointCloud2 and cv_bridge's 8-bit images (DESIGN.md f12) -------------------------------------
+    @staticmethod
+    def pointcloud2_mapping(layout: PointCloud2Layout, data_bytes: int | None = None) -> dict:
+        """createMapping<PointXYZRGBICT> of PCL 1.8 for `layout` (host code, no GPU): {spans: [(serialized_offset,
+        struct_offset, size), ...], fast_path, matched: [struct field names], points, bytes}.  data_bytes defaults to
+        the bytes the layout needs.  A refused layout raises GemError."""
+        lib = _lib.load()
+        mp = _lib.GemPc2Mapping()
+        nb = (1 << 64) - 1 if data_bytes is None else int(data_bytes)
+        rc = lib.gem_pointcloud2_mapping(C.byref(layout.c), nb, C.byref(mp))
+        if rc:
+            msg = lib.gem_last_error(None)
+            raise _lib.GemError(f"gem_pointcloud2_mapping: {_lib.ERR_NAMES.get(rc, rc)}: {msg.decode() if msg else ''}")
+        return {"spans": [(mp.spans[k].serialized_offset, mp.spans[k].struct_offset, mp.spans[k].size) for k in range(mp.nspans)],
+                "fast_path": bool(mp.fast_path), "matched": [n for k, n in enumerate(_lib.PC2_FIELDS) if mp.matched >> k & 1],
+                "points": int(mp.points), "bytes": int(mp.bytes)}
+
+    def decode_pointcloud2(self, layout: PointCloud2Layout, data, out=None, data_bytes: int | None = None):
+        """gem_decode_pointcloud2: the message bytes `data` (a CUDA tensor, any dtype and offset) into `out`, a contiguous
+        (width * height, 4) float32 CUDA tensor (new if None), {x, y, z, intensity} as fromPCLPointCloud2 gives them.
+        Asynchronous on the map's stream (the current torch stream is synchronised first): sync() before reading out."""
+        import torch
+        if not _is_device(data):
+            raise ValueError("decode_pointcloud2: data must be a CUDA tensor")
+        n = layout.points
+        if out is None:
+            out = torch.empty((n, 4), dtype=torch.float32, device=data.device)
+        nb = int(data.numel() * data.element_size()) if data_bytes is None else int(data_bytes)
+        torch.cuda.current_stream(data.device).synchronize()
+        check(self._lib.gem_decode_pointcloud2(self._h, C.byref(layout.c), _ptr(data), nb, _ptr(out)), self._h,
+              "gem_decode_pointcloud2")
+        return out
+
+    def image_to_bgr8(self, encoding: str, src, width: int, height: int, step: int | None = None, out=None,
+                      dst_step: int | None = None):
+        """gem_image_to_bgr8: cv_bridge::toCvCopy(image, "bgr8") for bgr8 / rgb8 / bgra8 / rgba8 / mono8 on CUDA uint8
+        tensors.  out defaults to a new (height, width, 3) tensor.  Asynchronous on the map's stream."""
+        import torch
+        ch = _lib.IMAGE_ENCODINGS.get(encoding, 3)
+        step = ch * int(width) if step is None else int(step)
+        if out is None:
+            out = torch.empty((int(height), int(width), 3), dtype=torch.uint8, device=src.device)
+        dst_step = 3 * int(width) if dst_step is None else int(dst_step)
+        torch.cuda.current_stream(src.device).synchronize()
+        check(self._lib.gem_image_to_bgr8(self._h, encoding.encode(), _ptr(src), int(width), int(height), step, _ptr(out),
+                                          dst_step), self._h, "gem_image_to_bgr8")
+        return out
+
+    def add_pointcloud2_host_async(self, layout: PointCloud2Layout, data, frame: GemFrame, image: CameraImage | None = None,
+                                   data_bytes: int | None = None):
+        """gem_add_pointcloud2_host_async: one sensor_msgs/PointCloud2 (host bytes: numpy, bytes or a CPU tensor, pinned
+        or pageable) and optionally its camera image, decoded, colourised and added pipelined.  Pinned buffers must stay
+        untouched until the call after next or sync(); pageable ones may be reused at once."""
+        ptr, nb = _host_bytes(data) if layout.points else (None, 0)
+        nb = nb if data_bytes is None else int(data_bytes)
+        check(self._lib.gem_add_pointcloud2_host_async(self._h, C.byref(layout.c), ptr, nb,
+                                                       C.byref(image.c) if image is not None else None, C.byref(frame)),
+              self._h, "gem_add_pointcloud2_host_async")
 
     # -- the MLS densification of the dense_mapping signal (DESIGN.md f10) ------------------------------------------------
     GEM_MLS = {"search_radius": 0.5, "sqr_gauss_param": 0.25, "polynomial_fit": True, "order": 5,

@@ -504,6 +504,89 @@ typedef struct gem_mls_info {
 int gem_mls_upsample(gem_map *m, const void *points32_device, int n, const gem_mls_params *p,
                      void *out_points32_device, long long capacity, gem_mls_info *info);
 
+/* ---- raw sensor messages: the first lines of ElevationMapping::Callback (ElevationMapping.cpp:311-317; DESIGN.md f12) ----
+ * gem_pointcloud2 mirrors sensor_msgs/PointCloud2 without a ROS dependency (fields points at nfields gem_pointfield,
+ * datatype = sensor_msgs/PointField's codes 1..8).  The node turns the message into pcl::PointCloud<PointXYZRGBICT>
+ * with pcl::fromPCLPointCloud2; these calls restate PCL 1.8's createMapping<PointXYZRGBICT> and fromPCLPointCloud2
+ * (the PCL of ROS Kinetic).  Unpinned: restated, PCL is not available.
+ *   M1 match: the struct fields x 0, y 4, z 8, rgb 16, intensity 24, covariance 20, travers 28 (bytes into the 32-byte
+ *      record), in this registration order, each take the FIRST message field in list order whose name is equal, whose
+ *      datatype is FLOAT32 and whose count is 1 or 0.  No rgb / rgba aliasing.  An unmatched struct field is left alone
+ *      (PCL only warns): matched bit k of gem_pc2_mapping says whether field k of that order was found.
+ *   M2 coalesce: the mappings sorted by message offset; one is merged into its predecessor when the two differences of
+ *      message and struct offsets are equal, the predecessor growing to the end of the later one, so a merged span also
+ *      copies the message bytes between the two fields into struct bytes no mapping of their own names.
+ *   M3 copy: with exactly one span left, at message and struct offset 0, and point_step == 32, each whole 32-byte
+ *      point is copied (the unmapped bytes too; PCL's memcpy fast path); otherwise every span of every point, in span
+ *      order (a later span overwrites what an earlier one wrote), from the point at row * row_step + col * point_step.
+ *      is_bigendian (and is_dense) are not read.
+ *   DEFINED: struct bytes nothing writes are 0 (the reference's constructor is empty: stale heap bytes).  So a cloud
+ *      without a FLOAT32 intensity (an Ouster's uint16 one) gets intensity 0, and the colour gate of gpu.cu:488 then
+ *      never passes: such a cloud writes no intensity or colour into the map.
+ *   DEFINED: GEM_ERR_INVALID, nothing written, where PCL reads out of bounds or wraps a size_t: a datatype outside 1..8,
+ *      width * height > INT_MAX, and with width * height > 0: row_step < width * point_step, data_bytes <
+ *      (height - 1) * row_step + width * point_step, a matched field ending past point_step, two matched fields
+ *      overlapping in the message.  Names longer than 31 bytes never match.
+ * gem_pointcloud2_mapping: host code, no handle, no GPU: validates the layout against data_bytes and fills *out.
+ * gem_decode_pointcloud2: width * height float4 {x, y, z, intensity} = struct bytes 0-11 and 24-27 of the records
+ *   M1-M3 define, row-major, into xyzi_out_device (16-byte aligned).  Bytes are copied, never computed on: NaN payloads
+ *   and -0 survive.  No point is removed (the sensor processors' cleanPointCloud and gem_voxel_grid cut non-finite
+ *   ones).  data_device may have any alignment; input and output may not overlap.  Asynchronous on the handle's stream.
+ * gem_image_to_bgr8: cv_bridge::toCvCopy(image, "bgr8") for the encodings where it is a byte permutation: "bgr8"
+ *   copied, "rgb8" channels swapped, "bgra8" / "rgba8" alpha dropped, "mono8" replicated into three channels.  Any other
+ *   encoding (cv_bridge scales or demosaics those) is GEM_ERR_INVALID.  step / dst_step: row strides in bytes (at least
+ *   channels * width / 3 * width); src and dst may not overlap.  Asynchronous on the handle's stream.
+ * gem_add_pointcloud2_host_async: Callback's lines 311-381 plus processpoints in one call: the message bytes (and the
+ *   image, when img != NULL) go to the device on the copy stream, are decoded into the staging set of
+ *   gem_add_points_host_async, colourised there by gem_colourise_points' kernel (img != NULL: intensities of points that
+ *   do not project are zeroed before the add reads them; img == NULL: no colour, like rgba NULL) and added pipelined.
+ *   It shares the three-slot ring of gem_add_points_host_async (staging sets, events, counters): the two calls may be
+ *   interleaved on one handle.  Its own message and image staging buffers grow on demand, after synchronising the
+ *   handle's streams and before anything is enqueued (a failed growth is GEM_ERR_NOMEM and changes nothing).  Host
+ *   buffers: pinned memory must stay untouched until the call after next (or gem_sync); pageable memory is accepted and
+ *   may be reused as soon as the call returns (CUDA stages it before the copy call returns), so a ROS message's data can
+ *   be passed as it is.  width * height > max_points is refused; width * height == 0 flushes. */
+enum { GEM_PF_INT8 = 1, GEM_PF_UINT8 = 2, GEM_PF_INT16 = 3, GEM_PF_UINT16 = 4, GEM_PF_INT32 = 5, GEM_PF_UINT32 = 6,
+       GEM_PF_FLOAT32 = 7, GEM_PF_FLOAT64 = 8 };
+enum { GEM_PC2_X = 0, GEM_PC2_Y = 1, GEM_PC2_Z = 2, GEM_PC2_RGB = 3, GEM_PC2_INTENSITY = 4, GEM_PC2_COVARIANCE = 5,
+       GEM_PC2_TRAVERS = 6, GEM_PC2_FIELDS = 7 };
+typedef struct gem_pointfield {
+    char name[32];
+    unsigned offset;
+    unsigned char datatype;       /* GEM_PF_*                                                 */
+    unsigned count;
+} gem_pointfield;
+typedef struct gem_pointcloud2 {
+    unsigned width, height, point_step, row_step;
+    unsigned char is_bigendian;   /* not read (as in PCL)                                     */
+    int nfields;
+    const gem_pointfield *fields; /* host memory                                              */
+} gem_pointcloud2;
+typedef struct gem_pc2_span {
+    unsigned serialized_offset, struct_offset, size;
+} gem_pc2_span;
+typedef struct gem_pc2_mapping {
+    int nspans;                   /* spans after M2, sorted by message offset                 */
+    gem_pc2_span spans[GEM_PC2_FIELDS];
+    int fast_path;                /* M3's whole-point copy                                    */
+    unsigned matched;             /* bit GEM_PC2_*: that struct field found a message field   */
+    long long points;             /* width * height                                           */
+    unsigned long long bytes;     /* message bytes the copy reads (from the first)            */
+} gem_pc2_mapping;
+typedef struct gem_camera_image {
+    double T_camera[12], T_lidar[16]; /* as gem_colourise_points                              */
+    char encoding[32];            /* sensor_msgs/Image encoding                               */
+    int width, height, step;
+    const void *data;             /* host memory, pinned or pageable                          */
+} gem_camera_image;
+int gem_pointcloud2_mapping(const gem_pointcloud2 *layout, unsigned long long data_bytes, gem_pc2_mapping *out);
+int gem_decode_pointcloud2(gem_map *m, const gem_pointcloud2 *layout, const void *data_device, unsigned long long data_bytes,
+                           void *xyzi_out_device);
+int gem_image_to_bgr8(gem_map *m, const char *encoding, const void *src_device, int width, int height, int step,
+                      void *dst_device, int dst_step);
+int gem_add_pointcloud2_host_async(gem_map *m, const gem_pointcloud2 *layout, const void *data_host, unsigned long long data_bytes,
+                                   const gem_camera_image *img, const gem_frame *frame);
+
 /* raw layer access (row-major L*L, float or int32 for the colour ids) for tests and
  * checkpoint/restore (the dead G_get_mapinfo/G_set_mapinfo of gpu.cu:457-475). */
 int gem_get_layer(gem_map *m, int layer, void *host_out);

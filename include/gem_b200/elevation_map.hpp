@@ -33,6 +33,47 @@ struct PointXYZRGBICT {
 };
 static_assert(sizeof(PointXYZRGBICT) == 32, "PCL record layout");
 
+// sensor_msgs/PointCloud2's layout without ROS (DESIGN.md f12): add the message's fields in order, then pass layout().
+// From a sensor_msgs::PointCloud2ConstPtr msg:
+//     gem_b200::PointCloud2Layout lay(msg->width, msg->height, msg->point_step, msg->row_step, msg->is_bigendian);
+//     for (const auto &f : msg->fields) lay.addField(f.name, f.offset, f.datatype, f.count);
+class PointCloud2Layout {
+public:
+    PointCloud2Layout(unsigned width, unsigned height, unsigned point_step, unsigned row_step, bool is_bigendian = false)
+    {
+        c_ = gem_pointcloud2{};
+        c_.width = width; c_.height = height; c_.point_step = point_step; c_.row_step = row_step;
+        c_.is_bigendian = is_bigendian ? 1 : 0;
+    }
+    // a name of 32 bytes or more is stored without its terminator and matches no struct field (none is that long)
+    void addField(const std::string &name, unsigned offset, unsigned char datatype, unsigned count)
+    {
+        gem_pointfield f{};
+        std::memcpy(f.name, name.data(), name.size() < sizeof f.name ? name.size() : sizeof f.name);
+        f.offset = offset; f.datatype = datatype; f.count = count;
+        fields_.push_back(f);
+    }
+    const gem_pointcloud2 *layout() const
+    {
+        c_.nfields = (int)fields_.size();
+        c_.fields = fields_.empty() ? nullptr : fields_.data();
+        return &c_;
+    }
+    // createMapping<PointXYZRGBICT>: the spans, the whole-point copy flag and the matched struct fields; throws on the
+    // layouts PCL would read out of bounds on (host code, no GPU)
+    gem_pc2_mapping mapping(unsigned long long data_bytes) const
+    {
+        gem_pc2_mapping m{};
+        if (gem_pointcloud2_mapping(layout(), data_bytes, &m) != GEM_OK)
+            throw std::runtime_error(std::string("gem_pointcloud2_mapping: ") + gem_last_error(nullptr));
+        return m;
+    }
+
+private:
+    std::vector<gem_pointfield> fields_;
+    mutable gem_pointcloud2 c_;
+};
+
 // sensor_processor/* parameters (config/sensor_processors/*.yaml)
 struct LaserSensorProcessor { // LaserSensorProcessor.cpp:38-47
     float min_radius = 0.018f, beam_angle = 0.0006f, beam_constant = 0.0015f;
@@ -353,6 +394,25 @@ class ElevationMap {
         gem_voxel_grid_info info{};
         check(gem_voxel_grid(h_, xyzi_device, (int)n, &p, out_device, (int)capacity, &info), "gem_voxel_grid");
         return info;
+    }
+    // raw sensor messages (DESIGN.md f12).  decodePointCloud2: fromPCLPointCloud2's x, y, z, intensity of every point into
+    // width * height float4 in device memory (asynchronous).  imageToBgr8: cv_bridge::toCvCopy(image, "bgr8") for bgr8,
+    // rgb8, bgra8, rgba8 and mono8 in device memory (asynchronous).  addPointCloud2HostAsync: the message bytes as they
+    // arrive (host memory, pinned or pageable) and optionally the camera image, decoded, colourised and added pipelined
+    // (Callback's first lines plus processpoints in one call).
+    void decodePointCloud2(const PointCloud2Layout &lay, const void *data_device, unsigned long long data_bytes, void *xyzi_out_device)
+    {
+        check(gem_decode_pointcloud2(h_, lay.layout(), data_device, data_bytes, xyzi_out_device), "gem_decode_pointcloud2");
+    }
+    void imageToBgr8(const std::string &encoding, const void *src_device, int width, int height, int step, void *dst_device,
+                     int dst_step)
+    {
+        check(gem_image_to_bgr8(h_, encoding.c_str(), src_device, width, height, step, dst_device, dst_step), "gem_image_to_bgr8");
+    }
+    void addPointCloud2HostAsync(const PointCloud2Layout &lay, const void *data_host, unsigned long long data_bytes,
+                                 const gem_camera_image *img, const gem_frame &frame)
+    {
+        check(gem_add_pointcloud2_host_async(h_, lay.layout(), data_host, data_bytes, img, &frame), "gem_add_pointcloud2_host_async");
     }
     // pointcloudinterpolation's MovingLeastSquares (GEM's dense_mapping signal, ElevationMapping.cpp:1072-1118; DESIGN.md
     // f10) over n PointXYZRGBICT records in device memory: min(count, capacity) new records go to out_device, which must
