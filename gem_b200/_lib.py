@@ -136,6 +136,8 @@ MLS_UPSAMPLING = {"none": 0, "random_uniform_density": 1}  # GEM_MLS_*
 # sensor_msgs/PointField datatypes (GEM_PF_*) and the PointXYZRGBICT fields in registration order (GEM_PC2_*)
 POINTFIELD_TYPES = {"int8": 1, "uint8": 2, "int16": 3, "uint16": 4, "int32": 5, "uint32": 6, "float32": 7, "float64": 8}
 PC2_FIELDS = ["x", "y", "z", "rgb", "intensity", "covariance", "travers"]
+PCD_BINARY, PCD_RGB_UINT32 = 1, 2   # GEM_PCD_*
+PCD_LINE_MAX, PCD_HEADER_MAX = 105, 512   # GEM_PCD_LINE_MAX, GEM_PCD_HEADER_MAX
 IMAGE_ENCODINGS = {"bgr8": 3, "rgb8": 3, "bgra8": 4, "rgba8": 4, "mono8": 1}   # the byte-permutation encodings: channels
 
 PROF_CLASSES = ["bin", "fold_long", "unused", "fold", "clear_floor", "features", "raytrace", "other", "route"]
@@ -216,6 +218,8 @@ SYMBOLS = {
     "gem_image_to_bgr8": (C.c_int, [_P, C.c_char_p, _P, C.c_int, C.c_int, C.c_int, _P, C.c_int]),
     "gem_add_pointcloud2_host_async": (C.c_int, [_P, C.POINTER(GemPointCloud2), _P, C.c_ulonglong, C.POINTER(GemCameraImage),
                                                  C.POINTER(GemFrame)]),
+    "gem_pcd_header": (C.c_int, [C.c_longlong, C.c_int, C.c_char_p, C.c_int, _IP]),
+    "gem_pcd_format": (C.c_int, [_P, _P, C.c_int, C.c_int, _P, C.c_longlong, C.POINTER(C.c_longlong)]),
 }
 
 _lib = None

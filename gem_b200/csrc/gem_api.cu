@@ -30,6 +30,7 @@
 #include "gem_ingest.cuh"
 #include "gem_mls.cuh"
 #include "gem_octree.cuh"
+#include "gem_pcd.cuh"
 #include "gem_route.cuh"
 #include "gem_submap.cuh"
 #include "gem_voxel.cuh"
@@ -77,6 +78,9 @@ struct VoxScratch { // gem_voxel_grid (gem_voxel.cuh): keys and input indices be
 struct MlsScratch { // gem_mls_upsample (gem_mls.cuh): cell keys and indices before / after the sort, the points in cell
                    // order, the distinct cells, neighbour and output counts, output offsets, the long lists and their keys
     OctBuf key[2], idx[2], spts, ukey, ucnt, uoff, nbr, ocnt, ooff, longs, lkeys, temp, acc;
+};
+struct PcdScratch { // gem_pcd_format (gem_pcd.cuh): per-tile byte counts, their inclusive scan, the scan's temporary
+    OctBuf bytes, ends, temp;
 };
 struct OctScratch { // gem_color_octree (gem_octree.cuh); every buffer is consistent with its own capacity at all times
     OctBuf code[2], idx[2], leaf, cnt, off, level, ghead, gid, val, groups, ctr, temp, key2[2], nkey[2], nrec[2], dense;
@@ -151,6 +155,7 @@ struct gem_map {
     CostMarksDev *cost_acc = nullptr; // costmap mark calls: counts and encoded touch bounds
     VoxScratch vox;                // gem_voxel_grid
     MlsScratch mls;                // gem_mls_upsample
+    PcdScratch pcd;                // gem_pcd_format
     unsigned long long *d_stamps = nullptr; // gem_debug_stamps
     int *d_raylist = nullptr;      // ray clean-up: cells that cast a ray + their count
     uint32_t *d_bitmap = nullptr;  // ray clean-up: validity bitmap of the lowest layer (own tile / map-wide)
@@ -862,7 +867,8 @@ int gem_destroy(gem_map *m)
                           &m->vox.cnt, &m->vox.off, &m->vox.temp, &m->vox.acc, &m->mls.key[0], &m->mls.key[1], &m->mls.idx[0],
                           &m->mls.idx[1], &m->mls.spts, &m->mls.ukey, &m->mls.ucnt, &m->mls.uoff, &m->mls.nbr, &m->mls.ocnt,
                           &m->mls.ooff, &m->mls.longs, &m->mls.lkeys, &m->mls.temp, &m->mls.acc, &m->pc2_raw[0],
-                          &m->pc2_raw[1], &m->pc2_raw[2], &m->pc2_img[0], &m->pc2_img[1], &m->pc2_img[2], &m->pc2_bgr})
+                          &m->pc2_raw[1], &m->pc2_raw[2], &m->pc2_img[0], &m->pc2_img[1], &m->pc2_img[2], &m->pc2_bgr,
+                          &m->pcd.bytes, &m->pcd.ends, &m->pcd.temp})
             if (b->p) cudaFree(b->p);
         if (m->h_ctr) cudaFreeHost(m->h_ctr);
         if (m->h_ctr_ring) cudaFreeHost(m->h_ctr_ring);
@@ -2877,6 +2883,67 @@ int gem_add_pointcloud2_host_async(gem_map *m, const gem_pointcloud2 *layout, co
         GEM_CUDA(m, cudaGetLastError());
     }
     return async_add_slot(m, i, n, img != nullptr, frame);
+}
+
+// ---- point clouds as PCD files: PCL's generateHeader / writeASCII / writeBinary (gem_pcd.cuh; f13) ----------------------
+int gem_pcd_header(long long n, int flags, char *out, int capacity, int *len_out)
+{
+    if (len_out) *len_out = 0;
+    if (!len_out || capacity < 0 || (capacity > 0 && !out)) return fail(nullptr, GEM_ERR_INVALID, "gem_pcd_header: bad argument");
+    if (n < 0 || (flags & ~(GEM_PCD_BINARY | GEM_PCD_RGB_UINT32))) return fail(nullptr, GEM_ERR_INVALID, "gem_pcd_header: n < 0 or unknown flags");
+    if (n == 0) return fail(nullptr, GEM_ERR_INVALID, "gem_pcd_header: the cloud is empty (PCL writes no file)");
+    char h[GEM_PCD_HEADER_MAX];
+    const int len = pcd_header(n, flags, h);
+    *len_out = len;
+    if (capacity > len) memcpy(out, h, (size_t)len + 1);
+    return GEM_OK;
+}
+
+int gem_pcd_format(gem_map *m, const void *points32_device, int n, int flags, void *out_device, long long capacity, long long *bytes_out)
+{
+    if (bytes_out) *bytes_out = 0;
+    if (!m) return GEM_ERR_INVALID;
+    if (!bytes_out || capacity < 0 || (capacity > 0 && !out_device)) return fail(m, GEM_ERR_INVALID, "gem_pcd_format: bad argument");
+    if (n < 0 || (flags & ~(GEM_PCD_BINARY | GEM_PCD_RGB_UINT32))) return fail(m, GEM_ERR_INVALID, "gem_pcd_format: n < 0 or unknown flags");
+    if (n == 0) return fail(m, GEM_ERR_INVALID, "gem_pcd_format: the cloud is empty (PCL writes no file)");
+    if (!points32_device || ((uintptr_t)points32_device & 15u))
+        return fail(m, GEM_ERR_INVALID, "gem_pcd_format: the records are NULL or not 16-byte aligned");
+    const float4 *rec = static_cast<const float4 *>(points32_device);
+    unsigned char *out = static_cast<unsigned char *>(out_device);
+    const size_t N = (size_t)n, tiles = (N + PCD_BLOCK - 1) / PCD_BLOCK;
+    Lock lk(m->mu);
+    SetDev sd(m->dev);
+    cudaStream_t st = m->stream;
+    long long bytes = (long long)N * PCD_BINARY_RECORD;
+    if (!(flags & GEM_PCD_BINARY)) {
+        PcdScratch &S = m->pcd;
+        const char *what = "gem_pcd_format";
+        size_t t_scan = 0;
+        GEM_CUDA(m, cub::DeviceScan::InclusiveSum(nullptr, t_scan, (long long *)nullptr, (long long *)nullptr, (int)tiles, st));
+        int rc;
+        if ((rc = scratch_grow(m, S.bytes, tiles * 8, what)) || (rc = scratch_grow(m, S.ends, tiles * 8, what)) ||
+            (rc = scratch_grow(m, S.temp, t_scan, what)))
+            return rc;
+        long long *tb = S.bytes.as<long long>(), *te = S.ends.as<long long>();
+        size_t tcap = S.temp.cap;
+        GEM_LAUNCH(m, GEM_PROF_OTHER, k_pcd_len<<<(unsigned)tiles, PCD_BLOCK, 0, st>>>(rec, n, flags & GEM_PCD_RGB_UINT32, tb));
+        GEM_CUDA(m, cudaGetLastError());
+        GEM_CUDA(m, cub::DeviceScan::InclusiveSum(S.temp.p, tcap, tb, te, (int)tiles, st));
+        GEM_CUDA(m, cudaMemcpyAsync(&bytes, te + (tiles - 1), sizeof bytes, cudaMemcpyDeviceToHost, st));
+        GEM_CUDA(m, cudaStreamSynchronize(st));
+    }
+    *bytes_out = bytes;
+    if (capacity < bytes) return GEM_OK; // a size query, or too small: nothing is written
+    if (ranges_meet(points32_device, N * 32, out_device, (size_t)bytes))
+        return fail(m, GEM_ERR_INVALID, "gem_pcd_format: the records and the output overlap");
+    if (flags & GEM_PCD_BINARY)
+        GEM_LAUNCH(m, GEM_PROF_OTHER, k_pcd_binary<<<(unsigned)tiles, PCD_BLOCK, 0, st>>>(rec, n, out));
+    else
+        GEM_LAUNCH(m, GEM_PROF_OTHER, k_pcd_ascii<<<(unsigned)tiles, PCD_BLOCK, 0, st>>>(rec, n, flags & GEM_PCD_RGB_UINT32,
+                                                                                     m->pcd.ends.as<long long>(), out));
+    GEM_CUDA(m, cudaGetLastError());
+    GEM_CUDA(m, cudaStreamSynchronize(st));
+    return GEM_OK;
 }
 
 } // extern "C"

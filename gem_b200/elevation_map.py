@@ -11,6 +11,7 @@ This is test/bench plumbing over libgem_b200.so; all arithmetic happens in the C
 from __future__ import annotations
 
 import ctypes as C
+import os
 from dataclasses import dataclass, field
 
 import numpy as np
@@ -878,6 +879,108 @@ class ElevationMap:
         self.local_map_take(out=rec[:nl])
         self.export_grid_cloud("shown", out=rec[nl:])
         return rec
+
+    # -- point clouds as PCD files: savingMap / savingSubMap's pcl::io::savePCDFile (DESIGN.md f13) -----------------------
+    PCD_CHUNK = 1 << 20   # records per save_pcd round trip: 32 MiB in, at most 105 MiB of text out
+
+    @staticmethod
+    def _pcd_flags(binary: bool, rgb_uint32: bool) -> int:
+        return (_lib.PCD_BINARY if binary else 0) | (_lib.PCD_RGB_UINT32 if rgb_uint32 else 0)
+
+    @staticmethod
+    def pcd_header(n: int, binary: bool = False, rgb_uint32: bool = False) -> bytes:
+        """the PCD header PCL's generateHeader writes for a PointXYZRGBICT cloud of n records (host code, no GPU); an empty
+        cloud raises GemError, as PCL throws"""
+        lib = _lib.load()
+        buf = C.create_string_buffer(_lib.PCD_HEADER_MAX)
+        k = C.c_int()
+        rc = lib.gem_pcd_header(int(n), ElevationMap._pcd_flags(binary, rgb_uint32), buf, _lib.PCD_HEADER_MAX, C.byref(k))
+        if rc:
+            msg = lib.gem_last_error(None)
+            raise _lib.GemError(f"gem_pcd_header: {_lib.ERR_NAMES.get(rc, rc)}: {msg.decode() if msg else ''}")
+        return buf.raw[:k.value]
+
+    def _pcd_points(self, points, what: str):
+        import torch
+        if not (_is_device(points) and points.dtype == torch.float32 and points.dim() == 2 and points.shape[1] == 8
+                and points.is_contiguous()):
+            raise ValueError(f"{what}: points must be a contiguous (n, 8) float32 CUDA tensor")
+        if points.device.index != self._device_index():
+            raise ValueError(f"{what}: the points are on {points.device}, the map on cuda:{self._device_index()}")
+
+    def format_pcd(self, points, binary: bool = False, rgb_uint32: bool = False, out=None):
+        """gem_pcd_format: the data section savePCDFile writes for `points`, a contiguous (n, 8) float32 CUDA tensor of
+        PointXYZRGBICT records -- ASCII lines of %.8g values, or 28-byte binary records.  Returns a uint8 CUDA tensor of
+        the bytes (a view of `out`, a uint8 CUDA tensor, when given: it must hold them all)"""
+        import torch
+        self._pcd_points(points, "format_pcd")
+        flags, n = self._pcd_flags(binary, rgb_uint32), int(points.shape[0])
+        torch.cuda.current_stream(points.device).synchronize()   # the library reads the points on its own stream
+        nb = C.c_longlong()
+        if out is None:
+            check(self._lib.gem_pcd_format(self._h, _ptr(points), n, flags, None, 0, C.byref(nb)), self._h, "gem_pcd_format")
+            out = torch.empty(nb.value, dtype=torch.uint8, device=points.device)
+        elif not (_is_device(out) and out.dtype == torch.uint8 and out.is_contiguous()):
+            raise ValueError("format_pcd: out must be a contiguous uint8 CUDA tensor")
+        check(self._lib.gem_pcd_format(self._h, _ptr(points), n, flags, _ptr(out), out.numel(), C.byref(nb)), self._h,
+              "gem_pcd_format")
+        if nb.value > out.numel():
+            raise ValueError(f"format_pcd: out holds {out.numel()} bytes, {nb.value} are needed")
+        return out.view(-1)[:nb.value]
+
+    def save_pcd(self, path, points, binary: bool = False, rgb_uint32: bool = False, chunk: int | None = None) -> int:
+        """pcl::io::savePCDFile(path, cloud) (ASCII) or savePCDFileBinary for `points`, (n, 8) float32 PointXYZRGBICT
+        records: a CUDA tensor, or a host array / CPU tensor (e.g. visualCloud_ gathered from harvest_*(records=True)).
+        The header goes first, then the records in chunks of `chunk` (default PCD_CHUNK) through fixed device and pinned
+        buffers, so a host cloud larger than free device memory still saves.  The file equals the one-shot
+        pcd_header(n) + format_pcd(points).  An empty cloud raises GemError and writes no file.  Returns the file's size"""
+        import torch
+        dev = torch.device("cuda", self._device_index())
+        if _is_device(points):
+            self._pcd_points(points, "save_pcd")
+            src = points
+        else:
+            src = torch.as_tensor(np.ascontiguousarray(points, np.float32) if isinstance(points, np.ndarray) else points)
+            if not (src.dtype == torch.float32 and src.dim() == 2 and src.shape[1] == 8):
+                raise ValueError("save_pcd: points must be (n, 8) float32 records")
+            src = src.contiguous()
+        n, flags = int(src.shape[0]), self._pcd_flags(binary, rgb_uint32)
+        head = self.pcd_header(n, binary, rgb_uint32)           # refuses an empty cloud before the file is opened
+        step = max(1, min(int(chunk or self.PCD_CHUNK), n))
+        per = 28 if binary else _lib.PCD_LINE_MAX
+        dout = torch.empty(step * per, dtype=torch.uint8, device=dev)
+        hout = torch.empty(step * per, dtype=torch.uint8, pin_memory=True)
+        din = hin = None
+        if not _is_device(src):
+            din = torch.empty((step, 8), dtype=torch.float32, device=dev)
+            hin = torch.empty((step, 8), dtype=torch.float32, pin_memory=True)
+        torch.cuda.current_stream(dev).synchronize()
+        size = len(head)
+        nb = C.c_longlong()
+        try:
+            with open(path, "wb") as f:
+                f.write(head)
+                for i in range(0, n, step):
+                    k = min(step, n - i)
+                    if din is None:
+                        part = src[i:i + k]
+                    else:
+                        hin[:k].copy_(src[i:i + k])
+                        part = din[:k]
+                        part.copy_(hin[:k], non_blocking=True)
+                        torch.cuda.current_stream(dev).synchronize()
+                    check(self._lib.gem_pcd_format(self._h, _ptr(part), k, flags, _ptr(dout), dout.numel(), C.byref(nb)),
+                          self._h, "gem_pcd_format")
+                    hout[:nb.value].copy_(dout[:nb.value])
+                    f.write(memoryview(hout.numpy())[:nb.value])
+                    size += nb.value
+        except BaseException:
+            try:
+                os.remove(path)
+            except OSError:
+                pass
+            raise
+        return size
 
     def get_layer_device(self, name: str, out):
         """dense (rows, cols) copy of a layer into a device tensor (float32, int32 for colours)"""

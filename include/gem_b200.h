@@ -587,6 +587,33 @@ int gem_image_to_bgr8(gem_map *m, const char *encoding, const void *src_device, 
 int gem_add_pointcloud2_host_async(gem_map *m, const gem_pointcloud2 *layout, const void *data_host, unsigned long long data_bytes,
                                    const gem_camera_image *img, const gem_frame *frame);
 
+/* ---- saving point clouds as PCD files (savingMap / savingSubMap / pointcloudinterpolation's pcl::io::savePCDFile,
+ * ElevationMapping.cpp:430-476, :1117; DESIGN.md f13) ----
+ * PCL's PCDWriter::generateHeader / writeASCII (savePCDFile's default) / writeBinary for pcl::PointCloud<PointXYZRGBICT>
+ * with width n, height 1 (what push_back and operator+ leave), restated; PCL itself is an unpinned dependency.
+ * gem_pcd_header: host code, no handle or GPU.  The header, 11 lines: "# .PCD v0.7 - Point Cloud Data file format",
+ *   "VERSION 0.7", "FIELDS x y z rgb intensity covariance travers" (registration order, PointXYZRGBICT.hpp:50-58),
+ *   "SIZE 4 4 4 4 4 4 4", "TYPE F F F F F F F", "COUNT 1 1 1 1 1 1 1", "WIDTH n", "HEIGHT 1", "VIEWPOINT 0 0 0 1 0 0 0",
+ *   "POINTS n", "DATA ascii" or "DATA binary", each ending in '\n'.  *len_out = its length (0 on an error); the bytes and
+ *   a terminating NUL are written only when capacity > length (capacity 0 is a size query).
+ * gem_pcd_format: the data section of n 32-byte PointXYZRGBICT records in device memory (16-byte aligned) into
+ *   out_device (any alignment, must not overlap the records):
+ *     ASCII: one line per record, x y z rgb intensity covariance travers separated by one space, '\n' after; a value is
+ *       "nan" for any NaN, else exactly glibc's printf("%.8g") of it ("-0", "inf", "-inf" included); with
+ *       GEM_PCD_RGB_UINT32 rgb is the unsigned decimal of its 32 bits (newer PCL; which release switched is not pinned).
+ *       A line is at most GEM_PCD_LINE_MAX bytes, so n * GEM_PCD_LINE_MAX bytes always suffice.
+ *     GEM_PCD_BINARY: 28 bytes per record, the same seven fields' bytes as they are in memory.
+ *   The record's w word (bytes 12-15) is never written.  *bytes_out is always set (0 on an error); all bytes are written
+ *   when they fit in capacity, none otherwise (out_device NULL with capacity 0 is a size query).  Host-synchronous.
+ * DEFINED where PCL throws (IOException, no file): an empty cloud (n == 0) is GEM_ERR_INVALID for both calls, and nothing
+ * is written.  n < 0, unknown flags and a record pointer that is NULL or not 16-byte aligned are GEM_ERR_INVALID. */
+enum { GEM_PCD_BINARY = 1, GEM_PCD_RGB_UINT32 = 2 };
+#define GEM_PCD_LINE_MAX 105    /* 7 values of at most 14 characters ("-1.2345678e-38"), 6 spaces, '\n' */
+#define GEM_PCD_HEADER_MAX 512  /* more than the longest header (n with 19 digits), NUL included */
+int gem_pcd_header(long long n, int flags, char *out, int capacity, int *len_out);
+int gem_pcd_format(gem_map *m, const void *points32_device, int n, int flags, void *out_device, long long capacity,
+                   long long *bytes_out);
+
 /* raw layer access (row-major L*L, float or int32 for the colour ids) for tests and
  * checkpoint/restore (the dead G_get_mapinfo/G_set_mapinfo of gpu.cu:457-475). */
 int gem_get_layer(gem_map *m, int layer, void *host_out);

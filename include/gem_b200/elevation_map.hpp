@@ -12,9 +12,11 @@
 // (the reference prints to stderr and continues, gpu_process.cu:987-992).
 #pragma once
 
+#include <algorithm>
 #include <cmath>
 #include <cstdint>
 #include <cstddef>
+#include <cstdio>
 #include <cstring>
 #include <limits>
 #include <stdexcept>
@@ -479,6 +481,59 @@ class ElevationMap {
         gridCloud(GEM_GRID_SHOWN, base + ((size_t)nl + (size_t)info.count) * sizeof(PointXYZRGBICT), (size_t)ng);
         return total;
     }
+    // Point clouds as PCD files (savingMap / savingSubMap's pcl::io::savePCDFile, ElevationMapping.cpp:430-476; DESIGN.md
+    // f13).  pcdHeader: PCL's header for n records (host only).  formatPcd: the data section of n records in device memory
+    // into out_device when all of it fits in capacity (nothing otherwise; capacity 0 is a size query); returns its bytes.
+    // savePcd: header and data to `path`, the records in device memory (onDevice) or host memory, streamed through pinned
+    // buffers in chunks of `chunk` records (the device reads and writes them directly), so the file is the same whatever
+    // the chunk.  An empty cloud throws, as PCL does, and writes no file.
+    static std::string pcdHeader(long long n, bool binary = false, bool rgbUint32 = false)
+    {
+        char h[GEM_PCD_HEADER_MAX];
+        int len = 0;
+        if (gem_pcd_header(n, pcdFlags(binary, rgbUint32), h, (int)sizeof h, &len) != GEM_OK)
+            throw std::runtime_error(std::string("gem_pcd_header: ") + gem_last_error(nullptr));
+        return std::string(h, (size_t)len);
+    }
+    long long formatPcd(const void *points32_device, size_t n, bool binary, bool rgbUint32, void *out_device, size_t capacity)
+    {
+        if (n > (size_t)std::numeric_limits<int>::max()) throw std::runtime_error("formatPcd: more than INT_MAX records");
+        long long bytes = 0;
+        check(gem_pcd_format(h_, points32_device, (int)n, pcdFlags(binary, rgbUint32), out_device, (long long)capacity, &bytes),
+              "gem_pcd_format");
+        return bytes;
+    }
+    void savePcd(const std::string &path, const void *records, size_t n, bool onDevice, bool binary = false, bool rgbUint32 = false,
+                 size_t chunk = (size_t)1 << 20)
+    {
+        const std::string head = pcdHeader((long long)n, binary, rgbUint32);
+        const size_t step = std::max<size_t>(1, std::min(chunk, n)), per = binary ? 28 : GEM_PCD_LINE_MAX;
+        void *in = nullptr, *out = nullptr;
+        if ((!onDevice && gem_host_alloc(&in, step * sizeof(PointXYZRGBICT)) != GEM_OK) || gem_host_alloc(&out, step * per) != GEM_OK) {
+            if (in) gem_host_free(in);
+            throw std::runtime_error("savePcd: gem_host_alloc failed");
+        }
+        FILE *f = std::fopen(path.c_str(), "wb");
+        bool ok = f && std::fwrite(head.data(), 1, head.size(), f) == head.size();
+        try {
+            for (size_t i = 0; ok && i < n; i += step) {
+                const size_t k = std::min(step, n - i);
+                const char *src = static_cast<const char *>(records) + i * sizeof(PointXYZRGBICT);
+                if (!onDevice) std::memcpy(in, src, k * sizeof(PointXYZRGBICT));
+                const long long bytes = formatPcd(onDevice ? src : in, k, binary, rgbUint32, out, step * per);
+                ok = std::fwrite(out, 1, (size_t)bytes, f) == (size_t)bytes;
+            }
+        } catch (...) {
+            ok = false;
+        }
+        if (f && std::fclose(f) != 0) ok = false;
+        if (in) gem_host_free(in);
+        gem_host_free(out);
+        if (!ok) {
+            if (f) std::remove(path.c_str());
+            throw std::runtime_error("savePcd: writing " + path + " failed");
+        }
+    }
     // Loop closure (ElevationMapping::updateGlobalMap, ElevationMapping.cpp:773-905), on device-resident submaps of
     // PointXYZRGBICT records: re-pose a submap (:805), and one pass of the pairwise fuse loop (:847-883) -- both clouds
     // come back reduced to one point per cell and compacted, *n_new / *n_old updated.  compat_precedence = true evaluates
@@ -508,6 +563,7 @@ class ElevationMap {
     void sync() { check(gem_sync(h_), "gem_sync"); }
 
   private:
+    static int pcdFlags(bool binary, bool rgbUint32) { return (binary ? GEM_PCD_BINARY : 0) | (rgbUint32 ? GEM_PCD_RGB_UINT32 : 0); }
     void check(int rc, const char *what)
     {
         if (rc != GEM_OK) throw std::runtime_error(std::string(what) + ": " + gem_last_error(h_));
