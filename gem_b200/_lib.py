@@ -87,6 +87,11 @@ class GemCostmapMarks(C.Structure):
                 ("max_x", C.c_double), ("max_y", C.c_double)]
 
 
+class GemCostmapInflation(C.Structure):
+    _fields_ = [("inflation_radius", C.c_double), ("cost_scaling_factor", C.c_double), ("inscribed_radius", C.c_double),
+                ("inflate_unknown", C.c_int)]
+
+
 class GemVoxelGridParams(C.Structure):
     _fields_ = [("leaf_size", C.c_float * 3), ("field", C.c_int), ("limit_min", C.c_double), ("limit_max", C.c_double),
                 ("limit_negative", C.c_int)]
@@ -130,6 +135,7 @@ class GemCameraImage(C.Structure):
 
 
 COST_FREE, COST_LETHAL, COST_UNKNOWN = 0, 254, 255           # GEM_COST_*
+INFLATE_MAX_CELLS = 4094                                     # GEM_INFLATE_MAX_CELLS
 COSTMAP_MODES = {"max": 0, "overwrite": 1}                  # GEM_COSTMAP_MAX / GEM_COSTMAP_OVERWRITE
 VOXEL_FIELDS = {None: -1, "x": 0, "y": 1, "z": 2, "intensity": 3}  # GEM_VOXEL_FIELD_*
 MLS_UPSAMPLING = {"none": 0, "random_uniform_density": 1}  # GEM_MLS_*
@@ -204,6 +210,8 @@ SYMBOLS = {
                                           C.POINTER(GemCostmapMarks)]),
     "gem_costmap_update_origin": (C.c_int, [_P, C.POINTER(GemCostmapWindow), C.c_double, C.c_double, C.c_ubyte, _P]),
     "gem_costmap_combine": (C.c_int, [_P, C.c_int, _P, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int]),
+    "gem_costmap_inflate": (C.c_int, [_P, C.POINTER(GemCostmapWindow), C.POINTER(GemCostmapInflation), _P, C.c_int, C.c_int,
+                                      C.c_int, C.c_int]),
     "gem_voxel_grid": (C.c_int, [_P, _P, C.c_int, C.POINTER(GemVoxelGridParams), _P, C.c_int, C.POINTER(GemVoxelGridInfo)]),
     "gem_mls_upsample": (C.c_int, [_P, _P, C.c_int, C.POINTER(GemMlsParams), _P, C.c_longlong, C.POINTER(GemMlsInfo)]),
     "gem_get_layer_device": (C.c_int, [_P, C.c_int, _P]),

@@ -5,10 +5,51 @@ into the master with updateWithMax) and the global one (PointMapLayer, 200 m x 2
 master).  Both roll with the robot.  `Costmap` owns one window and its grid; `update` does, on the host, what
 LayeredCostmap::updateMap does around the layer, so that a caller does not have to reproduce the grid-aligned origin
 drift of the rolling window or the bounds-to-rect arithmetic.  The cell work is the library's
-(gem_costmap_* of include/gem_b200.h)."""
+(gem_costmap_* of include/gem_b200.h).
+
+GEM's global costmap also lists costmap_2d's InflationLayer after the point layer; `InflationLayer` holds its parameters
+and bounds state, and `Costmap.update(..., inflation=layer)` runs it as LayeredCostmap::updateMap does with the two
+plugins (DESIGN.md f14)."""
 from __future__ import annotations
 
+import math
+
 from ._lib import COST_FREE, COST_LETHAL, COST_UNKNOWN  # noqa: F401
+
+FLT_MAX = 3.4028234663852886e38   # std::numeric_limits<float>::max(), as a double
+
+# GEM's robot footprint (move_base's costmap_common_params); its inscribed radius is 0.40 m
+GEM_FOOTPRINT = ((-0.64, -0.40), (-0.64, 0.40), (0.64, 0.40), (0.64, -0.40))
+
+
+def _distance_to_line(px, py, x0, y0, x1, y1):
+    """costmap_math's distanceToLine: the distance to the segment, its projection parameter clamped to [0, 1]"""
+    a, b, c, d = px - x0, py - y0, x1 - x0, y1 - y0
+    dot = a * c + b * d
+    len_sq = c * c + d * d
+    param = dot / len_sq if len_sq != 0 else math.copysign(math.inf, dot) if dot != 0 else math.nan
+    if param < 0:
+        xx, yy = x0, y0
+    elif param > 1:
+        xx, yy = x1, y1
+    else:
+        xx, yy = x0 + param * c, y0 + param * d
+    return math.hypot(px - xx, py - yy)
+
+
+def inscribed_radius(footprint, padding: float = 0.0) -> float:
+    """calculateMinAndMaxDistances' minimum (footprint.cpp) over the footprint padded as padFootprint does (each
+    coordinate moved away from 0 by `padding`): the least distance from the origin to a vertex or an edge.  A footprint
+    of two points or fewer gives DBL_MAX, as the reference's initial value."""
+    sign0 = lambda v: -1.0 if v < 0 else (1.0 if v > 0 else 0.0)   # noqa: E731
+    pts = [(float(x) + sign0(float(x)) * padding, float(y) + sign0(float(y)) * padding) for x, y in footprint]
+    best = 1.7976931348623157e308
+    if len(pts) <= 2:
+        return best
+    for k in range(len(pts)):
+        (x0, y0), (x1, y1) = pts[k], pts[(k + 1) % len(pts)]
+        best = min(best, min(math.hypot(x0, y0), _distance_to_line(0.0, 0.0, x0, y0, x1, y1)))
+    return best
 
 
 def world_to_map_enforce_bounds(window, wx: float, wy: float):
@@ -74,16 +115,22 @@ class Costmap:
         """PointMapLayer::updateBounds into this grid"""
         return self.emap.costmap_mark_points(points, self.window, self.grid, travers_thresh)
 
-    def update(self, layer: "Costmap", robot_xy, mode: str, mark):
+    def update(self, layer: "Costmap", robot_xy, mode: str, mark, inflation: "InflationLayer | None" = None):
         """LayeredCostmap::updateMap of this master grid with one layer: roll the master and the layer, let the layer
         mark (`mark(layer)` returns its marks, e.g. lambda l: l.mark_map(0.7)), turn the touch bounds into the rect,
         reset the rect to the master's fill and combine the layer into it ("max" for ElevationMapLayer, "overwrite" for
-        PointMapLayer).  Returns (rect or None, marks)."""
+        PointMapLayer).  With `inflation`, that InflationLayer is the second plugin: its update_bounds follows the
+        layer's, and its update_costs follows the combine.  Returns (rect or None, marks)."""
         import torch
         self.roll(robot_xy)
         layer.roll(robot_xy)
         marks = mark(layer)
-        rect = update_rect(self.window, marks)
+        if inflation is None:
+            rect = update_rect(self.window, marks)
+        else:
+            b = inflation.update_bounds((min(1e30, marks["min_x"]), min(1e30, marks["min_y"]),
+                                         max(-1e30, marks["max_x"]), max(-1e30, marks["max_y"])))
+            rect = update_rect(self.window, dict(zip(("min_x", "min_y", "max_x", "max_y"), b)))
         if rect is None:
             return None, marks
         x0, y0, xn, yn = rect
@@ -91,4 +138,42 @@ class Costmap:
             self.grid[y0:yn, x0:xn].fill_(self.fill)
         _, _, _, sx, sy = self.window
         self.emap.costmap_combine(mode, layer.grid, self.grid, sx, sy, rect)
+        if inflation is not None:
+            inflation.update_costs(self, rect)
         return rect, marks
+
+
+class InflationLayer:
+    """costmap_2d's InflationLayer (navigation 1.14): its parameters, need_reinflation and the last bounds.  Defaults are
+    costmap_2d's (0.55 m, factor 10); inscribed_radius is inscribed_radius(footprint) of the robot's footprint."""
+
+    def __init__(self, inflation_radius: float = 0.55, cost_scaling_factor: float = 10.0, inscribed_radius: float = 0.0,
+                 inflate_unknown: bool = False):
+        self.params = {}
+        self.need_reinflation = True
+        self.last = None
+        self.set_parameters(inflation_radius, cost_scaling_factor, inscribed_radius, inflate_unknown)
+
+    def set_parameters(self, inflation_radius: float, cost_scaling_factor: float, inscribed_radius: float,
+                       inflate_unknown: bool = False):
+        """a changed value makes the next update re-inflate the whole grid"""
+        p = {"inflation_radius": float(inflation_radius), "cost_scaling_factor": float(cost_scaling_factor),
+             "inscribed_radius": float(inscribed_radius), "inflate_unknown": bool(inflate_unknown)}
+        if p != self.params:
+            self.need_reinflation = True
+        self.params = p
+
+    def update_bounds(self, bounds):
+        """InflationLayer::updateBounds on (min_x, min_y, max_x, max_y): after a (re)configuration the bounds become the
+        float range, the whole grid; otherwise they are widened by the radius over the union with the last ones"""
+        last, self.last = self.last, tuple(float(v) for v in bounds)
+        if self.need_reinflation:
+            self.need_reinflation = False
+            return (-FLT_MAX, -FLT_MAX, FLT_MAX, FLT_MAX)
+        r = self.params["inflation_radius"]
+        return (min(last[0], bounds[0]) - r, min(last[1], bounds[1]) - r, max(last[2], bounds[2]) + r,
+                max(last[3], bounds[3]) + r)
+
+    def update_costs(self, master: Costmap, rect):
+        """InflationLayer::updateCosts of the master grid over rect = (min_i, min_j, max_i, max_j), on the device"""
+        master.emap.costmap_inflate(master.window, self.params, master.grid, rect)

@@ -25,6 +25,7 @@
 #include "../../include/gem_b200.h"
 #include "gem_add.cuh"
 #include "gem_costmap.cuh"
+#include "gem_inflate.cuh"
 #include "gem_kernels.cuh"
 #include "gem_global.cuh"
 #include "gem_ingest.cuh"
@@ -78,6 +79,14 @@ struct VoxScratch { // gem_voxel_grid (gem_voxel.cuh): keys and input indices be
 struct MlsScratch { // gem_mls_upsample (gem_mls.cuh): cell keys and indices before / after the sort, the points in cell
                    // order, the distinct cells, neighbour and output counts, output offsets, the long lists and their keys
     OctBuf key[2], idx[2], spts, ukey, ucnt, uoff, nbr, ocnt, ooff, longs, lkeys, temp, acc;
+};
+struct InflScratch { // gem_costmap_inflate (gem_inflate.cuh): per-cell keys and pop records, the tables, bin starts, block counts
+    OctBuf key, pops, tab, gstart, blk;
+    // the tables in `tab` were built for these parameters (r < 0: none)
+    long long r = -1;
+    double res = 0.0, weight = 0.0, inscribed = 0.0;
+    int nbins = 0, blocks = 0;
+    bool key_dirty = false; // `key` was (re)allocated and its clearing memset has not been enqueued yet
 };
 struct PcdScratch { // gem_pcd_format (gem_pcd.cuh): per-tile byte counts, their inclusive scan, the scan's temporary
     OctBuf bytes, ends, temp;
@@ -156,6 +165,7 @@ struct gem_map {
     VoxScratch vox;                // gem_voxel_grid
     MlsScratch mls;                // gem_mls_upsample
     PcdScratch pcd;                // gem_pcd_format
+    InflScratch infl;              // gem_costmap_inflate
     unsigned long long *d_stamps = nullptr; // gem_debug_stamps
     int *d_raylist = nullptr;      // ray clean-up: cells that cast a ray + their count
     uint32_t *d_bitmap = nullptr;  // ray clean-up: validity bitmap of the lowest layer (own tile / map-wide)
@@ -868,7 +878,8 @@ int gem_destroy(gem_map *m)
                           &m->mls.idx[1], &m->mls.spts, &m->mls.ukey, &m->mls.ucnt, &m->mls.uoff, &m->mls.nbr, &m->mls.ocnt,
                           &m->mls.ooff, &m->mls.longs, &m->mls.lkeys, &m->mls.temp, &m->mls.acc, &m->pc2_raw[0],
                           &m->pc2_raw[1], &m->pc2_raw[2], &m->pc2_img[0], &m->pc2_img[1], &m->pc2_img[2], &m->pc2_bgr,
-                          &m->pcd.bytes, &m->pcd.ends, &m->pcd.temp})
+                          &m->pcd.bytes, &m->pcd.ends, &m->pcd.temp, &m->infl.key, &m->infl.pops, &m->infl.tab,
+                          &m->infl.gstart, &m->infl.blk})
             if (b->p) cudaFree(b->p);
         if (m->h_ctr) cudaFreeHost(m->h_ctr);
         if (m->h_ctr_ring) cudaFreeHost(m->h_ctr_ring);
@@ -2005,6 +2016,126 @@ int gem_costmap_combine(gem_map *m, int mode, const unsigned char *layer_device,
     GEM_LAUNCH(m, GEM_PROF_OTHER, k_costmap_combine<<<grid, COST_BLOCK, 0, m->stream>>>(layer_device, master_device, size_x, i0, i1, j0, j1,
                                                                                     mode, vec));
     GEM_CUDA(m, cudaGetLastError());
+    return GEM_OK;
+}
+
+// InflationLayer::updateCosts (gem_inflate.cuh, DESIGN.md f14).  The host builds I2's tables with its libm, the bins (the
+// distinct table values <= r, in increasing order) and, per bin, the first bin that can push into it; one cooperative
+// kernel then runs the whole brushfire on the stream.
+int gem_costmap_inflate(gem_map *m, const gem_costmap_window *w, const gem_costmap_inflation *p, unsigned char *master_device,
+                        int min_i, int min_j, int max_i, int max_j)
+{
+    if (!m || !p || !master_device) return fail(m, GEM_ERR_INVALID, "gem_costmap_inflate: bad argument");
+    if (!cost_window_ok(w)) return fail(m, GEM_ERR_INVALID, "gem_costmap_inflate: bad window");
+    if (!std::isfinite(p->inflation_radius) || p->inflation_radius < 0.0 || !std::isfinite(p->cost_scaling_factor) ||
+        p->cost_scaling_factor < 0.0 || !std::isfinite(p->inscribed_radius) || p->inscribed_radius < 0.0)
+        return fail(m, GEM_ERR_INVALID, "gem_costmap_inflate: the radius, weight and inscribed radius must be finite and >= 0");
+    if (p->inflate_unknown != 0 && p->inflate_unknown != 1) return fail(m, GEM_ERR_INVALID, "gem_costmap_inflate: bad inflate_unknown");
+    const int sx = w->size_x, sy = w->size_y;
+    const double res = w->resolution;
+    // I1, with the DEFINED cap
+    const double cap = std::ceil(std::hypot((double)sx, (double)sy)) + 1.0;
+    const long long r = (long long)std::min(std::max(0.0, std::ceil(p->inflation_radius / res)), cap);
+    if (r == 0) return GEM_OK;
+    // DEFINED: the host tables grow with r^2, so r is bounded (a 16.8 M-entry table; 204 m at 0.05 m, 819 m at 0.2 m)
+    if (r > GEM_INFLATE_MAX_CELLS)
+        return fail(m, GEM_ERR_INVALID, "gem_costmap_inflate: the radius exceeds GEM_INFLATE_MAX_CELLS cells");
+    // I3: the widened rect, clamped
+    const long long i0 = std::max(0ll, (long long)min_i - r), i1 = std::min((long long)sx, (long long)max_i + r);
+    const long long j0 = std::max(0ll, (long long)min_j - r), j1 = std::min((long long)sy, (long long)max_j + r);
+    if (i0 >= i1 || j0 >= j1) return GEM_OK; // no seed
+    Lock lk(m->mu);
+    SetDev sd(m->dev);
+    InflScratch &S = m->infl;
+    const int tw = (int)r + 2;
+    const size_t T = (size_t)tw * tw;
+    const bool same = S.r == r && S.res == res && S.weight == p->cost_scaling_factor && S.inscribed == p->inscribed_radius;
+    std::vector<int> bin, lo;
+    std::vector<unsigned char> cost;
+    int nbins = S.nbins;
+    if (!same) try {
+        // I2: computeCaches
+        std::vector<double> dist(T);
+        cost.resize(T);
+        for (int i = 0; i < tw; i++)
+            for (int j = 0; j < tw; j++) {
+                const double d = std::hypot((double)i, (double)j);
+                dist[(size_t)i * tw + j] = d;
+                unsigned char c;
+                if (d == 0) c = COST_LETHAL;
+                else if (d * res <= p->inscribed_radius) c = 253;
+                else c = (unsigned char)(252 * std::exp(-1.0 * p->cost_scaling_factor * (d * res - p->inscribed_radius)));
+                cost[(size_t)i * tw + j] = c;
+            }
+        std::map<double, int> bins;
+        for (size_t t = 0; t < T; t++)
+            if (!(dist[t] > (double)r)) bins.emplace(dist[t], 0);
+        nbins = 0;
+        for (auto &kv : bins) kv.second = nbins++;
+        bin.assign(T, -1);
+        for (size_t t = 0; t < T; t++)
+            if (!(dist[t] > (double)r)) bin[t] = bins[dist[t]];
+        // lo[q]: the smallest bin holding a table neighbour of a cell of bin q (a push changes one |offset| by one)
+        lo.assign(nbins, INT32_MAX);
+        for (int i = 0; i < tw; i++)
+            for (int j = 0; j < tw; j++) {
+                const int q = bin[(size_t)i * tw + j];
+                if (q < 0) continue;
+                const int nb[4][2] = {{i - 1, j}, {i + 1, j}, {i, j - 1}, {i, j + 1}};
+                for (auto &n : nb) {
+                    if (n[0] < 0 || n[1] < 0 || n[0] >= tw || n[1] >= tw) continue;
+                    const int b = bin[(size_t)n[0] * tw + n[1]];
+                    if (b == q) return fail(m, GEM_ERR_INVALID, "gem_costmap_inflate: the distance table pushes a cell into its own bin");
+                    if (b >= 0 && b < lo[q]) lo[q] = b;
+                }
+            }
+        for (int q = 0; q < nbins; q++) lo[q] = std::min(lo[q], q);
+    } catch (const std::bad_alloc &) {
+        return fail(m, GEM_ERR_NOMEM, "gem_costmap_inflate: host memory for the distance tables");
+    }
+    // scratch, all grown before anything is written
+    const size_t ncells = (size_t)sx * sy;
+    const size_t tab_bytes = T * sizeof(int) + ((T + 15) / 16) * 16 + (size_t)nbins * sizeof(int);
+    if (!S.blocks) {
+        int per_sm = 0, sms = 0;
+        GEM_CUDA(m, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_inflate, INFL_BLOCK, 0));
+        GEM_CUDA(m, cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, m->dev));
+        S.blocks = std::max(1, std::min(per_sm, 4) * sms);
+    }
+    // A failed growth returns GEM_ERR_NOMEM, and a later call must still find consistent state: the tables are marked
+    // stale before `tab` may be replaced, and a replaced key buffer stays marked until its clearing memset is enqueued.
+    if (!same) S.r = -1;
+    void *old_key = S.key.p;
+    int rc = scratch_grow(m, S.key, ncells * 8, "gem_costmap_inflate");
+    if (S.key.p != old_key) S.key_dirty = true;
+    if (rc || (rc = scratch_grow(m, S.pops, ncells * 8, "gem_costmap_inflate")) ||
+        (rc = scratch_grow(m, S.tab, tab_bytes, "gem_costmap_inflate")) ||
+        (rc = scratch_grow(m, S.gstart, ((size_t)nbins + 1) * sizeof(int), "gem_costmap_inflate")) ||
+        (rc = scratch_grow(m, S.blk, (size_t)S.blocks * sizeof(int), "gem_costmap_inflate")))
+        return rc;
+    if (S.key_dirty) {
+        GEM_CUDA(m, cudaMemsetAsync(S.key.p, 0xFF, S.key.cap, m->stream)); // every cell unseen
+        S.key_dirty = false;
+    }
+    int *d_bin = S.tab.as<int>();
+    unsigned char *d_cost = reinterpret_cast<unsigned char *>(d_bin + T);
+    int *d_lo = reinterpret_cast<int *>(d_cost + ((T + 15) / 16) * 16);
+    if (!same) {
+        GEM_CUDA(m, cudaMemcpyAsync(d_bin, bin.data(), T * sizeof(int), cudaMemcpyHostToDevice, m->stream));
+        GEM_CUDA(m, cudaMemcpyAsync(d_cost, cost.data(), T, cudaMemcpyHostToDevice, m->stream));
+        GEM_CUDA(m, cudaMemcpyAsync(d_lo, lo.data(), (size_t)nbins * sizeof(int), cudaMemcpyHostToDevice, m->stream));
+        // from pageable memory each copy returns once its source is staged, so the vectors may go when this call returns
+        S.r = r;
+        S.res = res;
+        S.weight = p->cost_scaling_factor;
+        S.inscribed = p->inscribed_radius;
+        S.nbins = nbins;
+    }
+    GEM_CUDA(m, cudaMemsetAsync(S.gstart.p, 0, sizeof(int), m->stream));
+    InflateArgs a{master_device, sx, sy, (int)i0, (int)j0, (int)(i1 - i0), (int)(j1 - j0), d_bin, d_cost, d_lo, tw, nbins,
+                  p->inflate_unknown, S.key.as<unsigned long long>(), S.pops.as<int2>(), S.gstart.as<int>(), S.blk.as<int>()};
+    void *args[] = {&a};
+    GEM_LAUNCH(m, GEM_PROF_OTHER, GEM_CUDA(m, cudaLaunchCooperativeKernel((const void *)k_inflate, dim3((unsigned)S.blocks), dim3(INFL_BLOCK), args, 0, m->stream)));
     return GEM_OK;
 }
 

@@ -697,6 +697,18 @@ class ElevationMap:
         check(self._lib.gem_costmap_combine(self._h, _lib.COSTMAP_MODES[mode], pl, pm, int(size_x), int(size_y), i0, j0, i1, j1),
               self._h, "gem_costmap_combine")
 
+    def costmap_inflate(self, window, params, master, rect):
+        """InflationLayer::updateCosts (DESIGN.md f14) of the master grid over rect = (min_i, min_j, max_i, max_j);
+        params: a dict {inflation_radius, cost_scaling_factor, inscribed_radius, inflate_unknown}.  Asynchronous on
+        the library's stream (torch_stream())."""
+        w = self._cost_window(window)
+        p = _lib.GemCostmapInflation(float(params["inflation_radius"]), float(params["cost_scaling_factor"]),
+                                     float(params["inscribed_radius"]), 1 if params.get("inflate_unknown", False) else 0)
+        i0, j0, i1, j1 = (int(v) for v in rect)
+        check(self._lib.gem_costmap_inflate(self._h, C.byref(w), C.byref(p), self._cost_grid(master, w.size_x, w.size_y,
+                                                                                           "costmap_inflate"), i0, j0, i1, j1),
+              self._h, "gem_costmap_inflate")
+
     # -- the VoxelGrid pre-filter of GEM's demo launches (DESIGN.md f9) ---------------------------------------------------
     def voxel_grid(self, xyzi, leaf_size, field=None, limits=(-3.4028234663852886e38, 3.4028234663852886e38), negative=False,
                    out=None):

@@ -384,7 +384,7 @@ int gem_color_octree_read(gem_map *m, void *out, long long capacity);
  * update_origin and combine are asynchronous on the handle's stream and, like mark_points, work on any handle.  No call
  * modifies the map.  Every call rejects a bad window (size <= 0, size_x * size_y >= 2^31, a resolution that is <= 0 or not
  * finite); a rejected call writes nothing.  Out of scope: footprint clearing (footprint_clearing_enabled false),
- * InflationLayer (inflation_radius 0 in GEM's configs), publishing, and the elevation_map_available_ subscription gate. */
+ * publishing, and the elevation_map_available_ subscription gate.  InflationLayer is gem_costmap_inflate (DESIGN.md f14). */
 enum { GEM_COST_FREE = 0, GEM_COST_LETHAL = 254, GEM_COST_UNKNOWN = 255 };
 enum { GEM_COSTMAP_MAX = 0, GEM_COSTMAP_OVERWRITE = 1 };
 typedef struct gem_costmap_window {
@@ -402,6 +402,39 @@ int gem_costmap_mark_points(gem_map *m, const void *points32_device, int n, cons
 int gem_costmap_update_origin(gem_map *m, gem_costmap_window *w, double new_origin_x, double new_origin_y, unsigned char fill,
                               unsigned char *cost_device);
 int gem_costmap_combine(gem_map *m, int mode, const unsigned char *layer_device, unsigned char *master_device, int size_x, int size_y,
+                        int min_i, int min_j, int max_i, int max_j);
+
+/* ---- costmap_2d's InflationLayer::updateCosts on a master grid (GEM's global costmap; DESIGN.md f14) ----
+ * Restated from navigation 1.14 (unpinned):
+ *   I1 r = cellDistance(inflation_radius) = (unsigned)max(0.0, ceil(inflation_radius / resolution)); weight =
+ *      cost_scaling_factor; r == 0 writes nothing.  DEFINED: r is capped at ceil(hypot(size_x, size_y)) + 1, beyond which
+ *      every in-grid distance is within the radius and the result cannot change.  DEFINED: an r above GEM_INFLATE_MAX_CELLS
+ *      (after the cap) is GEM_ERR_INVALID, because the host tables grow with r^2.
+ *   I2 for 0 <= i, j <= r + 1: dist[i][j] = hypot(i, j); cost[i][j] = 254 when dist == 0, 253 when dist * resolution <=
+ *      inscribed_radius, else (unsigned char)(252 * exp(-weight * (dist * resolution - inscribed_radius))).  DEFINED: both
+ *      tables are computed on the host with its libm, as costmap_2d does, and uploaded.
+ *   I3 the rect [min_i, max_i) x [min_j, max_j) is widened by r on every side and clamped to the grid; its LETHAL cells are
+ *      the seeds of bin 0.0 in row-major order (j outer, i inner), each its own source.
+ *   I4 bins (std::map<double, std::vector<CellData>>) in increasing distance value, each in push order.  An entry whose cell
+ *      is seen is skipped; otherwise the cell is marked seen, c = cost[|mx - sx|][|my - sy|], and the master's old value o
+ *      becomes c if o == NO_INFORMATION && (inflate_unknown ? c > FREE : c >= 253), else max(o, c).  It then pushes
+ *      mx - 1, my - 1, mx + 1, my + 1 (inside the grid, unseen, same source) into bin dist[|nx - sx|][|ny - sy|] unless that
+ *      is > r.  Bins are keyed by the double values of the table; a push into a passed bin is never processed.  Any grid
+ *      cell within r of a seed can be written, inside the rect or not.  A table that would push a cell into its own bin
+ *      (a libm whose hypot is not monotone) is refused: GEM_ERR_INVALID.
+ * gem_costmap_inflate runs I3-I4 on master_device (size_x * size_y of the window; origin unused), asynchronously on the
+ * handle's stream; it works on any handle and does not read or modify the map.  The order-dependent brushfire is reproduced
+ * byte for byte.  Scratch on the handle: 16 bytes per cell plus the tables, grown on demand (a failed growth is GEM_ERR_NOMEM
+ * and writes nothing; the handle stays usable, and a later call computes the right bytes).  GEM_ERR_INVALID, with nothing
+ * written: NULL pointers, a bad window, a radius, weight or inscribed radius that is negative or not finite (DEFINED: a
+ * negative weight is refused), inflate_unknown other than 0 or 1, r above GEM_INFLATE_MAX_CELLS.
+ * The bounds (I5) and the inscribed radius of the footprint (I7) are host arithmetic: gem_b200/costmap.py. */
+enum { GEM_INFLATE_MAX_CELLS = 4094 };
+typedef struct gem_costmap_inflation {
+    double inflation_radius, cost_scaling_factor, inscribed_radius; /* metres, 1/metres, metres */
+    int inflate_unknown;                                            /* 0 or 1 */
+} gem_costmap_inflation;
+int gem_costmap_inflate(gem_map *m, const gem_costmap_window *w, const gem_costmap_inflation *p, unsigned char *master_device,
                         int min_i, int min_j, int max_i, int max_j);
 
 /* ---- the VoxelGrid pre-filter of GEM's demo launches (filter.launch, filter_kitti.launch; DESIGN.md f9) ----

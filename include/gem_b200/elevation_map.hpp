@@ -386,6 +386,13 @@ class ElevationMap {
     {
         check(gem_costmap_combine(h_, mode, layer_device, master_device, sizeX, sizeY, minI, minJ, maxI, maxJ), "gem_costmap_combine");
     }
+    // InflationLayer::updateCosts (DESIGN.md f14) of a master grid over [minI, maxI) x [minJ, maxJ), asynchronous on the
+    // handle's stream
+    void costmapInflate(const gem_costmap_window &w, const gem_costmap_inflation &p, unsigned char *master_device, int minI, int minJ,
+                        int maxI, int maxJ)
+    {
+        check(gem_costmap_inflate(h_, &w, &p, master_device, minI, minJ, maxI, maxJ), "gem_costmap_inflate");
+    }
     // pcl_ros's VoxelGrid nodelet (GEM's filter.launch / filter_kitti.launch; DESIGN.md f9) over n float4 {x, y, z, intensity}
     // in device memory: min(count, capacity) centroids go to out_device, which must not overlap the input (capacity 0 is
     // a size query).  Chain calls through two buffers.

@@ -4,7 +4,12 @@
   (75 x 75 at 0.2 m) and the global one (1000 x 1000 at 0.2 m), mark_unknown = 1;
 - gem_costmap_mark_points over 1 M and 4 M records (the c2 grid cloud, repeated and jittered) into 1000 x 1000;
 - gem_costmap_update_origin of a 1000 x 1000 grid by (3, -2) cells;
-- gem_costmap_combine over the whole 1000 x 1000 grid (max and overwrite).
+- gem_costmap_combine over the whole 1000 x 1000 grid (max and overwrite);
+- gem_costmap_inflate (DESIGN.md f14) of GEM's global costmap, 1000 x 1000 at 0.2 m whose master is PointMapLayer's
+  overwrite of the c2 grid cloud, over the update rect at GEM's 0.0 m (a no-op), costmap_2d's default 0.55 m (r = 3) and
+  2.0 m (r = 10), and over the whole grid at 0.55 m (the first update); and of a 4000 x 4000 grid at 0.05 m with the
+  same cloud marked, r = 40, over the whole grid, to show the cost of its many distance bins.  Factor 10, GEM's
+  footprint's inscribed radius 0.40 m.  Every call inflates the same master copy again, which is the same work.
 
 Each time is CUDA events on the library's stream around one Python call, the median of CALLS calls after WARM.  The
 interval therefore also holds the host's time between the launches (argument checks, waiting for the torch stream) and,
@@ -29,6 +34,8 @@ sys.path.insert(0, os.path.join(ROOT, "tests"))
 import gem_b200  # noqa: E402
 from gem_b200 import synth  # noqa: E402
 import costmap_oracle  # noqa: E402
+import inflation_oracle  # noqa: E402
+from gem_b200 import costmap  # noqa: E402
 
 WARM, CALLS, ORACLE_RUNS = 5, 50, 3
 
@@ -65,6 +72,35 @@ def host_ms(fn):
         fn()
         t.append((time.perf_counter() - t0) * 1e3)
     return float(np.median(t))
+
+
+def inflation_rows(g, cloud, centre, out):
+    ok = True
+    ins = costmap.inscribed_radius(costmap.GEM_FOOTPRINT)
+    cx, cy = float(centre[0]), float(centre[1])
+    for size, res, runs in ((1000, 0.2, (("0.0", None), ("0.55", None), ("2.0", None), ("0.55", "whole"))),
+                            (4000, 0.05, (("2.0", "whole"),))):
+        w = (cx - size * res / 2, cy - size * res / 2, res, size, size)
+        layer = torch.full((size, size), 255, dtype=torch.uint8, device="cuda:0")
+        marks = g.costmap_mark_points(cloud, w, layer, 0.7)
+        rect = costmap.update_rect(w, marks)
+        master0 = costmap_oracle.combine(1, layer.cpu().numpy(), np.zeros((size, size), np.uint8), size, size, rect)
+        out[f"inflate_{size}_lethal_cells"] = int((master0 == 254).sum())
+        out[f"inflate_{size}_rect"] = list(rect)
+        for radius, where in runs:
+            p = inflation_oracle.params(float(radius), 10.0, ins)
+            r = (0, 0, size, size) if where else rect
+            key = f"inflate_{size}_{radius}m" + ("_whole" if where else "")
+            grid = torch.from_numpy(master0).cuda()
+            out[f"{key}_ms"] = device_ms(g, lambda: g.costmap_inflate(w, p, grid, r))
+            out[f"{key}_oracle_ms"] = host_ms(lambda: inflation_oracle.inflate(master0, res, p, r))
+            grid = torch.from_numpy(master0).cuda()
+            g.costmap_inflate(w, p, grid, r)
+            g.sync()
+            want = inflation_oracle.inflate(master0, res, p, r)
+            out[f"{key}_cells_changed"] = int((want != master0).sum())
+            ok &= np.array_equal(grid.cpu().numpy(), want)
+    return ok
 
 
 def main():
@@ -136,6 +172,7 @@ def main():
         g.costmap_combine(mode, lay, mas, 1000, 1000, (0, 0, 1000, 1000))
         g.sync()
         ok &= np.array_equal(mas.cpu().numpy(), costmap_oracle.combine(mid, lay0, grid0, 1000, 1000, (0, 0, 1000, 1000)))
+    ok &= inflation_rows(g, cloud, centre, out)
     out["outputs_equal_oracle"] = bool(ok)
     print(json.dumps(out))
     return 0 if ok else 1
