@@ -3,4 +3,4 @@ hot path (the reference's libgpu.so).  The product is the CUDA library behind in
 this package is its Python host mirror used by tests and benchmarks."""
 from ._lib import GemError, GemFrame, GemSensorModel, load  # noqa: F401
 from .elevation_map import (CameraImage, ElevationMap, LaserSensorProcessor, PerfectSensorProcessor,  # noqa: F401
-                            PointCloud2Layout, StereoSensorProcessor, StructuredLightSensorProcessor, make_frame)
+                            PointCloud2Layout, RosHeader, StereoSensorProcessor, StructuredLightSensorProcessor, make_frame)

@@ -134,6 +134,14 @@ class GemCameraImage(C.Structure):
                 ("height", C.c_int), ("step", C.c_int), ("data", C.c_void_p)]
 
 
+class GemRosHeader(C.Structure):
+    _fields_ = [("seq", C.c_uint), ("stamp_sec", C.c_uint), ("stamp_nsec", C.c_uint), ("frame_id", C.c_char_p)]
+
+
+class GemRosPart(C.Structure):
+    _fields_ = [("points32", C.c_void_p), ("n", C.c_longlong)]
+
+
 COST_FREE, COST_LETHAL, COST_UNKNOWN = 0, 254, 255           # GEM_COST_*
 INFLATE_MAX_CELLS = 4094                                     # GEM_INFLATE_MAX_CELLS
 COSTMAP_MODES = {"max": 0, "overwrite": 1}                  # GEM_COSTMAP_MAX / GEM_COSTMAP_OVERWRITE
@@ -228,6 +236,12 @@ SYMBOLS = {
                                                  C.POINTER(GemFrame)]),
     "gem_pcd_header": (C.c_int, [C.c_longlong, C.c_int, C.c_char_p, C.c_int, _IP]),
     "gem_pcd_format": (C.c_int, [_P, _P, C.c_int, C.c_int, _P, C.c_longlong, C.POINTER(C.c_longlong)]),
+    "gem_ros_grid_map": (C.c_int, [_P, C.POINTER(GemRosHeader), _P, C.c_longlong, C.POINTER(C.c_longlong)]),
+    "gem_ros_orthomosaic": (C.c_int, [_P, C.POINTER(GemRosHeader), _P, C.c_longlong, C.POINTER(C.c_longlong)]),
+    "gem_ros_visual_points": (C.c_int, [_P, C.POINTER(GemRosHeader), _P, C.c_longlong, C.POINTER(C.c_longlong)]),
+    "gem_ros_cloud": (C.c_int, [_P, C.POINTER(GemRosHeader), C.POINTER(GemRosPart), C.c_int, C.c_int, _P, C.c_longlong,
+                                C.POINTER(C.c_longlong)]),
+    "gem_ros_octomap": (C.c_int, [_P, C.POINTER(GemRosHeader), _P, C.c_longlong, C.POINTER(C.c_longlong)]),
 }
 
 _lib = None

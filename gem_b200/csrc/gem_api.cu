@@ -32,6 +32,7 @@
 #include "gem_mls.cuh"
 #include "gem_octree.cuh"
 #include "gem_pcd.cuh"
+#include "gem_rosmsg.cuh"
 #include "gem_route.cuh"
 #include "gem_submap.cuh"
 #include "gem_voxel.cuh"
@@ -94,6 +95,7 @@ struct PcdScratch { // gem_pcd_format (gem_pcd.cuh): per-tile byte counts, their
 struct OctScratch { // gem_color_octree (gem_octree.cuh); every buffer is consistent with its own capacity at all times
     OctBuf code[2], idx[2], leaf, cnt, off, level, ghead, gid, val, groups, ctr, temp, key2[2], nkey[2], nrec[2], dense;
     long long bytes = -1; // size of the last stream (in nrec[1]); -1: none
+    double res = 0.0;     // the resolution it was built at
     gem_octree info{};
 };
 
@@ -165,6 +167,8 @@ struct gem_map {
     VoxScratch vox;                // gem_voxel_grid
     MlsScratch mls;                // gem_mls_upsample
     PcdScratch pcd;                // gem_pcd_format
+    OctBuf ros_framing;            // gem_ros_*: the framing bytes of the call, staged for k_ros_framing
+    OctBuf ros_stage;              // gem_ros_* map messages for pinned outputs, written here and copied over in one DMA
     InflScratch infl;              // gem_costmap_inflate
     unsigned long long *d_stamps = nullptr; // gem_debug_stamps
     int *d_raylist = nullptr;      // ray clean-up: cells that cast a ray + their count
@@ -879,7 +883,7 @@ int gem_destroy(gem_map *m)
                           &m->mls.ooff, &m->mls.longs, &m->mls.lkeys, &m->mls.temp, &m->mls.acc, &m->pc2_raw[0],
                           &m->pc2_raw[1], &m->pc2_raw[2], &m->pc2_img[0], &m->pc2_img[1], &m->pc2_img[2], &m->pc2_bgr,
                           &m->pcd.bytes, &m->pcd.ends, &m->pcd.temp, &m->infl.key, &m->infl.pops, &m->infl.tab,
-                          &m->infl.gstart, &m->infl.blk})
+                          &m->infl.gstart, &m->infl.blk, &m->ros_framing, &m->ros_stage})
             if (b->p) cudaFree(b->p);
         if (m->h_ctr) cudaFreeHost(m->h_ctr);
         if (m->h_ctr_ring) cudaFreeHost(m->h_ctr_ring);
@@ -1776,6 +1780,7 @@ int gem_color_octree(gem_map *m, const void *points32_device, int n, double reso
     gem_octree r{};
     if (n == 0) {
         S.bytes = 0;
+        S.res = resolution;
         S.info = r;
         *info = r;
         return GEM_OK;
@@ -1875,6 +1880,7 @@ int gem_color_octree(gem_map *m, const void *points32_device, int n, double reso
     r.inserted = hc.inserted;
     r.skipped = n - hc.inserted;
     S.bytes = r.bytes;
+    S.res = resolution;
     S.info = r;
     *info = r;
     return GEM_OK;
@@ -3074,6 +3080,213 @@ int gem_pcd_format(gem_map *m, const void *points32_device, int n, int flags, vo
                                                                                      m->pcd.ends.as<long long>(), out));
     GEM_CUDA(m, cudaGetLastError());
     GEM_CUDA(m, cudaStreamSynchronize(st));
+    return GEM_OK;
+}
+
+// ---- the node's map topics as serialised ROS1 messages (gem_rosfmt.h, gem_rosmsg.cuh; f15) -----------------------------
+// the checks every gem_ros_* call makes first.  *pinned: out is page-locked host memory (the kernels may store to
+// device, managed and pinned memory; pageable host memory is refused, since a store to it from the device faults)
+static int ros_args(gem_map *m, const gem_ros_header *h, void *out, long long capacity, long long *bytes_out, const char *what,
+                    bool *pinned)
+{
+    if (bytes_out) *bytes_out = 0;
+    if (!m) return GEM_ERR_INVALID;
+    if (!bytes_out || capacity < 0 || (capacity > 0 && !out)) return fail(m, GEM_ERR_INVALID, std::string(what) + ": bad argument");
+    if (!gem_ros::header_ok(h)) return fail(m, GEM_ERR_INVALID, std::string(what) + ": NULL header or frame_id");
+    if (m->geom.tiled) return fail(m, GEM_ERR_INVALID, std::string(what) + ": not available on tiled handles");
+    *pinned = false;
+    if (out) {
+        cudaPointerAttributes a{};
+        if (cudaPointerGetAttributes(&a, out) != cudaSuccess) {
+            cudaGetLastError(); // an unknown pointer: treated as pageable
+            a.type = cudaMemoryTypeUnregistered;
+        }
+        if (a.type == cudaMemoryTypeUnregistered)
+            return fail(m, GEM_ERR_INVALID, std::string(what) + ": out is pageable host memory (device or pinned memory only)");
+        *pinned = a.type == cudaMemoryTypeHost;
+    }
+    return GEM_OK;
+}
+
+// Where a map message's kernels write: device memory directly; for pinned host memory a device staging buffer at the
+// same 16-byte phase (so the kernels take the same paths and write the same bytes), copied to `out` in one DMA transfer
+// by ros_unstage.  The kernels' own stores across PCIe were measured slower than the copy (DESIGN.md f15).
+static int ros_stage(gem_map *m, unsigned char *out, long long size, bool pinned, unsigned char **dst)
+{
+    *dst = out;
+    if (!pinned) return GEM_OK;
+    const int rc = scratch_grow(m, m->ros_stage, (size_t)size + 16, "gem_ros staging");
+    if (rc) return rc;
+    *dst = m->ros_stage.as<unsigned char>() + ((uintptr_t)out & 15u);
+    return GEM_OK;
+}
+static int ros_unstage(gem_map *m, unsigned char *out, const unsigned char *dst, long long size, bool pinned)
+{
+    if (pinned) GEM_CUDA(m, cudaMemcpyAsync(out, dst, (size_t)size, cudaMemcpyDeviceToHost, m->stream));
+    return GEM_OK;
+}
+
+// the framing bytes into their places in `out`; the caller holds the lock.  They go to the device from pageable memory,
+// which CUDA copies to its staging memory before cudaMemcpyAsync returns, so `f` may go as soon as this returns, and the
+// device buffer is reused in stream order.
+static int ros_put_framing(gem_map *m, const gem_ros::Framing &f, unsigned char *out)
+{
+    const int rc = scratch_grow(m, m->ros_framing, f.bytes.size(), "gem_ros framing");
+    if (rc) return rc;
+    GEM_CUDA(m, cudaMemcpyAsync(m->ros_framing.p, f.bytes.data(), f.bytes.size(), cudaMemcpyHostToDevice, m->stream));
+    RosSegs s{};
+    for (int k = 0; k < f.nseg; k++) {
+        s.at[k] = f.seg[k].at;
+        s.src[k] = f.seg[k].src;
+        s.len[k] = f.seg[k].len;
+    }
+    GEM_LAUNCH(m, GEM_PROF_OTHER, k_ros_framing<<<f.nseg, 256, 0, m->stream>>>(m->ros_framing.as<unsigned char>(), s, out));
+    GEM_CUDA(m, cudaGetLastError());
+    return GEM_OK;
+}
+
+int gem_ros_grid_map(gem_map *m, const gem_ros_header *h, void *out, long long capacity, long long *bytes_out)
+{
+    bool pinned = false;
+    int rc = ros_args(m, h, out, capacity, bytes_out, "gem_ros_grid_map", &pinned);
+    if (rc) return rc;
+    Lock lk(m->mu);
+    SetDev sd(m->dev);
+    const GridMapFrame gf = grid_frame(m, m->geom.cx, m->geom.cy, m->geom.sx, m->geom.sy);
+    gem_ros::Framing f;
+    if (gem_ros::grid_map(*h, m->L, gf.res, gf.cx, gf.cy, m->geom.sx, m->geom.sy, f))
+        return fail(m, GEM_ERR_INVALID, "gem_ros_grid_map: a layer of more than 2^32 bytes");
+    if (capacity < f.size) { // a size query, or too small: nothing is written
+        *bytes_out = f.size;
+        return GEM_OK;
+    }
+    unsigned char *o = nullptr;
+    if ((rc = ros_stage(m, static_cast<unsigned char *>(out), f.size, pinned, &o)) || (rc = flush_for_observer(m)) ||
+        (rc = ros_put_framing(m, f, o)))
+        return rc;
+    const int nch = (m->L + 31) / 32;
+    GEM_LAUNCH(m, GEM_PROF_OTHER, k_ros_grid_map<<<dim3(nch, nch), 256, 0, m->stream>>>(m->ml, m->L, o + f.payload_at[0],
+                                                                                         f.payload_at[1] - f.payload_at[0]));
+    GEM_CUDA(m, cudaGetLastError());
+    if ((rc = ros_unstage(m, static_cast<unsigned char *>(out), o, f.size, pinned))) return rc;
+    *bytes_out = f.size;
+    return GEM_OK;
+}
+
+int gem_ros_orthomosaic(gem_map *m, const gem_ros_header *h, void *out, long long capacity, long long *bytes_out)
+{
+    bool pinned = false;
+    int rc = ros_args(m, h, out, capacity, bytes_out, "gem_ros_orthomosaic", &pinned);
+    if (rc) return rc;
+    Lock lk(m->mu);
+    SetDev sd(m->dev);
+    gem_ros::Framing f;
+    if (gem_ros::image(*h, m->L, f)) return fail(m, GEM_ERR_INVALID, "gem_ros_orthomosaic: an image of more than 2^32 bytes");
+    if (capacity < f.size) {
+        *bytes_out = f.size;
+        return GEM_OK;
+    }
+    unsigned char *o = nullptr;
+    if ((rc = ros_stage(m, static_cast<unsigned char *>(out), f.size, pinned, &o)) || (rc = flush_for_observer(m)) ||
+        (rc = ros_put_framing(m, f, o)))
+        return rc;
+    unsigned char *img = o + f.payload_at[0];
+    const long long nwords = ((long long)((uintptr_t)img & 15u) + f.payload_len[0] + 15) / 16;
+    GEM_LAUNCH(m, GEM_PROF_OTHER, k_ros_orthomosaic<<<(unsigned)((nwords + 255) / 256), 256, 0, m->stream>>>(m->geom, m->ml, img, nwords));
+    GEM_CUDA(m, cudaGetLastError());
+    if ((rc = ros_unstage(m, static_cast<unsigned char *>(out), o, f.size, pinned))) return rc;
+    *bytes_out = f.size;
+    return GEM_OK;
+}
+
+int gem_ros_visual_points(gem_map *m, const gem_ros_header *h, void *out, long long capacity, long long *bytes_out)
+{
+    bool pinned = false;
+    int rc = ros_args(m, h, out, capacity, bytes_out, "gem_ros_visual_points", &pinned);
+    if (rc) return rc;
+    Lock lk(m->mu);
+    SetDev sd(m->dev);
+    if ((rc = flush_for_observer(m))) return rc;
+    RosVisualSrc src;
+    src.ml = m->ml;
+    src.f = grid_frame(m, m->geom.cx, m->geom.cy, m->geom.sx, m->geom.sy);
+    src.out = nullptr;
+    int n = 0;
+    if ((rc = compact_cells(m, src, 0, &n))) return rc; // the count alone
+    gem_ros::Framing f;
+    if (gem_ros::cloud(*h, gem_ros::CLOUD_XYZRGB, n, 1, f))
+        return fail(m, GEM_ERR_INVALID, "gem_ros_visual_points: 32 n >= 2^32 (PointCloud2's data length is a uint32)");
+    if (capacity < f.size) {
+        *bytes_out = f.size;
+        return GEM_OK;
+    }
+    unsigned char *o = nullptr;
+    if ((rc = ros_stage(m, static_cast<unsigned char *>(out), f.size, pinned, &o)) || (rc = ros_put_framing(m, f, o))) return rc;
+    src.out = o + f.payload_at[0];
+    int *d_total = nullptr;
+    if ((rc = compact_cells_issue(m, src, n, &d_total)) || (rc = ros_unstage(m, static_cast<unsigned char *>(out), o, f.size, pinned)))
+        return rc;
+    GEM_CUDA(m, cudaStreamSynchronize(m->stream));
+    *bytes_out = f.size;
+    return GEM_OK;
+}
+
+int gem_ros_cloud(gem_map *m, const gem_ros_header *h, const gem_ros_part *parts, int nparts, int is_dense, void *out,
+                  long long capacity, long long *bytes_out)
+{
+    bool pinned = false;
+    int rc = ros_args(m, h, out, capacity, bytes_out, "gem_ros_cloud", &pinned);
+    if (rc) return rc;
+    if (nparts < 0 || (nparts > 0 && !parts)) return fail(m, GEM_ERR_INVALID, "gem_ros_cloud: nparts < 0 or no parts");
+    long long n = 0;
+    for (int i = 0; i < nparts; i++) {
+        if (parts[i].n < 0 || (parts[i].n > 0 && !parts[i].points32))
+            return fail(m, GEM_ERR_INVALID, "gem_ros_cloud: a part with n < 0 or without records");
+        n += std::min(parts[i].n, gem_ros::U32_LIMIT); // no overflow; any sum this large is refused below
+    }
+    gem_ros::Framing f;
+    if (gem_ros::cloud(*h, gem_ros::CLOUD_XYZRGBICT, n, is_dense, f))
+        return fail(m, GEM_ERR_INVALID, "gem_ros_cloud: 32 n >= 2^32 (PointCloud2's data length is a uint32)");
+    if (capacity < f.size) {
+        *bytes_out = f.size;
+        return GEM_OK;
+    }
+    for (int i = 0; i < nparts; i++)
+        if (parts[i].n > 0 && ranges_meet(parts[i].points32, (size_t)parts[i].n * 32, out, (size_t)f.size))
+            return fail(m, GEM_ERR_INVALID, "gem_ros_cloud: the output overlaps a part");
+    Lock lk(m->mu);
+    SetDev sd(m->dev);
+    unsigned char *o = static_cast<unsigned char *>(out);
+    if ((rc = ros_put_framing(m, f, o))) return rc;
+    long long at = f.payload_at[0];
+    for (int i = 0; i < nparts; i++) {
+        if (parts[i].n == 0) continue;
+        GEM_CUDA(m, cudaMemcpyAsync(o + at, parts[i].points32, (size_t)parts[i].n * 32, cudaMemcpyDefault, m->stream));
+        at += 32 * parts[i].n;
+    }
+    *bytes_out = f.size;
+    return GEM_OK;
+}
+
+int gem_ros_octomap(gem_map *m, const gem_ros_header *h, void *out, long long capacity, long long *bytes_out)
+{
+    bool pinned = false;
+    int rc = ros_args(m, h, out, capacity, bytes_out, "gem_ros_octomap", &pinned);
+    if (rc) return rc;
+    Lock lk(m->mu);
+    SetDev sd(m->dev);
+    const long long bytes = m->oct.bytes;
+    if (bytes < 0) return fail(m, GEM_ERR_INVALID, "gem_ros_octomap: no octree has been built");
+    gem_ros::Framing f;
+    if (gem_ros::octomap(*h, m->oct.res, bytes, f)) return fail(m, GEM_ERR_INVALID, "gem_ros_octomap: a stream of 2^32 bytes or more");
+    if (capacity < f.size) {
+        *bytes_out = f.size;
+        return GEM_OK;
+    }
+    unsigned char *o = static_cast<unsigned char *>(out);
+    if ((rc = ros_put_framing(m, f, o))) return rc;
+    if (bytes) GEM_CUDA(m, cudaMemcpyAsync(o + f.payload_at[0], m->oct.nrec[1].p, (size_t)bytes, cudaMemcpyDefault, m->stream));
+    *bytes_out = f.size;
     return GEM_OK;
 }
 

@@ -218,6 +218,18 @@ class CameraImage:
 
 
 # ------------------------------------------------------------------------------------------
+@dataclass
+class RosHeader:
+    """std_msgs/Header as the gem_ros_* calls write it (DESIGN.md f15 W1): seq, stamp (sec, nsec) and frame_id, as given"""
+    seq: int = 0
+    stamp_sec: int = 0
+    stamp_nsec: int = 0
+    frame_id: str = ""
+
+    def c(self) -> _lib.GemRosHeader:
+        return _lib.GemRosHeader(int(self.seq), int(self.stamp_sec), int(self.stamp_nsec), self.frame_id.encode())
+
+
 class ElevationMap:
     """One robot-centric elevation grid resident on one H100.
 
@@ -993,6 +1005,118 @@ class ElevationMap:
                 pass
             raise
         return size
+
+    # -- the node's map topics as serialised ROS1 messages (DESIGN.md f15) ---------------------------------------------------
+    # Each returns the message's bytes as a uint8 tensor: a new CUDA tensor, or a view of `out`, a contiguous uint8 CUDA
+    # tensor or pinned CPU tensor that must hold them all (the device writes pinned memory directly).  The call is
+    # complete when it returns.
+    def _ros_buffer(self, out, what: str):
+        import torch
+        if not (isinstance(out, torch.Tensor) and out.dtype == torch.uint8 and out.is_contiguous()
+                and (out.is_cuda or out.is_pinned())):
+            raise ValueError(f"{what}: out must be a contiguous uint8 CUDA tensor or pinned CPU tensor")
+        return out.view(-1)
+
+    def _ros_write(self, what: str, call, out, offset: int = 0) -> int:
+        """call(ptr, capacity, bytes_out) into out[offset:]; returns the bytes written (raises when they do not fit)"""
+        nb = C.c_longlong()
+        cap = out.numel() - offset
+        check(call(C.c_void_p(out.data_ptr() + offset) if cap > 0 else None, cap, C.byref(nb)), self._h, what)
+        if nb.value > cap:
+            raise ValueError(f"{what}: out holds {cap} bytes, {nb.value} are needed")
+        return nb.value
+
+    def _ros_size(self, what: str, call) -> int:
+        nb = C.c_longlong()
+        check(call(None, 0, C.byref(nb)), self._h, what)
+        return nb.value
+
+    def _ros_message(self, what: str, call, out):
+        import torch
+        dev = torch.device("cuda", self._device_index())
+        out = (torch.empty(self._ros_size(what, call), dtype=torch.uint8, device=dev) if out is None
+               else self._ros_buffer(out, what))
+        torch.cuda.current_stream(dev).synchronize()   # the library writes on its own stream
+        n = self._ros_write(what, call, out)
+        self.sync()
+        return out[:n]
+
+    def ros_grid_map(self, header: RosHeader, out=None):
+        """visual_map (grid_map_msgs/GridMap, W2): export_layers' 9 layers bit for bit, with the map's geometry"""
+        h = header.c()
+        return self._ros_message("gem_ros_grid_map", lambda p, c, nb: self._lib.gem_ros_grid_map(self._h, C.byref(h), p, c, nb), out)
+
+    def ros_orthomosaic(self, header: RosHeader | None = None, out=None):
+        """orthomosaic (sensor_msgs/Image "bgr8", W3) of export_orthomosaic's image; show() publishes it with an empty header
+        (the default)"""
+        h = (header or RosHeader()).c()
+        return self._ros_message("gem_ros_orthomosaic",
+                                 lambda p, c, nb: self._lib.gem_ros_orthomosaic(self._h, C.byref(h), p, c, nb), out)
+
+    def ros_visual_points(self, header: RosHeader, out=None):
+        """visualpoints (PointCloud2 of pcl::PointXYZRGB, W6) of export_visual_points' points, in its order"""
+        h = header.c()
+        return self._ros_message("gem_ros_visual_points",
+                                 lambda p, c, nb: self._lib.gem_ros_visual_points(self._h, C.byref(h), p, c, nb), out)
+
+    def _ros_parts(self, parts):
+        """gem_ros_part array of (n, 8) float32 record arrays (CUDA tensors, CPU tensors or numpy arrays), kept alive"""
+        keep, arr = [], (_lib.GemRosPart * max(len(parts), 1))()
+        for i, p in enumerate(parts):
+            if isinstance(p, np.ndarray):
+                p = np.ascontiguousarray(p)
+                ok = p.dtype in (np.float32, np.uint32) and p.ndim == 2 and p.shape[1] == 8
+            else:
+                ok = p.element_size() == 4 and p.dim() == 2 and p.shape[1] == 8 and p.is_contiguous()
+            if not ok:
+                raise ValueError("ros_cloud: every part must be a contiguous (n, 8) array of 32-bit words")
+            keep.append(p)
+            arr[i].points32 = _ptr(p).value if p.shape[0] else None
+            arr[i].n = int(p.shape[0])
+        return arr, keep
+
+    def ros_cloud(self, header: RosHeader, parts, is_dense: bool = True, out=None):
+        """history_point / global_point (PointCloud2 of PointXYZRGBICT, W5): the parts' records back to back (device,
+        pinned or pageable host memory); is_dense as pcl::PointCloud's flag (push_back and operator+ leave it true)"""
+        h = header.c()
+        arr, keep = self._ros_parts(list(parts))
+        n = len(keep)
+        return self._ros_message("gem_ros_cloud", lambda p, c, nb: self._lib.gem_ros_cloud(
+            self._h, C.byref(h), arr, n, 1 if is_dense else 0, p, c, nb), out)
+
+    def ros_octomap(self, header: RosHeader, out=None):
+        """road_octomap / obs_octomap (octomap_msgs/Octomap, W7) of the last color_octree's stream and resolution"""
+        h = header.c()
+        return self._ros_message("gem_ros_octomap", lambda p, c, nb: self._lib.gem_ros_octomap(self._h, C.byref(h), p, c, nb), out)
+
+    def ros_submap(self, records, keyframe_pc: bytes, pose, header: RosHeader, image_header: RosHeader | None = None,
+                   is_dense: bool = True, out=None):
+        """submap (dislam_msgs/SubMap, W8): the cloud of `records` (W5), the received keyframe cloud's serialised bytes as
+        they are, this map's orthomosaic (W3) and the pose (position xyz, orientation xyzw) as 7 float64, each part
+        written at its offset in one buffer"""
+        import torch
+        import struct
+        h, ih = header.c(), (image_header or RosHeader()).c()
+        arr, keep = self._ros_parts([records])
+        cloud = lambda p, c, nb: self._lib.gem_ros_cloud(self._h, C.byref(h), arr, 1, 1 if is_dense else 0, p, c, nb)
+        image = lambda p, c, nb: self._lib.gem_ros_orthomosaic(self._h, C.byref(ih), p, c, nb)
+        kf = np.frombuffer(bytes(keyframe_pc), np.uint8)
+        tail = np.frombuffer(struct.pack("<7d", *[float(v) for v in pose]), np.uint8)
+        n_cloud, n_image = self._ros_size("gem_ros_cloud", cloud), self._ros_size("gem_ros_orthomosaic", image)
+        size = n_cloud + kf.size + n_image + tail.size
+        dev = torch.device("cuda", self._device_index())
+        out = torch.empty(size, dtype=torch.uint8, device=dev) if out is None else self._ros_buffer(out, "ros_submap")
+        if out.numel() < size:
+            raise ValueError(f"ros_submap: out holds {out.numel()} bytes, {size} are needed")
+        torch.cuda.current_stream(dev).synchronize()
+        self._ros_write("gem_ros_cloud", cloud, out, 0)
+        self._ros_write("gem_ros_orthomosaic", image, out, n_cloud + kf.size)
+        self.sync()
+        out[n_cloud:n_cloud + kf.size].copy_(torch.from_numpy(kf.copy()))
+        out[size - tail.size:size].copy_(torch.from_numpy(tail.copy()))
+        if out.is_cuda:
+            torch.cuda.current_stream(dev).synchronize()
+        return out[:size]
 
     def get_layer_device(self, name: str, out):
         """dense (rows, cols) copy of a layer into a device tensor (float32, int32 for colours)"""

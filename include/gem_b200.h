@@ -647,6 +647,51 @@ int gem_pcd_header(long long n, int flags, char *out, int capacity, int *len_out
 int gem_pcd_format(gem_map *m, const void *points32_device, int n, int flags, void *out_device, long long capacity,
                    long long *bytes_out);
 
+/* ---- the node's map topics as serialised ROS1 messages (show()'s publishes, ElevationMap.cpp:123-147, and the clouds
+ * and octomaps of ElevationMapping.cpp:491-531, :662-681; DESIGN.md f15) ----
+ * The bytes roscpp would put on the wire for visual_map (grid_map_msgs/GridMap), orthomosaic (sensor_msgs/Image),
+ * visualpoints (PointCloud2 of pcl::PointXYZRGB), history_point / global_point / the SubMap's cloud (PointCloud2 of
+ * PointXYZRGBICT) and road_octomap / obs_octomap (octomap_msgs/Octomap), restated (W1-W8 in gem_b200/csrc/gem_rosfmt.h;
+ * ROS, grid_map, PCL and cv_bridge are unpinned).  A node can publish them as they are (e.g. topic_tools::ShapeShifter).
+ *   header: {seq, stamp, frame_id} written as given (W1).
+ *   gem_ros_grid_map: the 9 layers of gem_export_layers bit for bit (column-major, storage order), resolution = the
+ *     handle's grid_resolution (or its float resolution), length_x = length_y = L * resolution (double), pose position =
+ *     the handle's centre (cx, cy, 0) -- DEFINED as the centre gem_export_visual_points and gem_export_grid_cloud compute
+ *     positions from, which after gem_opt_move is the aligned optimised centre (the reference's visualMap_ keeps the last
+ *     ElevationMap::move's) -- orientation (0, 0, 0, 1), start index (sx, sy) as uint16.  737 + |frame_id| + 36 L^2 bytes.
+ *   gem_ros_orthomosaic: gem_export_orthomosaic's image, "bgr8", step 3L.  41 + |frame_id| + 3 L^2 bytes.
+ *   gem_ros_visual_points: one record {x, y, z, 1.0f, b, g, r, 0xff, 12 zero bytes} per point of gem_export_visual_points,
+ *     in its order (the bytes the reference leaves uninitialised DEFINED as 0); is_dense 1.  100 + |frame_id| + 32n bytes.
+ *     Host-synchronous (the size needs the shown-cell count).
+ *   gem_ros_cloud: the nparts parts' n 32-byte PointXYZRGBICT records each, back to back (byte copies; device, pinned or
+ *     pageable host memory).  165 + |frame_id| + 32 * sum(n) bytes; a sum with 32 * sum >= 2^32 is GEM_ERR_INVALID.
+ *   gem_ros_octomap: the last gem_color_octree stream (gem_color_octree_read's bytes), id "ColorOcTree", binary 0, that
+ *     build's resolution.  44 + |frame_id| + bytes.  GEM_ERR_INVALID when no octree has been built.
+ * Common to all five: out is device or pinned host memory at any alignment; pageable host memory is GEM_ERR_INVALID.
+ *   The map messages are written by the kernels in place into device memory, and for pinned memory into a device staging
+ *   buffer on the handle (grown on demand) that one DMA copy moves to out; clouds and the octree stream are byte copies.
+ * *bytes_out is always set (0 on an error); the message is written whole when it fits in capacity, and nothing
+ * otherwise (out NULL with capacity 0 is a size query).  No byte outside [out, out + size) is written.  GEM_ERR_INVALID,
+ * writing nothing: a NULL header or frame_id, capacity < 0, out NULL with capacity > 0, nparts < 0, a part with n < 0 or
+ * NULL records with n > 0, an output overlapping a part, a tiled handle (as for the other post-processing calls).
+ * The calls read what gem_export_layers reads and change nothing; asynchronous on the handle's stream except
+ * gem_ros_visual_points.  No allocation per call beyond the framing and staging buffers on the handle, which grow on
+ * demand. */
+typedef struct gem_ros_header {
+    unsigned seq, stamp_sec, stamp_nsec;
+    const char *frame_id;
+} gem_ros_header;
+typedef struct gem_ros_part {
+    const void *points32;         /* n 32-byte records                                        */
+    long long n;
+} gem_ros_part;
+int gem_ros_grid_map(gem_map *m, const gem_ros_header *h, void *out, long long capacity, long long *bytes_out);
+int gem_ros_orthomosaic(gem_map *m, const gem_ros_header *h, void *out, long long capacity, long long *bytes_out);
+int gem_ros_visual_points(gem_map *m, const gem_ros_header *h, void *out, long long capacity, long long *bytes_out);
+int gem_ros_cloud(gem_map *m, const gem_ros_header *h, const gem_ros_part *parts, int nparts, int is_dense, void *out,
+                  long long capacity, long long *bytes_out);
+int gem_ros_octomap(gem_map *m, const gem_ros_header *h, void *out, long long capacity, long long *bytes_out);
+
 /* raw layer access (row-major L*L, float or int32 for the colour ids) for tests and
  * checkpoint/restore (the dead G_get_mapinfo/G_set_mapinfo of gpu.cu:457-475). */
 int gem_get_layer(gem_map *m, int layer, void *host_out);

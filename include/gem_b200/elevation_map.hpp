@@ -19,6 +19,7 @@
 #include <cstdio>
 #include <cstring>
 #include <limits>
+#include <new>
 #include <stdexcept>
 #include <string>
 #include <vector>
@@ -34,6 +35,24 @@ struct PointXYZRGBICT {
     float covariance, intensity, travers;
 };
 static_assert(sizeof(PointXYZRGBICT) == 32, "PCL record layout");
+
+// An allocator of pinned host memory (gem_host_alloc), for buffers the device writes directly, e.g. the rosX messages:
+//     std::vector<uint8_t, gem_b200::PinnedAllocator<uint8_t>> msg;
+template <class T> struct PinnedAllocator {
+    using value_type = T;
+    PinnedAllocator() = default;
+    template <class U> PinnedAllocator(const PinnedAllocator<U> &) {}
+    T *allocate(size_t n)
+    {
+        void *p = nullptr;
+        if (gem_host_alloc(&p, n * sizeof(T)) != GEM_OK) throw std::bad_alloc();
+        return static_cast<T *>(p);
+    }
+    void deallocate(T *p, size_t) { gem_host_free(p); }
+    template <class U> bool operator==(const PinnedAllocator<U> &) const { return true; }
+    template <class U> bool operator!=(const PinnedAllocator<U> &) const { return false; }
+};
+using PinnedBytes = std::vector<uint8_t, PinnedAllocator<uint8_t>>;
 
 // sensor_msgs/PointCloud2's layout without ROS (DESIGN.md f12): add the message's fields in order, then pass layout().
 // From a sensor_msgs::PointCloud2ConstPtr msg:
@@ -541,6 +560,54 @@ class ElevationMap {
             throw std::runtime_error("savePcd: writing " + path + " failed");
         }
     }
+    // The node's map topics as serialised ROS1 messages (DESIGN.md f15, W1-W8), into a pinned byte buffer (PinnedBytes or
+    // any std::vector-like buffer of bytes in pinned or device-visible memory; the library refuses pageable memory with
+    // GEM_ERR_INVALID, so a plain std::vector throws) that a node can publish as it is, e.g. through
+    // topic_tools::ShapeShifter.  Each call resizes `out` to the message and returns when the bytes are there.
+    // rosGridMap: visual_map; rosOrthomosaic: orthomosaic; rosVisualPoints: visualpoints; rosCloud: history_point /
+    // global_point of device or host record parts; rosOctomap: the last colorOctree; rosSubmap: dislam_msgs/SubMap of the
+    // records, the received keyframe cloud's serialised bytes, this map's orthomosaic and the pose (xyz, then xyzw).
+    template <class Buffer> size_t rosGridMap(const gem_ros_header &h, Buffer &out)
+    {
+        return rosInto(out, 0, "gem_ros_grid_map", [&](void *p, long long c, long long *nb) { return gem_ros_grid_map(h_, &h, p, c, nb); });
+    }
+    template <class Buffer> size_t rosOrthomosaic(const gem_ros_header &h, Buffer &out)
+    {
+        return rosInto(out, 0, "gem_ros_orthomosaic", [&](void *p, long long c, long long *nb) { return gem_ros_orthomosaic(h_, &h, p, c, nb); });
+    }
+    template <class Buffer> size_t rosVisualPoints(const gem_ros_header &h, Buffer &out)
+    {
+        return rosInto(out, 0, "gem_ros_visual_points", [&](void *p, long long c, long long *nb) { return gem_ros_visual_points(h_, &h, p, c, nb); });
+    }
+    template <class Buffer> size_t rosCloud(const gem_ros_header &h, const std::vector<gem_ros_part> &parts, Buffer &out, bool isDense = true)
+    {
+        return rosInto(out, 0, "gem_ros_cloud", [&](void *p, long long c, long long *nb) {
+            return gem_ros_cloud(h_, &h, parts.data(), (int)parts.size(), isDense ? 1 : 0, p, c, nb);
+        });
+    }
+    template <class Buffer> size_t rosOctomap(const gem_ros_header &h, Buffer &out)
+    {
+        return rosInto(out, 0, "gem_ros_octomap", [&](void *p, long long c, long long *nb) { return gem_ros_octomap(h_, &h, p, c, nb); });
+    }
+    template <class Buffer>
+    size_t rosSubmap(const gem_ros_header &h, const void *records, size_t n, const void *keyframe, size_t keyframeBytes,
+                     const double pose[7], Buffer &out, const gem_ros_header &imageHeader = gem_ros_header{0, 0, 0, ""},
+                     bool isDense = true)
+    {
+        const gem_ros_part part{records, (long long)n};
+        auto cloud = [&](void *p, long long c, long long *nb) { return gem_ros_cloud(h_, &h, &part, 1, isDense ? 1 : 0, p, c, nb); };
+        auto image = [&](void *p, long long c, long long *nb) { return gem_ros_orthomosaic(h_, &imageHeader, p, c, nb); };
+        long long nc = 0, ni = 0;
+        check(cloud(nullptr, 0, &nc), "gem_ros_cloud");
+        check(image(nullptr, 0, &ni), "gem_ros_orthomosaic");
+        out.resize((size_t)nc + keyframeBytes + (size_t)ni + 7 * sizeof(double));
+        rosInto(out, 0, "gem_ros_cloud", cloud, false);
+        rosInto(out, (size_t)nc + keyframeBytes, "gem_ros_orthomosaic", image, false);
+        sync();
+        if (keyframeBytes) std::memcpy(&out[(size_t)nc], keyframe, keyframeBytes);
+        std::memcpy(&out[out.size() - 7 * sizeof(double)], pose, 7 * sizeof(double));
+        return out.size();
+    }
     // Loop closure (ElevationMapping::updateGlobalMap, ElevationMapping.cpp:773-905), on device-resident submaps of
     // PointXYZRGBICT records: re-pose a submap (:805), and one pass of the pairwise fuse loop (:847-883) -- both clouds
     // come back reduced to one point per cell and compacted, *n_new / *n_old updated.  compat_precedence = true evaluates
@@ -570,6 +637,20 @@ class ElevationMap {
     void sync() { check(gem_sync(h_), "gem_sync"); }
 
   private:
+    // one gem_ros_* call into out at byte `at`: with resize, out becomes the message (size query first) and the call is
+    // waited for; without, out must already hold it
+    template <class Buffer, class Call> size_t rosInto(Buffer &out, size_t at, const char *what, Call call, bool resize = true)
+    {
+        long long bytes = 0;
+        if (resize) {
+            check(call(nullptr, 0, &bytes), what);
+            out.resize((size_t)bytes);
+        }
+        check(call(&out[0] + at, (long long)(out.size() - at), &bytes), what);
+        if ((size_t)bytes > out.size() - at) throw std::runtime_error(std::string(what) + ": the buffer is too small");
+        if (resize) sync();
+        return (size_t)bytes;
+    }
     static int pcdFlags(bool binary, bool rgbUint32) { return (binary ? GEM_PCD_BINARY : 0) | (rgbUint32 ? GEM_PCD_RGB_UINT32 : 0); }
     void check(int rc, const char *what)
     {
