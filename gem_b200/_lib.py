@@ -227,6 +227,15 @@ SYMBOLS = {
     "gem_raytracing_tiled": (C.c_int, [_P, _P]),
     "gem_transform_cloud": (C.c_int, [_P, _P, C.c_int, _FP]),
     "gem_refuse_submaps": (C.c_int, [_P, _P, _IP, _P, _IP, C.c_double, C.c_int, _IP]),
+    "gem_global_map_reset": (C.c_int, [_P]),
+    "gem_global_map_reserve": (C.c_int, [_P, C.c_longlong, C.c_int]),
+    "gem_global_map_push": (C.c_int, [_P, _P, C.c_int, _FP]),
+    "gem_global_map_update": (C.c_int, [_P, _FP, C.c_int, C.c_double, C.c_double, C.c_int, _IP]),
+    "gem_global_map_info": (C.c_int, [_P, _IP, _IP, C.POINTER(C.c_longlong)]),
+    "gem_global_map_submap": (C.c_int, [_P, C.c_int, C.POINTER(_P), _IP]),
+    "gem_global_map_records": (C.c_int, [_P, C.POINTER(_P), C.POINTER(C.c_longlong)]),
+    "gem_global_map_pose": (C.c_int, [_P, C.c_int, _FP, _FP]),
+    "gem_global_map_stream": (_P, [_P]),
     "gem_tiled_attach": (C.c_int, [_P, C.POINTER(GemTiledPeers)]),
     "gem_tiled_step": (C.c_int, [_P, _P, _P, C.c_int, C.POINTER(GemFrame)]),
     "gem_pointcloud2_mapping": (C.c_int, [C.POINTER(GemPointCloud2), C.c_ulonglong, C.POINTER(GemPc2Mapping)]),

@@ -20,6 +20,7 @@ LIB = os.path.join(LIBDIR, "libgem_b200.so")
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",
     "-lineinfo", "-O3", "-fmad=false", "-std=c++17",
+    "-Xcompiler", "-ffp-contract=off",
     "-Xcompiler", "-fPIC", "-shared",
 ]
 

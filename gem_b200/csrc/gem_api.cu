@@ -28,6 +28,7 @@
 #include "gem_inflate.cuh"
 #include "gem_kernels.cuh"
 #include "gem_global.cuh"
+#include "gem_globalmap.h"
 #include "gem_ingest.cuh"
 #include "gem_mls.cuh"
 #include "gem_octree.cuh"
@@ -109,6 +110,21 @@ struct LocalStore { // localMap_ on the device (gem_harvest_to_local_map, gem_lo
     size_t slots = 0;                  // index slots (a power of two >= 2 * cap)
 };
 
+struct GlobalStore { // globalMap_, trajectory_ and localMapLoc_ on the device (gem_global_map_*; DESIGN.md f16)
+    std::mutex mu;                     // the stack's own lock: no call on it takes the handle's mutex except a push, briefly
+    cudaStream_t stream = nullptr;     // the stack's own stream
+    cudaEvent_t ev = nullptr;          // push: the handle's stream -> the stack's stream
+    OctBuf arena[2];                   // arena[cur]: the submaps back to back in push order; the other: the re-pack target
+    int cur = 0;
+    long long cap = 0;                 // records each arena buffer holds
+    OctBuf meta;                       // update: counts, old and new offsets, fused count, the re-pose table
+    int meta_submaps = 0;              // submaps `meta` is laid out for
+    OctBuf pair;                       // update: one pair's hash tables, keep flags, scan counts and compaction output
+    std::vector<int> cnt, off{0};      // host mirror: per submap its count, and its offset (one entry more)
+    std::vector<float> poses{1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1}; // trajectory_: 16 floats per keyframe
+    std::vector<float> centres{0.0f, 0.0f};                                  // localMapLoc_: x, y per keyframe
+};
+
 struct FrameGraph { // {long lists || the other lists of the previous call || bin of this call} as one three-node CUDA graph
     cudaGraph_t graph = nullptr;
     cudaGraphExec_t exec = nullptr;
@@ -170,6 +186,8 @@ struct gem_map {
     OctBuf ros_framing;            // gem_ros_*: the framing bytes of the call, staged for k_ros_framing
     OctBuf ros_stage;              // gem_ros_* map messages for pinned outputs, written here and copied over in one DMA
     InflScratch infl;              // gem_costmap_inflate
+    OctBuf refuse;                 // gem_refuse_submaps: one pair's scratch (pair_layout)
+    GlobalStore gmap;              // gem_global_map_*
     unsigned long long *d_stamps = nullptr; // gem_debug_stamps
     int *d_raylist = nullptr;      // ray clean-up: cells that cast a ray + their count
     uint32_t *d_bitmap = nullptr;  // ray clean-up: validity bitmap of the lowest layer (own tile / map-wide)
@@ -883,8 +901,11 @@ int gem_destroy(gem_map *m)
                           &m->mls.ooff, &m->mls.longs, &m->mls.lkeys, &m->mls.temp, &m->mls.acc, &m->pc2_raw[0],
                           &m->pc2_raw[1], &m->pc2_raw[2], &m->pc2_img[0], &m->pc2_img[1], &m->pc2_img[2], &m->pc2_bgr,
                           &m->pcd.bytes, &m->pcd.ends, &m->pcd.temp, &m->infl.key, &m->infl.pops, &m->infl.tab,
-                          &m->infl.gstart, &m->infl.blk, &m->ros_framing, &m->ros_stage})
+                          &m->infl.gstart, &m->infl.blk, &m->ros_framing, &m->ros_stage, &m->refuse, &m->gmap.arena[0],
+                          &m->gmap.arena[1], &m->gmap.meta, &m->gmap.pair})
             if (b->p) cudaFree(b->p);
+        if (m->gmap.stream) { cudaStreamSynchronize(m->gmap.stream); cudaStreamDestroy(m->gmap.stream); }
+        if (m->gmap.ev) cudaEventDestroy(m->gmap.ev);
         if (m->h_ctr) cudaFreeHost(m->h_ctr);
         if (m->h_ctr_ring) cudaFreeHost(m->h_ctr_ring);
         if (m->h_frames) cudaFreeHost(m->h_frames);
@@ -2709,6 +2730,80 @@ int gem_transform_cloud(gem_map *m, void *points32, int n, const float T[16])
     return GEM_OK;
 }
 
+// One pair's scratch, laid out in one buffer for clouds of at most nn and no records: two hash tables (keys + first index),
+// the keep flags, the scan counts of the compaction, its output and four counters.
+struct PairScratch {
+    unsigned long long *kn, *ko;
+    int *fn, *fo, *cnt, *ctr;
+    unsigned char *keepn, *keepo;
+    SubPoint *out;
+    size_t cn, co, nchunk;
+};
+static size_t hash_slots(int n) { size_t p = 64; while (p < 2 * (size_t)n + 2) p <<= 1; return p; }
+static PairScratch pair_layout(void *base, int nn, int no, size_t *bytes = nullptr)
+{
+    PairScratch s;
+    const int big = std::max(nn, no);
+    s.cn = hash_slots(nn);
+    s.co = hash_slots(no);
+    s.nchunk = ((size_t)big + 31) / 32 + 1;
+    const size_t nseg = s.nchunk / SCAN_SEG + 1;
+    char *p = (char *)base;
+    size_t at = 0;
+    auto take = [&](size_t n) { char *q = p + at; at = (at + n + 31) & ~(size_t)31; return q; };
+    s.out = (SubPoint *)take((size_t)big * sizeof(SubPoint));
+    s.kn = (unsigned long long *)take((s.cn + s.co) * 8);
+    s.ko = s.kn + s.cn;
+    s.fn = (int *)take((s.cn + s.co) * 4);
+    s.fo = s.fn + s.cn;
+    s.cnt = (int *)take((s.nchunk + nseg) * 4);
+    s.ctr = (int *)take(16);
+    s.keepn = (unsigned char *)take((size_t)nn + no);
+    s.keepo = s.keepn + nn;
+    if (bytes) *bytes = at;
+    return s;
+}
+static size_t pair_bytes(int nn, int no)
+{
+    size_t b = 0;
+    pair_layout(nullptr, nn, no, &b);
+    return b;
+}
+
+// compact p[0, *n) by its keep flags, in order and in place (through s.out); ub >= *n is known on the host
+static cudaError_t enqueue_compact(cudaStream_t st, const PairScratch &s, SubPoint *p, unsigned char *keep, int ub, int *n, int &launches)
+{
+    if (ub == 0) return cudaSuccess;
+    const int nchunk = (ub + 31) / 32, nseg = (nchunk + SCAN_SEG - 1) / SCAN_SEG, nb = (ub + TAKE_BLOCK - 1) / TAKE_BLOCK;
+    int *segtot = s.cnt + s.nchunk;
+    k_keep_count<<<nb, TAKE_BLOCK, 0, st>>>(keep, n, ub, s.cnt);
+    k_compact_scan<<<nseg, SCAN_SEG, 0, st>>>(s.cnt, nchunk, segtot);
+    k_keep_write<<<nb, TAKE_BLOCK, 0, st>>>(p, keep, ub, s.cnt, segtot, nseg, SCAN_SEG, s.out, n);
+    launches += 3;
+    return cudaMemcpyAsync(p, s.out, (size_t)ub * sizeof(SubPoint), cudaMemcpyDeviceToDevice, st);
+}
+
+// One pass of :847-883 for the pair (new = pn, old = po), enqueued on `st` with no allocation and no host synchronisation:
+// the counts *nn / *no stay in device memory and come back updated, ubn / ubo are host-known upper bounds on them (the
+// tables, flags and grids are sized from those), fused cells are added to *fused.  s = pair_layout for (ubn, ubo) or more.
+static cudaError_t enqueue_pair(cudaStream_t st, const PairScratch &s, SubPoint *pn, int ubn, int *nn, SubPoint *po, int ubo, int *no,
+                                double res, int compat, int *fused, int &launches)
+{
+    cudaError_t e = cudaMemsetAsync(s.kn, 0xff, (s.cn + s.co) * 8, st);
+    if (e == cudaSuccess) e = cudaMemsetAsync(s.fn, 0x7f, (s.cn + s.co) * 4, st);
+    if (e != cudaSuccess) return e;
+    const unsigned mn = (unsigned)(s.cn - 1), mo = (unsigned)(s.co - 1);
+    if (ubn) k_hash_insert<<<blocks_for((size_t)ubn, 256, 1 << 30), 256, 0, st>>>(pn, nn, res, s.kn, s.fn, mn);
+    if (ubo) k_hash_insert<<<blocks_for((size_t)ubo, 256, 1 << 30), 256, 0, st>>>(po, no, res, s.ko, s.fo, mo);
+    if (ubo) k_refuse_keep<<<blocks_for((size_t)ubo, 256, 1 << 30), 256, 0, st>>>(po, no, res, s.ko, s.fo, mo, s.keepo);
+    if (ubn) k_refuse_pair<<<blocks_for((size_t)ubn, 256, 1 << 30), 256, 0, st>>>(pn, nn, po, res, s.kn, s.fn, mn, s.ko, s.fo, mo, s.keepn, compat, fused);
+    launches += (ubn ? 2 : 0) + (ubo ? 2 : 0);
+    if ((e = cudaGetLastError()) != cudaSuccess) return e;
+    if ((e = enqueue_compact(st, s, pn, s.keepn, ubn, nn, launches)) != cudaSuccess) return e;
+    if ((e = enqueue_compact(st, s, po, s.keepo, ubo, no, launches)) != cudaSuccess) return e;
+    return cudaGetLastError();
+}
+
 int gem_refuse_submaps(gem_map *m, void *new_points32, int *n_new, void *old_points32, int *n_old, double resolution, int compat,
                        int *fused_out)
 {
@@ -2717,41 +2812,269 @@ int gem_refuse_submaps(gem_map *m, void *new_points32, int *n_new, void *old_poi
     Lock lk(m->mu);
     SetDev sd(m->dev);
     const int nn = *n_new, no = *n_old;
-    auto pow2 = [](size_t v) { size_t p = 64; while (p < v) p <<= 1; return p; };
-    const size_t cn = pow2(2 * (size_t)nn + 2), co = pow2(2 * (size_t)no + 2);
-    // one scratch block: two hash tables (keys + first index), keep flags, compaction outputs, counters
-    const size_t bytes = (cn + co) * (8 + 4) + (size_t)nn + no + 64 + ((size_t)nn + no) * sizeof(SubPoint) + 64;
-    char *d = nullptr;
-    GEM_CUDA(m, cudaMalloc((void **)&d, bytes));
-    unsigned long long *kn = (unsigned long long *)d, *ko = kn + cn;
-    int *fn = (int *)(ko + co), *fo = fn + cn;
-    int *cnts = fo + co; // [0] fused, [1] kept new, [2] kept old
-    SubPoint *outn = (SubPoint *)(((uintptr_t)(cnts + 4) + 31) & ~(uintptr_t)31), *outo = outn + nn;
-    unsigned char *keepn = (unsigned char *)(outo + no), *keepo = keepn + nn;
-    auto done = [&](int rc) { cudaFree(d); return rc; };
-    cudaError_t e = cudaMemsetAsync(kn, 0xff, (cn + co) * 8, m->stream);
-    if (e == cudaSuccess) e = cudaMemsetAsync(fn, 0x7f, (cn + co) * 4, m->stream);
-    if (e == cudaSuccess) e = cudaMemsetAsync(cnts, 0, 16, m->stream);
-    if (e != cudaSuccess) return done(fail(m, GEM_ERR_CUDA, cudaGetErrorString(e)));
-    SubPoint *pn = (SubPoint *)new_points32, *po = (SubPoint *)old_points32;
-    if (nn) GEM_LAUNCH(m, GEM_PROF_OTHER, k_hash_insert<<<blocks_for((size_t)nn, 256, 1 << 30), 256, 0, m->stream>>>(pn, nn, resolution, kn, fn, (unsigned)(cn - 1)));
-    if (no) GEM_LAUNCH(m, GEM_PROF_OTHER, k_hash_insert<<<blocks_for((size_t)no, 256, 1 << 30), 256, 0, m->stream>>>(po, no, resolution, ko, fo, (unsigned)(co - 1)));
-    if (no) GEM_LAUNCH(m, GEM_PROF_OTHER, k_refuse_keep<<<blocks_for((size_t)no, 256, 1 << 30), 256, 0, m->stream>>>(po, no, resolution, ko, fo, (unsigned)(co - 1), keepo));
-    if (nn) GEM_LAUNCH(m, GEM_PROF_OTHER, k_refuse_pair<<<blocks_for((size_t)nn, 256, 1 << 30), 256, 0, m->stream>>>(pn, nn, po, resolution, kn, fn, (unsigned)(cn - 1), ko, fo, (unsigned)(co - 1), keepn, compat, cnts));
-    GEM_LAUNCH(m, GEM_PROF_OTHER, k_compact_points<<<1, 1024, 0, m->stream>>>(pn, keepn, nn, outn, cnts + 1));
-    GEM_LAUNCH(m, GEM_PROF_OTHER, k_compact_points<<<1, 1024, 0, m->stream>>>(po, keepo, no, outo, cnts + 2));
-    int h[4] = {0, 0, 0, 0};
-    e = cudaGetLastError();
-    if (e == cudaSuccess) e = cudaMemcpyAsync(h, cnts, 16, cudaMemcpyDeviceToHost, m->stream);
+    int rc = scratch_grow(m, m->refuse, pair_bytes(nn, no), "gem_refuse_submaps");
+    if (rc) return rc;
+    const PairScratch s = pair_layout(m->refuse.p, nn, no);
+    int h[4] = {0, nn, no, 0}; // fused, n_new, n_old
+    int launches = 0;
+    cudaError_t e = cudaMemcpyAsync(s.ctr, h, 16, cudaMemcpyHostToDevice, m->stream);
+    if (e == cudaSuccess)
+        e = enqueue_pair(m->stream, s, (SubPoint *)new_points32, nn, s.ctr + 1, (SubPoint *)old_points32, no, s.ctr + 2, resolution, compat,
+                         s.ctr, launches);
+    m->launches += launches;
+    if (e == cudaSuccess) e = cudaMemcpyAsync(h, s.ctr, 16, cudaMemcpyDeviceToHost, m->stream);
     if (e == cudaSuccess) e = cudaStreamSynchronize(m->stream);
-    if (e == cudaSuccess && h[1] > 0) e = cudaMemcpyAsync(pn, outn, (size_t)h[1] * sizeof(SubPoint), cudaMemcpyDeviceToDevice, m->stream);
-    if (e == cudaSuccess && h[2] > 0) e = cudaMemcpyAsync(po, outo, (size_t)h[2] * sizeof(SubPoint), cudaMemcpyDeviceToDevice, m->stream);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(m->stream);
-    if (e != cudaSuccess) return done(fail(m, GEM_ERR_CUDA, std::string("gem_refuse_submaps: ") + cudaGetErrorString(e)));
+    if (e != cudaSuccess) return fail(m, GEM_ERR_CUDA, std::string("gem_refuse_submaps: ") + cudaGetErrorString(e));
     *n_new = h[1];
     *n_old = h[2];
     if (fused_out) *fused_out = h[0];
-    return done(GEM_OK);
+    return GEM_OK;
+}
+
+// ---- the global map: keyframe submap stack, poses and updateGlobalMap (DESIGN.md f16) ----------------------------------
+using GLock = std::lock_guard<std::mutex>;
+
+// the stack's stream and event, created on first use (caller holds g.mu)
+static int gmap_ready(gem_map *m)
+{
+    GlobalStore &g = m->gmap;
+    if (!g.stream) GEM_CUDA(m, cudaStreamCreateWithFlags(&g.stream, cudaStreamNonBlocking));
+    if (!g.ev) GEM_CUDA(m, cudaEventCreateWithFlags(&g.ev, cudaEventDisableTiming));
+    return GEM_OK;
+}
+// a scratch buffer of the stack: like scratch_grow, but drained on the stack's stream
+static int gmap_grow(gem_map *m, OctBuf &b, size_t bytes, const char *what)
+{
+    if (b.cap >= bytes) return GEM_OK;
+    bytes = std::max(std::max(bytes, 2 * b.cap), (size_t)4096);
+    void *q = nullptr;
+    const cudaError_t e = cudaMalloc(&q, bytes);
+    if (e != cudaSuccess) { cudaGetLastError(); return fail(m, GEM_ERR_NOMEM, std::string(what) + ": cudaMalloc: " + cudaGetErrorString(e)); }
+    if (b.p) { cudaStreamSynchronize(m->gmap.stream); cudaFree(b.p); }
+    b.p = q;
+    b.cap = bytes;
+    return GEM_OK;
+}
+// room for `need` records in both arena buffers (capacity doubles from 1024).  Both are allocated before anything is
+// released, so a failed growth leaves the stack as it was.
+static int gmap_reserve_records(gem_map *m, long long need)
+{
+    GlobalStore &g = m->gmap;
+    if (need <= g.cap) return GEM_OK;
+    long long cap = g.cap > 0 ? g.cap : 1024;
+    while (cap < need) cap *= 2;
+    if (cap > (1 << 30)) return fail(m, GEM_ERR_NOMEM, "global map: more than 2^30 records");
+    void *q[2] = {nullptr, nullptr};
+    for (int b = 0; b < 2; b++) {
+        const cudaError_t e = cudaMalloc(&q[b], (size_t)cap * sizeof(SubPoint));
+        if (e != cudaSuccess) {
+            cudaGetLastError();
+            if (q[0]) cudaFree(q[0]);
+            return fail(m, GEM_ERR_NOMEM, std::string("global map: cudaMalloc: ") + cudaGetErrorString(e));
+        }
+    }
+    const int total = g.off.back();
+    cudaError_t e = total ? cudaMemcpyAsync(q[0], g.arena[g.cur].p, (size_t)total * sizeof(SubPoint), cudaMemcpyDeviceToDevice, g.stream)
+                          : cudaSuccess;
+    if (e == cudaSuccess) e = cudaStreamSynchronize(g.stream);
+    if (e != cudaSuccess) {
+        cudaFree(q[0]);
+        cudaFree(q[1]);
+        return fail(m, GEM_ERR_CUDA, std::string("global map: growth: ") + cudaGetErrorString(e));
+    }
+    for (int b = 0; b < 2; b++) {
+        if (g.arena[b].p) cudaFree(g.arena[b].p);
+        g.arena[b].p = q[b];
+        g.arena[b].cap = (size_t)cap * sizeof(SubPoint);
+    }
+    g.cur = 0;
+    g.cap = cap;
+    return GEM_OK;
+}
+// the update's device bookkeeping for K submaps: counts [K], old offsets [K + 1], new offsets [K + 1], counters [4],
+// then the re-pose table Rigid [K]
+static size_t gmap_meta_ints(int K) { return ((3 * (size_t)K + 6) + 3) & ~(size_t)3; }
+static int gmap_reserve_meta(gem_map *m, int K)
+{
+    GlobalStore &g = m->gmap;
+    if (K <= g.meta_submaps) return GEM_OK;
+    int cap = std::max(g.meta_submaps * 2, 64);
+    while (cap < K) cap *= 2;
+    const int rc = gmap_grow(m, g.meta, gmap_meta_ints(cap) * 4 + (size_t)cap * sizeof(Rigid), "global map");
+    if (rc == GEM_OK) g.meta_submaps = cap;
+    return rc;
+}
+
+int gem_global_map_reset(gem_map *m)
+{
+    if (!m) return GEM_ERR_INVALID;
+    GlobalStore &g = m->gmap;
+    GLock lk(g.mu);
+    g.cnt.clear();
+    g.off.assign(1, 0);
+    g.poses.assign({1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1});
+    g.centres.assign({0.0f, 0.0f});
+    return GEM_OK;
+}
+
+int gem_global_map_reserve(gem_map *m, long long records, int submaps)
+{
+    if (!m || records < 0 || submaps < 0) return fail(m, GEM_ERR_INVALID, "gem_global_map_reserve: bad argument");
+    if (records > (1 << 30)) return fail(m, GEM_ERR_NOMEM, "gem_global_map_reserve: more than 2^30 records");
+    GlobalStore &g = m->gmap;
+    GLock lk(g.mu);
+    SetDev sd(m->dev);
+    int rc;
+    if ((rc = gmap_ready(m)) || (rc = gmap_reserve_records(m, records)) || (rc = gmap_reserve_meta(m, submaps))) return rc;
+    // one pair of the largest submaps the arena can hold
+    const int big = (int)std::min<long long>(records, g.cap);
+    return gmap_grow(m, g.pair, pair_bytes(big, big), "gem_global_map_reserve");
+}
+
+int gem_global_map_push(gem_map *m, const void *records_device, int n, const float pose[16])
+{
+    if (!m || n < 0 || !pose || (n > 0 && !records_device)) return fail(m, GEM_ERR_INVALID, "gem_global_map_push: bad argument");
+    SetDev sd(m->dev);
+    if (n > 0) {
+        cudaPointerAttributes a{};
+        if (cudaPointerGetAttributes(&a, records_device) != cudaSuccess || (a.type != cudaMemoryTypeDevice && a.type != cudaMemoryTypeManaged)) {
+            cudaGetLastError();
+            return fail(m, GEM_ERR_INVALID, "gem_global_map_push: the records are not in device memory");
+        }
+    }
+    GlobalStore &g = m->gmap;
+    GLock lk(g.mu);
+    int rc;
+    const long long total = g.off.back();
+    if ((rc = gmap_ready(m)) || (rc = gmap_reserve_records(m, total + n))) return rc;
+    { // a cut_submap issued just before on the handle's stream is complete before the copy reads it
+        Lock hl(m->mu);
+        GEM_CUDA(m, cudaEventRecord(g.ev, m->stream));
+    }
+    GEM_CUDA(m, cudaStreamWaitEvent(g.stream, g.ev, 0));
+    if (n) GEM_CUDA(m, cudaMemcpyAsync(g.arena[g.cur].as<SubPoint>() + total, records_device, (size_t)n * sizeof(SubPoint),
+                                       cudaMemcpyDeviceToDevice, g.stream));
+    GEM_CUDA(m, cudaStreamSynchronize(g.stream));
+    // :636-642, then :660: the keyframe (pose, centre = its translation x, y) first, then its submap
+    g.poses.insert(g.poses.end(), pose, pose + 16);
+    g.centres.push_back(pose[3]);
+    g.centres.push_back(pose[7]);
+    g.cnt.push_back(n);
+    g.off.push_back((int)(total + n));
+    return GEM_OK;
+}
+
+int gem_global_map_update(gem_map *m, const float *opt_poses, int k, double resolution, double radius, int compat, int *fused_out)
+{
+    if (!m || k < 0 || (k > 0 && !opt_poses) || !(resolution > 0.0) || !std::isfinite(resolution) || !(radius >= 0.0))
+        return fail(m, GEM_ERR_INVALID, "gem_global_map_update: bad argument");
+    GlobalStore &g = m->gmap;
+    GLock lk(g.mu);
+    SetDev sd(m->dev);
+    int rc;
+    if ((rc = gmap_ready(m))) return rc;
+    const int K = (int)g.cnt.size(), Kp = std::min(k, K); // :784-786
+    // :791-809 on the host: the re-pose of submaps 1 .. K'-1 (submap 0 keeps its pose)
+    std::vector<Rigid> T((size_t)std::max(Kp, 1));
+    for (int i = 1; i < Kp; i++) {
+        float t[16];
+        gem_gmap::relative_pose(opt_poses + 16 * (size_t)i, &g.poses[16 * (size_t)i], t);
+        for (int q = 0; q < 12; q++) T[i].t[q] = t[q];
+    }
+    // :812-891's pairs from the pushed centres (localMapLoc_ is never updated)
+    std::vector<std::pair<int, int>> pairs;
+    gem_gmap::pair_schedule(g.centres.data(), Kp, radius, pairs);
+    int big = 0;
+    for (int i = 0; i < Kp; i++) big = std::max(big, g.cnt[i]);
+    if ((rc = gmap_reserve_meta(m, std::max(K, 1))) || (rc = gmap_grow(m, g.pair, pair_bytes(big, big), "gem_global_map_update"))) return rc;
+    int *d_cnt = g.meta.as<int>(), *d_off = d_cnt + K, *d_off_new = d_off + K + 1, *d_ctr = d_off_new + K + 1;
+    Rigid *d_T = (Rigid *)(g.meta.as<int>() + gmap_meta_ints(g.meta_submaps));
+    std::vector<int> h((size_t)3 * K + 6, 0);
+    std::copy(g.cnt.begin(), g.cnt.end(), h.begin());
+    std::copy(g.off.begin(), g.off.end(), h.begin() + K);
+    GEM_CUDA(m, cudaMemcpyAsync(d_cnt, h.data(), h.size() * 4, cudaMemcpyHostToDevice, g.stream));
+    SubPoint *arena = g.arena[g.cur].as<SubPoint>();
+    if (Kp > 1) {
+        GEM_CUDA(m, cudaMemcpyAsync(d_T, T.data(), (size_t)Kp * sizeof(Rigid), cudaMemcpyHostToDevice, g.stream));
+        const int n = g.off[Kp] - g.off[1];
+        if (n > 0) k_transform_segments<<<blocks_for((size_t)n, 256, 1 << 30), 256, 0, g.stream>>>(arena, d_off + 1, d_T + 1, Kp - 1);
+        GEM_CUDA(m, cudaGetLastError());
+    }
+    int launches = 0;
+    for (const auto &pr : pairs) { // each pair's scratch laid out for its own two upper bounds (within pair_bytes(big, big))
+        const int j = pr.first, i = pr.second;
+        const cudaError_t e = enqueue_pair(g.stream, pair_layout(g.pair.p, g.cnt[j], g.cnt[i]), arena + g.off[j], g.cnt[j], d_cnt + j, arena + g.off[i], g.cnt[i], d_cnt + i,
+                                           resolution, compat, d_ctr, launches);
+        if (e != cudaSuccess) return fail(m, GEM_ERR_CUDA, std::string("gem_global_map_update: ") + cudaGetErrorString(e));
+    }
+    if (!pairs.empty()) { // the stack back to back again, into the other arena buffer
+        k_pack_offsets<<<1, 1, 0, g.stream>>>(d_cnt, K, d_off_new);
+        k_pack_segments<<<blocks_for((size_t)g.off[K], 256, 1 << 30), 256, 0, g.stream>>>(arena, g.arena[g.cur ^ 1].as<SubPoint>(), d_off,
+                                                                                          d_off_new, d_cnt, K);
+        GEM_CUDA(m, cudaGetLastError());
+    }
+    GEM_CUDA(m, cudaMemcpyAsync(h.data(), d_cnt, h.size() * 4, cudaMemcpyDeviceToHost, g.stream));
+    GEM_CUDA(m, cudaStreamSynchronize(g.stream));
+    if (!pairs.empty()) g.cur ^= 1;
+    for (int i = 0; i < K; i++) {
+        g.cnt[i] = h[i];
+        g.off[i + 1] = g.off[i] + h[i];
+    }
+    for (int i = 1; i < Kp; i++) std::copy(opt_poses + 16 * (size_t)i, opt_poses + 16 * (size_t)(i + 1), &g.poses[16 * (size_t)i]);
+    if (fused_out) *fused_out = h[3 * (size_t)K + 2];
+    return GEM_OK;
+}
+
+int gem_global_map_info(gem_map *m, int *submaps, int *keyframes, long long *records)
+{
+    if (!m) return GEM_ERR_INVALID;
+    GlobalStore &g = m->gmap;
+    GLock lk(g.mu);
+    if (submaps) *submaps = (int)g.cnt.size();
+    if (keyframes) *keyframes = (int)(g.centres.size() / 2);
+    if (records) *records = g.off.back();
+    return GEM_OK;
+}
+
+int gem_global_map_submap(gem_map *m, int i, void **records_out, int *count_out)
+{
+    if (!m || !records_out || !count_out) return fail(m, GEM_ERR_INVALID, "gem_global_map_submap: bad argument");
+    GlobalStore &g = m->gmap;
+    GLock lk(g.mu);
+    if (i < 0 || i >= (int)g.cnt.size()) return fail(m, GEM_ERR_INVALID, "gem_global_map_submap: no such submap");
+    *records_out = g.arena[g.cur].as<SubPoint>() + g.off[i];
+    *count_out = g.cnt[i];
+    return GEM_OK;
+}
+
+int gem_global_map_records(gem_map *m, void **records_out, long long *count_out)
+{
+    if (!m || !records_out || !count_out) return fail(m, GEM_ERR_INVALID, "gem_global_map_records: bad argument");
+    GlobalStore &g = m->gmap;
+    GLock lk(g.mu);
+    *records_out = g.arena[g.cur].p;
+    *count_out = g.off.back();
+    return GEM_OK;
+}
+
+int gem_global_map_pose(gem_map *m, int i, float pose_out[16], float centre_out[2])
+{
+    if (!m) return GEM_ERR_INVALID;
+    GlobalStore &g = m->gmap;
+    GLock lk(g.mu);
+    if (i < 0 || i >= (int)(g.centres.size() / 2)) return fail(m, GEM_ERR_INVALID, "gem_global_map_pose: no such keyframe");
+    if (pose_out) std::copy(&g.poses[16 * (size_t)i], &g.poses[16 * (size_t)i] + 16, pose_out);
+    if (centre_out) { centre_out[0] = g.centres[2 * (size_t)i]; centre_out[1] = g.centres[2 * (size_t)i + 1]; }
+    return GEM_OK;
+}
+
+void *gem_global_map_stream(gem_map *m)
+{
+    if (!m) return nullptr;
+    GlobalStore &g = m->gmap;
+    GLock lk(g.mu);
+    SetDev sd(m->dev);
+    return gmap_ready(m) == GEM_OK ? (void *)g.stream : nullptr;
 }
 
 // ---- tiled maps, peer path (gem_route.cuh "Peer path, round 2") --------------------------------------------------------

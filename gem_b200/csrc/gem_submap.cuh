@@ -20,14 +20,31 @@ static_assert(sizeof(SubPoint) == 32, "PointXYZRGBICT is 32 bytes");
 // pcl::transformPointCloud (ElevationMapping.cpp:805): x' = t00 x + t01 y + t02 z + t03, left to right in float (the
 // scalar code of PCL <= 1.9; PCL is an unpinned dependency of the reference).  T: row-major 4 x 4.
 struct Rigid { float t[12]; };
+__device__ __forceinline__ void rigid_apply(SubPoint &q, const Rigid &T)
+{
+    const float x = q.x, y = q.y, z = q.z;
+    q.x = ((T.t[0] * x + T.t[1] * y) + T.t[2] * z) + T.t[3];
+    q.y = ((T.t[4] * x + T.t[5] * y) + T.t[6] * z) + T.t[7];
+    q.z = ((T.t[8] * x + T.t[9] * y) + T.t[10] * z) + T.t[11];
+}
 __global__ void __launch_bounds__(256) k_transform_cloud(SubPoint *p, int n, const __grid_constant__ Rigid T)
 {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
-    const float x = p[i].x, y = p[i].y, z = p[i].z;
-    p[i].x = ((T.t[0] * x + T.t[1] * y) + T.t[2] * z) + T.t[3];
-    p[i].y = ((T.t[4] * x + T.t[5] * y) + T.t[6] * z) + T.t[7];
-    p[i].z = ((T.t[8] * x + T.t[9] * y) + T.t[10] * z) + T.t[11];
+    rigid_apply(p[i], T);
+}
+// the same per point over the records [off[0], off[nseg]) of a packed stack: record r of segment s (off[s] <= r <
+// off[s + 1]) is moved by T[s].  off and T are in device memory, nseg + 1 and nseg entries.
+__global__ void __launch_bounds__(256) k_transform_segments(SubPoint *p, const int *off, const Rigid *T, int nseg)
+{
+    const int r = off[0] + (int)(blockIdx.x * blockDim.x + threadIdx.x);
+    if (r >= off[nseg]) return;
+    int lo = 0, hi = nseg - 1; // the last s with off[s] <= r
+    while (lo < hi) {
+        const int mid = (lo + hi + 1) >> 1;
+        if (off[mid] <= r) lo = mid; else hi = mid - 1;
+    }
+    rigid_apply(p[r], T[lo]);
 }
 
 // pointCloudtoHash (ElevationMapping.cpp:1180-1192): the cell of a point is the float pair
@@ -49,10 +66,11 @@ __device__ __forceinline__ unsigned hash_slot(unsigned long long k, unsigned mas
     return (unsigned)k & mask;
 }
 // umap::insert keeps the FIRST point of a cell: the table stores, per cell, the smallest point index
-__global__ void __launch_bounds__(256) k_hash_insert(const SubPoint *p, int n, double res, unsigned long long *keys, int *first, unsigned mask)
+// The count of every cloud is read from device memory (n): a chain of pairs runs without host round trips.
+__global__ void __launch_bounds__(256) k_hash_insert(const SubPoint *p, const int *n, double res, unsigned long long *keys, int *first, unsigned mask)
 {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
+    if (i >= *n) return;
     float rx, ry;
     const unsigned long long k = cell_key(p[i].x, p[i].y, res, rx, ry);
     if (k == HASH_EMPTY || rx != rx || ry != ry) return; // a NaN position equals nothing, itself included: such points never meet another
@@ -81,10 +99,10 @@ __device__ __forceinline__ int hash_find(const unsigned long long *keys, const i
 // of its cell, and its centre rounds (a tie, to even) to 2^(m+23), which lies in the cell below.  So the old side reads
 // only unmodified positions.
 __global__ void __launch_bounds__(256)
-k_refuse_keep(SubPoint *po, int no, double res, const unsigned long long *ko, const int *fo, unsigned mo, unsigned char *keep_o)
+k_refuse_keep(SubPoint *po, const int *no, double res, const unsigned long long *ko, const int *fo, unsigned mo, unsigned char *keep_o)
 {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= no) return;
+    if (i >= *no) return;
     float rx, ry;
     const unsigned long long k = cell_key(po[i].x, po[i].y, res, rx, ry);
     const bool nan = rx != rx || ry != ry;
@@ -100,11 +118,11 @@ k_refuse_keep(SubPoint *po, int no, double res, const unsigned long long *ko, co
 // compat != 0: the fused values as the reference's expression evaluates (C operator precedence, :862-863);
 // compat == 0: the weighting the expression was written for.
 __global__ void __launch_bounds__(256)
-k_refuse_pair(SubPoint *pn, int nn, SubPoint *po, double res, const unsigned long long *kn, const int *fn, unsigned mn,
+k_refuse_pair(SubPoint *pn, const int *nn, SubPoint *po, double res, const unsigned long long *kn, const int *fn, unsigned mn,
               const unsigned long long *ko, const int *fo, unsigned mo, unsigned char *keep_n, int compat, int *count)
 {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= nn) return;
+    if (i >= *nn) return;
     float rx, ry;
     const unsigned long long k = cell_key(pn[i].x, pn[i].y, res, rx, ry);
     const bool nan = rx != rx || ry != ry;
@@ -195,29 +213,63 @@ __global__ void __launch_bounds__(TAKE_BLOCK) k_local_write(const float4 *log, i
     }
 }
 
-// order-preserving compaction of the kept points (one block; a loop-closure event is rare and a submap has < 1e6 points)
-__global__ void __launch_bounds__(1024) k_compact_points(const SubPoint *in, const unsigned char *keep, int n, SubPoint *out, int *n_out)
+// Order-preserving compaction of a re-fused cloud, with its count in device memory and a host-known upper bound ub on it
+// (the count before the pair: a re-fusion only shrinks a cloud).  Pass 1 counts the kept records per 32 (and clears the
+// flags in [*n, ub), so pass 2 needs no count), k_compact_scan scans those counts over many blocks, pass 2 writes every
+// kept record to its rank and the new count to *n.
+__global__ void __launch_bounds__(TAKE_BLOCK) k_keep_count(unsigned char *keep, const int *n, int ub, int *cnt)
 {
-    __shared__ int s_w[32];
-    __shared__ int s_carry;
-    if (threadIdx.x == 0) s_carry = 0;
-    __syncthreads();
-    const unsigned lane = threadIdx.x & 31u;
-    const int w = threadIdx.x >> 5;
-    for (int base = 0; base < n; base += 1024) {
-        const int i = base + threadIdx.x;
-        const int f = (i < n && keep[i]) ? 1 : 0;
-        const unsigned b = __ballot_sync(0xffffffffu, f);
-        if (lane == 0u) s_w[w] = __popc(b);
-        __syncthreads();
-        int before = s_carry;
-        for (int q = 0; q < w; q++) before += s_w[q];
-        if (f) out[before + __popc(b & ((1u << lane) - 1u))] = in[i];
-        __syncthreads();
-        if (threadIdx.x == 0) { int t = 0; for (int q = 0; q < 32; q++) t += s_w[q]; s_carry += t; }
-        __syncthreads();
+    const int i = blockIdx.x * TAKE_BLOCK + threadIdx.x;
+    bool k = false;
+    if (i < ub) {
+        if (i < *n) k = keep[i] != 0; else keep[i] = 0;
     }
-    if (threadIdx.x == 0) *n_out = s_carry;
+    const unsigned b = __ballot_sync(0xffffffffu, k);
+    if ((threadIdx.x & 31u) == 0u && i < ub) cnt[i >> 5] = __popc(b);
+}
+__global__ void __launch_bounds__(TAKE_BLOCK) k_keep_write(const SubPoint *in, const unsigned char *keep, int ub, const int *ofs,
+                                                           const int *segtot, int nseg, int seg_size, SubPoint *out, int *n)
+{
+    const int i = blockIdx.x * TAKE_BLOCK + threadIdx.x;
+    const unsigned lane = threadIdx.x & 31u;
+    const bool k = i < ub && keep[i] != 0;
+    const unsigned b = __ballot_sync(0xffffffffu, k);
+    const int chunk = i >> 5, seg = chunk / seg_size;
+    int pre = 0;
+    for (int q = (int)lane; q < seg; q += 32) pre += segtot[q];
+#pragma unroll
+    for (int d = 16; d > 0; d >>= 1) pre += __shfl_xor_sync(0xffffffffu, pre, d);
+    if (k) out[pre + ofs[chunk] + __popc(b & ((1u << lane) - 1u))] = in[i];
+    if (i == 0) {
+        int t = 0;
+        for (int q = 0; q < nseg; q++) t += segtot[q];
+        *n = t;
+    }
+}
+
+// ---- the global map's submap stack (DESIGN.md f16) ----------------------------------------------------------------------
+// Re-pack after an update: off_new[s] = exclusive prefix of the submaps' device counts (one thread: the stack holds
+// hundreds of submaps, not millions), off_new[nseg] = the total
+__global__ void k_pack_offsets(const int *cnt, int nseg, int *off_new)
+{
+    int t = 0;
+    for (int s = 0; s < nseg; s++) { off_new[s] = t; t += cnt[s]; }
+    off_new[nseg] = t;
+}
+// record r of segment s (off_old[s] <= r < off_old[s + 1]) goes to off_new[s] + (r - off_old[s]) if it is among the
+// segment's first cnt[s]; src and dst are different buffers
+__global__ void __launch_bounds__(256) k_pack_segments(const SubPoint *src, SubPoint *dst, const int *off_old, const int *off_new,
+                                                       const int *cnt, int nseg)
+{
+    const int r = (int)(blockIdx.x * blockDim.x + threadIdx.x);
+    if (r >= off_old[nseg]) return;
+    int lo = 0, hi = nseg - 1;
+    while (lo < hi) {
+        const int mid = (lo + hi + 1) >> 1;
+        if (off_old[mid] <= r) lo = mid; else hi = mid - 1;
+    }
+    const int l = r - off_old[lo];
+    if (l < cnt[lo]) dst[off_new[lo] + l] = src[r];
 }
 
 } // namespace gem

@@ -1141,6 +1141,90 @@ class ElevationMap:
                                            1 if compat else 0, C.byref(fused)), self._h, "gem_refuse_submaps")
         return nn.value, no.value, fused.value
 
+    # -- the global map: globalMap_, trajectory_, localMapLoc_ and updateGlobalMap on the device (DESIGN.md f16) -----------
+    def global_map_reset(self):
+        """the init branch (ElevationMapping.cpp:688-707): no submap, trajectory_ = [identity], centres = [(0, 0)]"""
+        check(self._lib.gem_global_map_reset(self._h), self._h, "gem_global_map_reset")
+
+    def global_map_reserve(self, records: int, submaps: int = 0):
+        """room for `records` records and `submaps` submaps (and the update's scratch), so that pushes and updates do not
+        allocate"""
+        check(self._lib.gem_global_map_reserve(self._h, int(records), int(submaps)), self._h, "gem_global_map_reserve")
+
+    def global_map_push(self, records, pose):
+        """the keyframe branch (:633-662): trajectory_.push_back(pose) (4 x 4, row 3 ignored), its centre = the pose's x, y,
+        then globalMap_.push_back(records), a contiguous (n, 8) float32 CUDA tensor (e.g. cut_submap()), copied"""
+        import torch
+        if not (_is_device(records) and records.dtype == torch.float32 and records.dim() == 2 and records.shape[1] == 8
+                and records.is_contiguous()):
+            raise ValueError("global_map_push: records must be a contiguous (n, 8) float32 CUDA tensor")
+        torch.cuda.current_stream(records.device).synchronize()   # the library reads the records on its own stream
+        p = (C.c_float * 16)(*[float(v) for v in np.asarray(pose, np.float32).reshape(16)])
+        check(self._lib.gem_global_map_push(self._h, _ptr(records), int(records.shape[0]), p), self._h, "gem_global_map_push")
+
+    def global_map_update(self, opt_poses, resolution: float, radius: float = 25.0, compat: bool = True) -> int:
+        """updateGlobalMap (:773-905) in one call: re-pose submaps 1 .. K'-1 with opt_poses (k x 4 x 4, K' = min(k,
+        submaps)), re-fuse every neighbour pair within `radius` of the pushed centres, pack the stack.  Returns the fused
+        cell count"""
+        poses = np.ascontiguousarray(np.asarray(opt_poses, np.float32).reshape(-1, 16))
+        fused = C.c_int(0)
+        check(self._lib.gem_global_map_update(self._h, poses.ctypes.data_as(_lib._FP), int(poses.shape[0]), float(resolution),
+                                              float(radius), 1 if compat else 0, C.byref(fused)), self._h, "gem_global_map_update")
+        return fused.value
+
+    def global_map_info(self):
+        """(submaps, keyframes, records)"""
+        s, k, r = C.c_int(), C.c_int(), C.c_longlong()
+        check(self._lib.gem_global_map_info(self._h, C.byref(s), C.byref(k), C.byref(r)), self._h, "gem_global_map_info")
+        return s.value, k.value, r.value
+
+    def _device_view(self, ptr: int, n: int):
+        """an (n, 8) float32 CUDA tensor over library memory, without a copy"""
+        import torch
+
+        class _View:
+            __cuda_array_interface__ = {"shape": (n, 8), "typestr": "<f4", "data": (ptr, False), "version": 2, "strides": None,
+                                        "stream": None}
+        dev = torch.device("cuda", self._device_index())
+        return torch.empty((0, 8), dtype=torch.float32, device=dev) if n == 0 else torch.as_tensor(_View(), device=dev)
+
+    def global_map_submaps(self):
+        """views of every submap as (n, 8) float32 CUDA tensors, valid until the next push, update, reserve or reset"""
+        out = []
+        p, n = C.c_void_p(), C.c_int()
+        for i in range(self.global_map_info()[0]):
+            check(self._lib.gem_global_map_submap(self._h, i, C.byref(p), C.byref(n)), self._h, "gem_global_map_submap")
+            out.append(self._device_view(p.value or 0, n.value))
+        return out
+
+    def global_map_records(self):
+        """the whole stack, submaps back to back in push order (composingGlobalMap's cloudpt, updateGlobalMap's
+        visualCloud_), as a view like global_map_submaps'"""
+        p, n = C.c_void_p(), C.c_longlong()
+        check(self._lib.gem_global_map_records(self._h, C.byref(p), C.byref(n)), self._h, "gem_global_map_records")
+        return self._device_view(p.value or 0, n.value)
+
+    def global_map_poses(self):
+        """(trajectory_ as (keyframes, 4, 4) float32, centres as (keyframes, 2) float32)"""
+        k = self.global_map_info()[1]
+        poses, centres = np.zeros((k, 16), np.float32), np.zeros((k, 2), np.float32)
+        for i in range(k):
+            check(self._lib.gem_global_map_pose(self._h, i, poses[i].ctypes.data_as(_lib._FP), centres[i].ctypes.data_as(_lib._FP)),
+                  self._h, "gem_global_map_pose")
+        return poses.reshape(k, 4, 4), centres
+
+    def save_submaps(self, directory, binary: bool = False, rgb_uint32: bool = False):
+        """savingSubMap (:461-476): every submap to `directory`/<i>.pcd through save_pcd.  An empty submap writes no file
+        (PCL throws there).  Returns the paths written"""
+        paths = []
+        for i, sub in enumerate(self.global_map_submaps()):
+            if sub.shape[0] == 0:
+                continue
+            path = os.path.join(str(directory), f"{i}.pcd")
+            self.save_pcd(path, sub, binary, rgb_uint32)
+            paths.append(path)
+        return paths
+
     def tiled_attach(self, tiles_r, tiles_c, my_rank, bucket_capacity, recv_records, recv_intensity, recv_counts, flags):
         """gem_tiled_attach: lists of device addresses (ints), one per rank, of the four peer-accessible buffers"""
         p = _lib.GemTiledPeers()

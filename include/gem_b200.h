@@ -777,6 +777,48 @@ int gem_transform_cloud(gem_map *m, void *points32_device, int n, const float T[
 int gem_refuse_submaps(gem_map *m, void *new_points32_device, int *n_new, void *old_points32_device, int *n_old, double resolution,
                        int compat, int *fused_out);
 
+/* ---- the global map: globalMap_, trajectory_, localMapLoc_ and updateGlobalMap (ElevationMapping.cpp:633-662, :688-707,
+ * :773-905, :491-498; DESIGN.md f16) ----
+ * A stack of keyframe submaps on the handle, in one device arena of 32-byte PointXYZRGBICT records, with the keyframe poses
+ * (trajectory_, row-major 4 x 4 floats, row 3 ignored) and centres (localMapLoc_, x, y).  The stack has its own stream and
+ * lock: reset, reserve, update, info, submap, records, pose and stream never take the handle's lock nor wait on its stream,
+ * so a loop closure does not hold up the add path.  After every call that changes it the submaps lie back to back in push
+ * order: the whole stack is one run of records, composingGlobalMap's cloudpt (:491-493) and the visualCloud_ updateGlobalMap
+ * rebuilds (:893-897), ready for gem_ros_cloud or gem_pcd_format as it is.
+ * gem_global_map_reset: the init branch (:688-707): no submap, trajectory_ = {identity}, centres = {(0, 0)}.  A new handle
+ *   starts in this state.
+ * gem_global_map_reserve: room for `records` records and `submaps` submaps, and the update scratch for a pair of submaps of
+ *   up to `records` records each, so that later pushes and updates do not allocate.  Otherwise capacity doubles on demand;
+ *   a growth that fails returns GEM_ERR_NOMEM and leaves the stack as it was.
+ * gem_global_map_push: the keyframe branch (:633-662): trajectory_.push_back(pose), centre = (pose[3], pose[7]), then
+ *   globalMap_.push_back of the n records (device memory, e.g. the output of cutSubmap), which are copied.  Submap k thus
+ *   belongs to keyframe k, where its accumulation started, and there is always one keyframe more than submaps.  The copy
+ *   waits for the work already enqueued on the handle's stream; the call returns when the copy is done.
+ * gem_global_map_update: updateGlobalMap (:773-905) in one call: K' = min(k, submaps); submap i of 1 <= i < K' is re-posed
+ *   with T = opt_poses[i] * trajectory_[i]^-1 (Eigen's Isometry3f arithmetic in float, DESIGN.md f16) and trajectory_[i] =
+ *   opt_poses[i]; then every pair (j, i) of :812-891 (kd-tree of the first K' centres within `radius`, nearest first,
+ *   ties by index; only when more than two results; the first result and i itself skipped) is re-fused as by
+ *   gem_refuse_submaps, with the counts on the device and no host round trip between pairs; the stack is packed again.
+ *   Centres are not updated (the reference never does), nor are trajectory_[0] and submap 0.  *fused_out = the cells
+ *   fused over all pairs.  One synchronisation, at the end.  opt_poses: k row-major 4 x 4 floats (Eigen's
+ *   Isometry3f::matrix().data() is column-major: transpose it).
+ * gem_global_map_info: submaps, keyframes (submaps + 1) and records in the stack; any pointer may be NULL.
+ * gem_global_map_submap / gem_global_map_records: device pointer and count of submap i / of the whole packed stack, valid
+ *   until the next push, update, reserve or reset.
+ * gem_global_map_pose: keyframe i's pose (16 floats) and centre (2 floats); either may be NULL.
+ * gem_global_map_stream: the stack's stream (NULL on failure).
+ * GEM_ERR_INVALID, with nothing changed, for: k < 0 or NULL opt_poses with k > 0; resolution <= 0 or not finite; radius
+ * negative or NaN; n < 0, NULL pose, or NULL or non-device records with n > 0 on a push; an index out of range. */
+int gem_global_map_reset(gem_map *m);
+int gem_global_map_reserve(gem_map *m, long long records, int submaps);
+int gem_global_map_push(gem_map *m, const void *records_device, int n, const float pose[16]);
+int gem_global_map_update(gem_map *m, const float *opt_poses, int k, double resolution, double radius, int compat, int *fused_out);
+int gem_global_map_info(gem_map *m, int *submaps, int *keyframes, long long *records);
+int gem_global_map_submap(gem_map *m, int i, void **records_device_out, int *count_out);
+int gem_global_map_records(gem_map *m, void **records_device_out, long long *count_out);
+int gem_global_map_pose(gem_map *m, int i, float pose_out[16], float centre_out[2]);
+void *gem_global_map_stream(gem_map *m);
+
 /* ---- tiled maps, peer path: one kernel routes AND exchanges (no collective library, no barrier kernel) ----------
  * The caller allocates, on every rank, four peer-accessible buffers (e.g. CUDA IPC / torch symmetric memory; the
  * library does no inter-process plumbing) and passes the addresses under which THIS device sees every rank's copy:

@@ -624,6 +624,51 @@ class ElevationMap {
               "gem_refuse_submaps");
         return fused;
     }
+    // The global map (DESIGN.md f16): globalMap_, trajectory_ and localMapLoc_ on the device, with updateGlobalMap in one
+    // call.  Poses are row-major 4 x 4 floats (row 3 ignored); Eigen's Isometry3f::matrix().data() is column-major, so
+    // transpose it first.  globalMapPush = the keyframe branch (:633-662), globalMapUpdate = updateGlobalMap (:773-905),
+    // globalMapRecords = composingGlobalMap's cloudpt (:491-493), saveSubmaps = savingSubMap (:461-476).  Device pointers
+    // from globalMapSubmap / globalMapRecords are valid until the next push, update, reserve or reset.
+    void globalMapReset() { check(gem_global_map_reset(h_), "gem_global_map_reset"); }
+    void globalMapReserve(long long records, int submaps = 0) { check(gem_global_map_reserve(h_, records, submaps), "gem_global_map_reserve"); }
+    void globalMapPush(const void *records_device, size_t n, const float pose_rowmajor[16])
+    {
+        check(gem_global_map_push(h_, records_device, (int)n, pose_rowmajor), "gem_global_map_push");
+    }
+    int globalMapUpdate(const float *opt_poses_rowmajor, int k, double resolution, double radius = 25.0, bool compat_precedence = true)
+    {
+        int fused = 0;
+        check(gem_global_map_update(h_, opt_poses_rowmajor, k, resolution, radius, compat_precedence ? 1 : 0, &fused), "gem_global_map_update");
+        return fused;
+    }
+    int globalMapSubmaps()
+    {
+        int n = 0;
+        check(gem_global_map_info(h_, &n, nullptr, nullptr), "gem_global_map_info");
+        return n;
+    }
+    const void *globalMapSubmap(int i, int *count)
+    {
+        void *p = nullptr;
+        check(gem_global_map_submap(h_, i, &p, count), "gem_global_map_submap");
+        return p;
+    }
+    const void *globalMapRecords(long long *count)
+    {
+        void *p = nullptr;
+        check(gem_global_map_records(h_, &p, count), "gem_global_map_records");
+        return p;
+    }
+    void globalMapPose(int i, float pose_rowmajor[16], float centre[2]) { check(gem_global_map_pose(h_, i, pose_rowmajor, centre), "gem_global_map_pose"); }
+    // every non-empty submap to directory + i + ".pcd" (directory ends with '/', like GEM's submap_saving_dir)
+    void saveSubmaps(const std::string &directory, bool binary = false, bool rgbUint32 = false)
+    {
+        for (int i = 0, k = globalMapSubmaps(); i < k; i++) {
+            int n = 0;
+            const void *p = globalMapSubmap(i, &n);
+            if (n > 0) savePcd(directory + std::to_string(i) + ".pcd", p, (size_t)n, true, binary, rgbUint32);
+        }
+    }
     // upstream visibilityCleanup / GEM Raytracing (gpu_process.cu:1304)
     void clean() { check(gem_raytracing(h_), "gem_raytracing"); }
     void optMove(const float p[2], float dz, float aligned[2]) { check(gem_opt_move(h_, p, dz, aligned), "gem_opt_move"); }
