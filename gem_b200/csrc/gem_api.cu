@@ -70,20 +70,26 @@ struct TiledState { // gem_tiled_attach
     const void *route_func = nullptr; // the route kernel the graph was built with (k_route_peer or k_route_peer_any)
 };
 
-struct OctBuf { // a device scratch buffer (octree, costmap and voxel-grid calls): grows on demand, never shrinks
+struct DevBuf { // a device buffer and its capacity in bytes; scratch buffers grow on demand (scratch_grow), never shrink
     void *p = nullptr;
     size_t cap = 0;
     template <typename T> T *as() const { return static_cast<T *>(p); }
 };
-struct VoxScratch { // gem_voxel_grid (gem_voxel.cuh): keys and input indices before / after the sort, runs, offsets
-    OctBuf key[2], idx[2], cnt, off, temp, acc;
+struct KeyRuns { // records bucketed by a 64-bit key (key_runs_grow, key_runs_enqueue): keys and record indices before /
+                 // after the sort, the run lengths and their offsets, the temporary of the sort, the encoding and the scan
+    DevBuf key[2], idx[2], cnt, off, temp;
 };
-struct MlsScratch { // gem_mls_upsample (gem_mls.cuh): cell keys and indices before / after the sort, the points in cell
-                   // order, the distinct cells, neighbour and output counts, output offsets, the long lists and their keys
-    OctBuf key[2], idx[2], spts, ukey, ucnt, uoff, nbr, ocnt, ooff, longs, lkeys, temp, acc;
+struct VoxScratch { // gem_voxel_grid (gem_voxel.cuh): the voxel keys' runs, the bounds and counters
+    KeyRuns kr;
+    DevBuf acc;
+};
+struct MlsScratch { // gem_mls_upsample (gem_mls.cuh): the cell keys' runs, the points in cell order, the distinct cells,
+                   // neighbour and output counts, output offsets, the long lists and their keys
+    KeyRuns kr;
+    DevBuf spts, ukey, nbr, ocnt, ooff, longs, lkeys, acc;
 };
 struct InflScratch { // gem_costmap_inflate (gem_inflate.cuh): per-cell keys and pop records, the tables, bin starts, block counts
-    OctBuf key, pops, tab, gstart, blk;
+    DevBuf key, pops, tab, gstart, blk;
     // the tables in `tab` were built for these parameters (r < 0: none)
     long long r = -1;
     double res = 0.0, weight = 0.0, inscribed = 0.0;
@@ -91,10 +97,11 @@ struct InflScratch { // gem_costmap_inflate (gem_inflate.cuh): per-cell keys and
     bool key_dirty = false; // `key` was (re)allocated and its clearing memset has not been enqueued yet
 };
 struct PcdScratch { // gem_pcd_format (gem_pcd.cuh): per-tile byte counts, their inclusive scan, the scan's temporary
-    OctBuf bytes, ends, temp;
+    DevBuf bytes, ends, temp;
 };
 struct OctScratch { // gem_color_octree (gem_octree.cuh); every buffer is consistent with its own capacity at all times
-    OctBuf code[2], idx[2], leaf, cnt, off, level, ghead, gid, val, groups, ctr, temp, key2[2], nkey[2], nrec[2], dense;
+    KeyRuns kr;          // the leaf codes' runs; kr.temp also serves the phase-2 sorts
+    DevBuf leaf, level, ghead, gid, val, groups, ctr, key2[2], nkey[2], nrec[2], dense;
     long long bytes = -1; // size of the last stream (in nrec[1]); -1: none
     double res = 0.0;     // the resolution it was built at
     gem_octree info{};
@@ -114,12 +121,12 @@ struct GlobalStore { // globalMap_, trajectory_ and localMapLoc_ on the device (
     std::mutex mu;                     // the stack's own lock: no call on it takes the handle's mutex except a push, briefly
     cudaStream_t stream = nullptr;     // the stack's own stream
     cudaEvent_t ev = nullptr;          // push: the handle's stream -> the stack's stream
-    OctBuf arena[2];                   // arena[cur]: the submaps back to back in push order; the other: the re-pack target
+    DevBuf arena[2];                   // arena[cur]: the submaps back to back in push order; the other: the re-pack target
     int cur = 0;
     long long cap = 0;                 // records each arena buffer holds
-    OctBuf meta;                       // update: counts, old and new offsets, fused count, the re-pose table
+    DevBuf meta;                       // update: counts, old and new offsets, fused count, the re-pose table
     int meta_submaps = 0;              // submaps `meta` is laid out for
-    OctBuf pair;                       // update: one pair's hash tables, keep flags, scan counts and compaction output
+    DevBuf pair;                       // update: one pair's hash tables, keep flags, scan counts and compaction output
     std::vector<int> cnt, off{0};      // host mirror: per submap its count, and its offset (one entry more)
     std::vector<float> poses{1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1}; // trajectory_: 16 floats per keyframe
     std::vector<float> centres{0.0f, 0.0f};                                  // localMapLoc_: x, y per keyframe
@@ -178,15 +185,15 @@ struct gem_map {
     int *split_queue = nullptr, *split_ctr = nullptr;
     SplitStats *split_stats = nullptr;
     OctScratch oct;                // gem_color_octree: scratch and the last stream
-    OctBuf cost_scratch;           // costmap calls: the winner per costmap cell (int), or the copy of a rolled grid
+    DevBuf cost_scratch;           // costmap calls: the winner per costmap cell (int), or the copy of a rolled grid
     CostMarksDev *cost_acc = nullptr; // costmap mark calls: counts and encoded touch bounds
     VoxScratch vox;                // gem_voxel_grid
     MlsScratch mls;                // gem_mls_upsample
     PcdScratch pcd;                // gem_pcd_format
-    OctBuf ros_framing;            // gem_ros_*: the framing bytes of the call, staged for k_ros_framing
-    OctBuf ros_stage;              // gem_ros_* map messages for pinned outputs, written here and copied over in one DMA
+    DevBuf ros_framing;            // gem_ros_*: the framing bytes of the call, staged for k_ros_framing
+    DevBuf ros_stage;              // gem_ros_* map messages for pinned outputs, written here and copied over in one DMA
     InflScratch infl;              // gem_costmap_inflate
-    OctBuf refuse;                 // gem_refuse_submaps: one pair's scratch (pair_layout)
+    DevBuf refuse;                 // gem_refuse_submaps: one pair's scratch (pair_layout)
     GlobalStore gmap;              // gem_global_map_*
     unsigned long long *d_stamps = nullptr; // gem_debug_stamps
     int *d_raylist = nullptr;      // ray clean-up: cells that cast a ray + their count
@@ -203,7 +210,7 @@ struct gem_map {
     unsigned async_calls = 0;
     // gem_add_pointcloud2_host_async: per ring slot the message bytes and the camera image as they arrive (copy
     // stream), and one BGR8 conversion target (handle's stream); grown on demand
-    OctBuf pc2_raw[3], pc2_img[3], pc2_bgr;
+    DevBuf pc2_raw[3], pc2_img[3], pc2_bgr;
     // gem_add_points_multi: ring of per-call FrameParams tables (pinned host + device)
     FrameParams *h_frames = nullptr, *d_frames = nullptr;
     cudaEvent_t ev_frames[4] = {nullptr, nullptr, nullptr, nullptr};
@@ -287,10 +294,78 @@ template <typename T> int dev_alloc(gem_map *m, T **p, size_t count)
 {
     void *q = nullptr;
     cudaError_t e = cudaMalloc(&q, count * sizeof(T) + 16);
-    if (e != cudaSuccess) return fail(m, GEM_ERR_NOMEM, std::string("cudaMalloc: ") + cudaGetErrorString(e));
+    if (e != cudaSuccess) {
+        cudaGetLastError(); // a failed cudaMalloc stays recorded as the last error, which the next launch check would report
+        return fail(m, GEM_ERR_NOMEM, std::string("cudaMalloc: ") + cudaGetErrorString(e));
+    }
     m->allocs.push_back(q);
     *p = (T *)q;
     return GEM_OK;
+}
+
+// Grow a device scratch buffer to at least `bytes`, with a quarter of slack and at least 4 KiB so that slowly growing
+// inputs do not reallocate on every call.  The new buffer is allocated before the old one is released, so a failed
+// growth leaves the buffer as it was; `stream` (the one the buffer's users run on) is drained before the old buffer
+// goes, because work queued on it (an update_origin, say) may still read it.
+int scratch_grow(gem_map *m, DevBuf &b, size_t bytes, const char *what, cudaStream_t stream)
+{
+    if (b.cap >= bytes) return GEM_OK;
+    bytes = std::max(bytes + bytes / 4, (size_t)4096);
+    void *q = nullptr;
+    const cudaError_t e = cudaMalloc(&q, bytes);
+    if (e != cudaSuccess) {
+        cudaGetLastError(); // as in dev_alloc
+        return fail(m, GEM_ERR_NOMEM, std::string(what) + ": cudaMalloc: " + cudaGetErrorString(e));
+    }
+    if (b.p) {
+        cudaStreamSynchronize(stream);
+        cudaFree(b.p);
+    }
+    b.p = q;
+    b.cap = bytes;
+    return GEM_OK;
+}
+
+// Size every buffer of `k` for n records, its temporary for the sort (up to 64 key bits), the run-length encoding, the
+// scan of the run lengths and `temp_bytes` more that the caller needs later.  Every buffer is sized before the first
+// write, so that a failed growth writes nothing.
+int key_runs_grow(gem_map *m, KeyRuns &k, int n, size_t temp_bytes, const char *what)
+{
+    using u64 = unsigned long long;
+    const size_t N = (size_t)n;
+    cudaStream_t st = m->stream;
+    size_t t_sort = 0, t_rle = 0, t_scan = 0;
+    GEM_CUDA(m, cub::DeviceRadixSort::SortPairs(nullptr, t_sort, (u64 *)nullptr, (u64 *)nullptr, (int *)nullptr, (int *)nullptr, n, 0, 64, st));
+    GEM_CUDA(m, cub::DeviceRunLengthEncode::Encode(nullptr, t_rle, (u64 *)nullptr, (u64 *)nullptr, (int *)nullptr, (int *)nullptr, n, st));
+    GEM_CUDA(m, cub::DeviceScan::ExclusiveSum(nullptr, t_scan, (int *)nullptr, (int *)nullptr, n, st));
+    int rc;
+    if ((rc = scratch_grow(m, k.key[0], N * 8, what, st)) || (rc = scratch_grow(m, k.key[1], N * 8, what, st)) ||
+        (rc = scratch_grow(m, k.idx[0], N * 4, what, st)) || (rc = scratch_grow(m, k.idx[1], N * 4, what, st)) ||
+        (rc = scratch_grow(m, k.cnt, N * 4, what, st)) || (rc = scratch_grow(m, k.off, N * 4, what, st)))
+        return rc;
+    return scratch_grow(m, k.temp, std::max(std::max(t_sort, t_rle), std::max(t_scan, temp_bytes)), what, st);
+}
+
+// Bucket the n records whose keys and indices the caller wrote to k.key[0] and k.idx[0]: the stable sort on key bits
+// [0, bits) into k.key[1] / k.idx[1], the runs of equal keys (their keys to `unique`, their lengths to k.cnt, their number
+// to *nruns, all on the device) and the runs' offsets in k.off, issued on the handle's stream
+int key_runs_enqueue(gem_map *m, KeyRuns &k, int n, int bits, unsigned long long *unique, int *nruns)
+{
+    using u64 = unsigned long long;
+    cudaStream_t st = m->stream;
+    size_t tcap = k.temp.cap;
+    // the run-length encoding writes nruns <= n counts; the scan runs over all n, so the rest must be defined
+    GEM_CUDA(m, cudaMemsetAsync(k.cnt.p, 0, (size_t)n * sizeof(int), st));
+    GEM_CUDA(m, cub::DeviceRadixSort::SortPairs(k.temp.p, tcap, k.key[0].as<u64>(), k.key[1].as<u64>(), k.idx[0].as<int>(), k.idx[1].as<int>(), n, 0, bits, st));
+    GEM_CUDA(m, cub::DeviceRunLengthEncode::Encode(k.temp.p, tcap, k.key[1].as<u64>(), unique, k.cnt.as<int>(), nruns, n, st));
+    GEM_CUDA(m, cub::DeviceScan::ExclusiveSum(k.temp.p, tcap, k.cnt.as<int>(), k.off.as<int>(), n, st));
+    return GEM_OK;
+}
+
+bool ranges_meet(const void *a, size_t na, const void *b, size_t nb)
+{
+    const uintptr_t a0 = (uintptr_t)a, b0 = (uintptr_t)b;
+    return na > 0 && nb > 0 && a0 < b0 + nb && b0 < a0 + na;
 }
 
 // capacity of a per-call list of the cells holding MORE than k of a call's <= P records: at most P / (k + 1) such
@@ -720,6 +795,29 @@ static GridMapFrame grid_frame(const gem_map *m, float cx, float cy, int sx, int
     return f;
 }
 
+// the cells and the geometry of the shown map or of the snapshot gem_snapshot_shown took (out = nullptr)
+static GridCloudSrc grid_cells(const gem_map *m, int source)
+{
+    const MapGeom &g = source == GEM_GRID_SHOWN ? m->geom : m->prev_geom;
+    GridCloudSrc src;
+    src.s = source == GEM_GRID_SHOWN ? live_cells(m->ml) : snapshot_cells(m->prev_ev, m->prev_ci, m->prev_tr);
+    src.f = grid_frame(m, g.cx, g.cy, g.sx, g.sy);
+    src.out = nullptr;
+    return src;
+}
+
+// the grid a call `what` reads (GEM_GRID_SHOWN or GEM_GRID_SNAPSHOT), ready to be read; the caller holds the lock
+static int grid_source(gem_map *m, int source, const char *what, GridCloudSrc *src)
+{
+    if (m->geom.tiled) return fail(m, GEM_ERR_INVALID, std::string(what) + ": not available on tiled handles");
+    if (source == GEM_GRID_SNAPSHOT && !m->prev_valid)
+        return fail(m, GEM_ERR_INVALID, std::string(what) + ": no snapshot (call gem_snapshot_shown first)");
+    const int rc = flush_for_observer(m);
+    if (rc) return rc;
+    *src = grid_cells(m, source);
+    return GEM_OK;
+}
+
 // count -> scan -> write of the cells Src takes, in GridMapIterator order, issued on the handle's stream; the total is
 // left in device memory (*d_total_out: the compaction scratch, valid until the next compaction)
 template <class Src> static int compact_cells_issue(gem_map *m, const Src &src, int capacity, int **d_total_out)
@@ -892,13 +990,13 @@ int gem_destroy(gem_map *m)
         for (cudaEvent_t e : m->free_events) cudaEventDestroy(e);
         for (void *p : m->allocs) cudaFree(p);
         if (m->local.buf) cudaFree(m->local.buf);
-        for (OctBuf *b : {&m->oct.code[0], &m->oct.code[1], &m->oct.idx[0], &m->oct.idx[1], &m->oct.leaf, &m->oct.cnt, &m->oct.off,
-                          &m->oct.level, &m->oct.ghead, &m->oct.gid, &m->oct.val, &m->oct.groups, &m->oct.ctr, &m->oct.temp,
+        for (KeyRuns *k : {&m->oct.kr, &m->vox.kr, &m->mls.kr})
+            for (DevBuf *b : {&k->key[0], &k->key[1], &k->idx[0], &k->idx[1], &k->cnt, &k->off, &k->temp})
+                if (b->p) cudaFree(b->p);
+        for (DevBuf *b : {&m->oct.leaf, &m->oct.level, &m->oct.ghead, &m->oct.gid, &m->oct.val, &m->oct.groups, &m->oct.ctr,
                           &m->oct.key2[0], &m->oct.key2[1], &m->oct.nkey[0], &m->oct.nkey[1], &m->oct.nrec[0], &m->oct.nrec[1],
-                          &m->oct.dense, &m->cost_scratch, &m->vox.key[0], &m->vox.key[1], &m->vox.idx[0], &m->vox.idx[1],
-                          &m->vox.cnt, &m->vox.off, &m->vox.temp, &m->vox.acc, &m->mls.key[0], &m->mls.key[1], &m->mls.idx[0],
-                          &m->mls.idx[1], &m->mls.spts, &m->mls.ukey, &m->mls.ucnt, &m->mls.uoff, &m->mls.nbr, &m->mls.ocnt,
-                          &m->mls.ooff, &m->mls.longs, &m->mls.lkeys, &m->mls.temp, &m->mls.acc, &m->pc2_raw[0],
+                          &m->oct.dense, &m->cost_scratch, &m->vox.acc, &m->mls.spts, &m->mls.ukey, &m->mls.nbr, &m->mls.ocnt,
+                          &m->mls.ooff, &m->mls.longs, &m->mls.lkeys, &m->mls.acc, &m->pc2_raw[0],
                           &m->pc2_raw[1], &m->pc2_raw[2], &m->pc2_img[0], &m->pc2_img[1], &m->pc2_img[2], &m->pc2_bgr,
                           &m->pcd.bytes, &m->pcd.ends, &m->pcd.temp, &m->infl.key, &m->infl.pops, &m->infl.tab,
                           &m->infl.gstart, &m->infl.blk, &m->ros_framing, &m->ros_stage, &m->refuse, &m->gmap.arena[0],
@@ -1629,9 +1727,10 @@ static int harvest_to_staging(gem_map *m, const float current_xy[2], const float
 {
     int rc = ensure_out_staging(m);
     if (rc) return rc;
+    const GridCloudSrc snap = grid_cells(m, GEM_GRID_SNAPSHOT);
     HarvestSrc src;
-    src.s = snapshot_cells(m->prev_ev, m->prev_ci, m->prev_tr);
-    src.f = grid_frame(m, m->prev_geom.cx, m->prev_geom.cy, m->prev_geom.sx, m->prev_geom.sy);
+    src.s = snap.s;
+    src.f = snap.f;
     // :727-734: current_x (float) -+ length_ * resolution_ / 2 with the node's double resolution_
     const double halfwin = (double)m->L * src.f.res / 2;
     src.lox = (double)current_xy[0] - halfwin; src.hix = (double)current_xy[0] + halfwin;
@@ -1665,17 +1764,11 @@ int gem_export_grid_cloud(gem_map *m, int source, void *points32_device, int cap
 {
     if (!m || !count_out || capacity < 0 || (capacity > 0 && !points32_device) || (source != GEM_GRID_SHOWN && source != GEM_GRID_SNAPSHOT))
         return fail(m, GEM_ERR_INVALID, "gem_export_grid_cloud: bad argument");
-    if (m->geom.tiled) return fail(m, GEM_ERR_INVALID, "gem_export_grid_cloud: not available on tiled handles");
     Lock lk(m->mu);
     SetDev sd(m->dev);
-    if (source == GEM_GRID_SNAPSHOT && !m->prev_valid)
-        return fail(m, GEM_ERR_INVALID, "gem_export_grid_cloud: no snapshot (call gem_snapshot_shown first)");
-    int rc = flush_for_observer(m);
-    if (rc) return rc;
     GridCloudSrc src;
-    const MapGeom &g = source == GEM_GRID_SHOWN ? m->geom : m->prev_geom;
-    src.s = source == GEM_GRID_SHOWN ? live_cells(m->ml) : snapshot_cells(m->prev_ev, m->prev_ci, m->prev_tr);
-    src.f = grid_frame(m, g.cx, g.cy, g.sx, g.sy);
+    int rc = grid_source(m, source, "gem_export_grid_cloud", &src);
+    if (rc) return rc;
     src.out = reinterpret_cast<float4 *>(points32_device);
     int total = 0;
     if ((rc = compact_cells(m, src, (int)std::min<size_t>((size_t)capacity, m->nc), &total))) return rc;
@@ -1694,12 +1787,10 @@ int gem_grid_cloud_split(gem_map *m, int source, int mean_k, double stddev_mul, 
         (distance_capacity > 0 && !mean_distance_device))
         return fail(m, GEM_ERR_INVALID, "gem_grid_cloud_split: bad argument");
     if (mean_k < 1 || mean_k > SPLIT_MAX_K) return fail(m, GEM_ERR_INVALID, "gem_grid_cloud_split: mean_k must be in [1, 64]");
-    if (m->geom.tiled) return fail(m, GEM_ERR_INVALID, "gem_grid_cloud_split: not available on tiled handles");
     Lock lk(m->mu);
     SetDev sd(m->dev);
-    if (source == GEM_GRID_SNAPSHOT && !m->prev_valid)
-        return fail(m, GEM_ERR_INVALID, "gem_grid_cloud_split: no snapshot (call gem_snapshot_shown first)");
-    int rc = flush_for_observer(m);
+    GridCloudSrc g;
+    int rc = grid_source(m, source, "gem_grid_cloud_split", &g);
     if (rc) return rc;
     const int L = m->L;
     if (!m->split_stats) { // the scratch is published only once every buffer exists (a failed call leaves it unset)
@@ -1713,11 +1804,6 @@ int gem_grid_cloud_split(gem_map *m, int source, int mean_k, double stddev_mul, 
         m->split_zg = zg; m->split_xg = xg; m->split_yg = yg; m->split_dcell = dcell; m->split_dist = dist;
         m->split_queue = queue; m->split_ctr = ctr; m->split_stats = st;
     }
-    GridCloudSrc g;
-    const MapGeom &geo = source == GEM_GRID_SHOWN ? m->geom : m->prev_geom;
-    g.s = source == GEM_GRID_SHOWN ? live_cells(m->ml) : snapshot_cells(m->prev_ev, m->prev_ci, m->prev_tr);
-    g.f = grid_frame(m, geo.cx, geo.cy, geo.sx, geo.sy);
-    g.out = nullptr;
     GEM_CUDA(m, cudaMemsetAsync(m->split_ctr, 0, 2 * sizeof(int), m->stream));
     GEM_LAUNCH(m, GEM_PROF_OTHER, k_split_stage<<<blocks_for(m->nc, 256), 256, 0, m->stream>>>(g, m->split_zg, m->split_xg, m->split_yg, m->split_dcell));
     const int nt = (L + SPLIT_TILE - 1) / SPLIT_TILE;
@@ -1726,8 +1812,8 @@ int gem_grid_cloud_split(gem_map *m, int source, int mean_k, double stddev_mul, 
     // the queue's length stays on the device: k_split_knn_far's fixed grid strides over it
 #define GEM_SPLIT_KNN(KC)                                                                                                              \
     do {                                                                                                                               \
-        GEM_LAUNCH(m, GEM_PROF_OTHER, k_split_knn<KC><<<grid, SPLIT_TILE * SPLIT_TILE, 0, m->stream>>>(m->split_zg, m->split_xg, m->split_yg, L, geo.sx, geo.sy, mean_k, m->split_dcell, m->split_queue, m->split_ctr)); \
-        GEM_LAUNCH(m, GEM_PROF_OTHER, k_split_knn_far<KC><<<NUM_SMS * 4, 128, 0, m->stream>>>(m->split_zg, m->split_xg, m->split_yg, L, geo.sx, geo.sy, mean_k, m->split_dcell, m->split_queue, m->split_ctr)); \
+        GEM_LAUNCH(m, GEM_PROF_OTHER, k_split_knn<KC><<<grid, SPLIT_TILE * SPLIT_TILE, 0, m->stream>>>(m->split_zg, m->split_xg, m->split_yg, L, g.f.sx, g.f.sy, mean_k, m->split_dcell, m->split_queue, m->split_ctr)); \
+        GEM_LAUNCH(m, GEM_PROF_OTHER, k_split_knn_far<KC><<<NUM_SMS * 4, 128, 0, m->stream>>>(m->split_zg, m->split_xg, m->split_yg, L, g.f.sx, g.f.sy, mean_k, m->split_dcell, m->split_queue, m->split_ctr)); \
     } while (0)
     if (K <= 8) GEM_SPLIT_KNN(8);
     else if (K <= 24) GEM_SPLIT_KNN(24);
@@ -1764,27 +1850,6 @@ int gem_grid_cloud_split(gem_map *m, int source, int mean_k, double stddev_mul, 
     out->threshold = st.threshold;
     return GEM_OK;
 }
-
-// Grow a device scratch buffer (octree, costmap, voxel grid) to at least `bytes`, with a quarter of slack and at least
-// 4 KiB so that slowly growing inputs do not reallocate on every call.  The new buffer is allocated before the old one is
-// released, so a failed growth leaves the buffer as it was; the stream is drained before the old buffer goes, because
-// work queued on it (an update_origin, say) may still read it.
-static int scratch_grow(gem_map *m, OctBuf &b, size_t bytes, const char *what)
-{
-    if (b.cap >= bytes) return GEM_OK;
-    bytes = std::max(bytes + bytes / 4, (size_t)4096);
-    void *q = nullptr;
-    const cudaError_t e = cudaMalloc(&q, bytes);
-    if (e != cudaSuccess) return fail(m, GEM_ERR_NOMEM, std::string(what) + ": cudaMalloc: " + cudaGetErrorString(e));
-    if (b.p) {
-        cudaStreamSynchronize(m->stream);
-        cudaFree(b.p);
-    }
-    b.p = q;
-    b.cap = bytes;
-    return GEM_OK;
-}
-static int oct_grow(gem_map *m, OctBuf &b, size_t bytes) { return scratch_grow(m, b, bytes, "gem_color_octree"); }
 
 // pointCloudtoOctomap's tree (ElevationMapping.cpp:1157-1174) as the ColorOcTree::writeData stream (gem_octree.cuh,
 // DESIGN.md f7)
@@ -1827,32 +1892,21 @@ int gem_color_octree(gem_map *m, const void *points32_device, int n, double reso
     cudaStream_t st = m->stream;
     int rc;
     // phase 1: keys, the sort by code, the leaves and their runs, the classification (sizes of phase 2)
-    size_t t_sort = 0, t_rle = 0, t_scan = 0;
-    GEM_CUDA(m, cub::DeviceRadixSort::SortPairs(nullptr, t_sort, (u64 *)nullptr, (u64 *)nullptr, (int *)nullptr, (int *)nullptr, n, 0, 49, st));
-    GEM_CUDA(m, cub::DeviceRunLengthEncode::Encode(nullptr, t_rle, (u64 *)nullptr, (u64 *)nullptr, (int *)nullptr, (int *)nullptr, n, st));
-    GEM_CUDA(m, cub::DeviceScan::ExclusiveSum(nullptr, t_scan, (int *)nullptr, (int *)nullptr, n, st));
-    if ((rc = oct_grow(m, S.code[0], N * 8)) || (rc = oct_grow(m, S.code[1], N * 8)) || (rc = oct_grow(m, S.idx[0], N * 4)) ||
-        (rc = oct_grow(m, S.idx[1], N * 4)) || (rc = oct_grow(m, S.leaf, N * 8)) || (rc = oct_grow(m, S.cnt, N * 4)) ||
-        (rc = oct_grow(m, S.off, N * 4)) || (rc = oct_grow(m, S.level, N * 4)) || (rc = oct_grow(m, S.ghead, N * 4)) ||
-        (rc = oct_grow(m, S.gid, N * 4)) || (rc = oct_grow(m, S.val, N * 4)) ||
-        (rc = oct_grow(m, S.groups, (N / 8 + 1) * sizeof(OctGroup))) || (rc = oct_grow(m, S.ctr, sizeof(OctCounters))) ||
-        (rc = oct_grow(m, S.temp, std::max(t_sort, std::max(t_rle, t_scan)))))
+    const char *what = "gem_color_octree";
+    if ((rc = key_runs_grow(m, S.kr, n, 0, what)) || (rc = scratch_grow(m, S.leaf, N * 8, what, st)) ||
+        (rc = scratch_grow(m, S.level, N * 4, what, st)) || (rc = scratch_grow(m, S.ghead, N * 4, what, st)) ||
+        (rc = scratch_grow(m, S.gid, N * 4, what, st)) || (rc = scratch_grow(m, S.val, N * 4, what, st)) ||
+        (rc = scratch_grow(m, S.groups, (N / 8 + 1) * sizeof(OctGroup), what, st)) || (rc = scratch_grow(m, S.ctr, sizeof(OctCounters), what, st)))
         return rc;
     const float4 *pts = static_cast<const float4 *>(points32_device);
     OctCounters *ctr = S.ctr.as<OctCounters>();
     u64 *leaf = S.leaf.as<u64>();
-    int *cnt = S.cnt.as<int>(), *off = S.off.as<int>(), *level = S.level.as<int>(), *sidx = S.idx[1].as<int>();
+    int *cnt = S.kr.cnt.as<int>(), *off = S.kr.off.as<int>(), *level = S.level.as<int>(), *sidx = S.kr.idx[1].as<int>();
     uint32_t *val = S.val.as<uint32_t>();
-    size_t tcap = S.temp.cap;
     GEM_CUDA(m, cudaMemsetAsync(ctr, 0, sizeof(OctCounters), st));
-    // the run-length encoding writes nruns <= n counts (a device-side number); the scan below runs over all n, so the
-    // rest must be defined
-    GEM_CUDA(m, cudaMemsetAsync(cnt, 0, N * sizeof(int), st));
-    GEM_LAUNCH(m, GEM_PROF_OTHER, k_oct_keys<<<blocks_for(N, 256, 1 << 30), 256, 0, st>>>(pts, n, rf, S.code[0].as<u64>(), S.idx[0].as<int>(), ctr));
+    GEM_LAUNCH(m, GEM_PROF_OTHER, k_oct_keys<<<blocks_for(N, 256, 1 << 30), 256, 0, st>>>(pts, n, rf, S.kr.key[0].as<u64>(), S.kr.idx[0].as<int>(), ctr));
     GEM_CUDA(m, cudaGetLastError());
-    GEM_CUDA(m, cub::DeviceRadixSort::SortPairs(S.temp.p, tcap, S.code[0].as<u64>(), S.code[1].as<u64>(), S.idx[0].as<int>(), sidx, n, 0, 49, st));
-    GEM_CUDA(m, cub::DeviceRunLengthEncode::Encode(S.temp.p, tcap, S.code[1].as<u64>(), leaf, cnt, &ctr->nruns, n, st));
-    GEM_CUDA(m, cub::DeviceScan::ExclusiveSum(S.temp.p, tcap, cnt, off, n, st));
+    if ((rc = key_runs_enqueue(m, S.kr, n, 49, leaf, &ctr->nruns))) return rc;
     GEM_LAUNCH(m, GEM_PROF_OTHER, k_oct_classify<<<blocks_for(N, 256, 1 << 30), 256, 0, st>>>(leaf, cnt, off, sidx, pts, P, level, S.ghead.as<int>(), S.gid.as<int>(),
                                                                                              S.groups.as<OctGroup>(), val, ctr, n));
     GEM_CUDA(m, cudaGetLastError());
@@ -1869,18 +1923,19 @@ int gem_color_octree(gem_map *m, const void *points32_device, int n, double reso
         size_t t_keys = 0, t_nodes = 0;
         GEM_CUDA(m, cub::DeviceRadixSort::SortKeys(nullptr, t_keys, (u64 *)nullptr, (u64 *)nullptr, (int)ngp, 0, 32 + gbits, st));
         GEM_CUDA(m, cub::DeviceRadixSort::SortPairs(nullptr, t_nodes, (u64 *)nullptr, (u64 *)nullptr, (u64 *)nullptr, (u64 *)nullptr, (int)nnode, 0, 53, st));
-        if ((rc = oct_grow(m, S.key2[0], ngp * 8)) || (rc = oct_grow(m, S.key2[1], ngp * 8)) || (rc = oct_grow(m, S.nkey[0], nnode * 8)) ||
-            (rc = oct_grow(m, S.nkey[1], nnode * 8)) || (rc = oct_grow(m, S.nrec[0], nnode * 8)) || (rc = oct_grow(m, S.nrec[1], nnode * 8)) ||
-            (rc = oct_grow(m, S.dense, (size_t)hc.dense * 4)) || (rc = oct_grow(m, S.temp, std::max(t_keys, t_nodes))))
+        if ((rc = scratch_grow(m, S.key2[0], ngp * 8, what, st)) || (rc = scratch_grow(m, S.key2[1], ngp * 8, what, st)) ||
+            (rc = scratch_grow(m, S.nkey[0], nnode * 8, what, st)) || (rc = scratch_grow(m, S.nkey[1], nnode * 8, what, st)) ||
+            (rc = scratch_grow(m, S.nrec[0], nnode * 8, what, st)) || (rc = scratch_grow(m, S.nrec[1], nnode * 8, what, st)) ||
+            (rc = scratch_grow(m, S.dense, (size_t)hc.dense * 4, what, st)) || (rc = scratch_grow(m, S.kr.temp, std::max(t_keys, t_nodes), what, st)))
             return rc;
-        tcap = S.temp.cap;
+        size_t tcap = S.kr.temp.cap;
         u64 *nkey = S.nkey[0].as<u64>(), *nrec = S.nrec[0].as<u64>();
         GEM_CUDA(m, cudaMemsetAsync(nkey, 0xFF, nnode * 8, st)); // OCT_EMPTY: unused group slots sort last
         if (ngp) {
             GEM_CUDA(m, cudaMemsetAsync(S.dense.p, 0, (size_t)hc.dense * 4, st));
             GEM_LAUNCH(m, GEM_PROF_OTHER, k_oct_group_keys<<<blocks_for((size_t)nleaf, 256, 1 << 30), 256, 0, st>>>(leaf, nleaf, cnt, off, sidx, level, S.ghead.as<int>(),
                                                                                                                     S.gid.as<int>(), S.key2[0].as<u64>(), ctr));
-            GEM_CUDA(m, cub::DeviceRadixSort::SortKeys(S.temp.p, tcap, S.key2[0].as<u64>(), S.key2[1].as<u64>(), (int)ngp, 0, 32 + gbits, st));
+            GEM_CUDA(m, cub::DeviceRadixSort::SortKeys(S.kr.temp.p, tcap, S.key2[0].as<u64>(), S.key2[1].as<u64>(), (int)ngp, 0, 32 + gbits, st));
             // every subtree up to level OCT_SMEM_LEVEL is simulated in shared memory sized for the largest such group
             const int smem_words = (int)oct_dense_size(std::min(hc.max_level, OCT_SMEM_LEVEL));
             const size_t smem = (size_t)smem_words * sizeof(uint32_t);
@@ -1891,7 +1946,7 @@ int gem_color_octree(gem_map *m, const void *points32_device, int n, double reso
         for (int k = 0; k <= 16; k++)
             GEM_LAUNCH(m, GEM_PROF_OTHER, k_oct_upper<<<blocks_for((size_t)nleaf, 256, 1 << 30), 256, 0, st>>>(leaf, nleaf, level, k, P, val, nkey, nrec, ctr));
         GEM_CUDA(m, cudaGetLastError());
-        GEM_CUDA(m, cub::DeviceRadixSort::SortPairs(S.temp.p, tcap, nkey, S.nkey[1].as<u64>(), nrec, S.nrec[1].as<u64>(), (int)nnode, 0, 53, st));
+        GEM_CUDA(m, cub::DeviceRadixSort::SortPairs(S.kr.temp.p, tcap, nkey, S.nkey[1].as<u64>(), nrec, S.nrec[1].as<u64>(), (int)nnode, 0, 53, st));
         GEM_CUDA(m, cudaMemcpyAsync(&hc, ctr, sizeof hc, cudaMemcpyDeviceToHost, st));
         GEM_CUDA(m, cudaStreamSynchronize(st));
     }
@@ -1928,7 +1983,6 @@ static bool cost_window_ok(const gem_costmap_window *w)
 {
     return w && cost_sizes_ok(w->size_x, w->size_y) && std::isfinite(w->resolution) && w->resolution > 0.0;
 }
-static int cost_grow(gem_map *m, size_t bytes) { return scratch_grow(m, m->cost_scratch, bytes, "costmap scratch"); }
 // the last-writer scatter of both mark calls (pass 1, pass 2), then the marks back to the host
 extern "C++" {
 template <class Src> static int cost_mark(gem_map *m, const Src &src, long long nchunks, const gem_costmap_window *w, unsigned char *cost,
@@ -1936,7 +1990,7 @@ template <class Src> static int cost_mark(gem_map *m, const Src &src, long long 
 {
     const int ncells = w->size_x * w->size_y;
     int rc;
-    if ((rc = cost_grow(m, (size_t)ncells * sizeof(int)))) return rc;
+    if ((rc = scratch_grow(m, m->cost_scratch, (size_t)ncells * sizeof(int), "costmap scratch", m->stream))) return rc;
     if (!m->cost_acc && (rc = dev_alloc(m, &m->cost_acc, 1))) return rc;
     const CostWindow cw{w->origin_x, w->origin_y, w->resolution, w->size_x, w->size_y};
     CostMarksDev init{0, 0, cm_key(INFINITY), cm_key(INFINITY), cm_key(-INFINITY), cm_key(-INFINITY)};
@@ -1966,18 +2020,11 @@ int gem_costmap_mark_map(gem_map *m, int source, const gem_costmap_window *w, do
     if (!m || !cost_device || !out || (source != GEM_GRID_SHOWN && source != GEM_GRID_SNAPSHOT))
         return fail(m, GEM_ERR_INVALID, "gem_costmap_mark_map: bad argument");
     if (!cost_window_ok(w)) return fail(m, GEM_ERR_INVALID, "gem_costmap_mark_map: bad window");
-    if (m->geom.tiled) return fail(m, GEM_ERR_INVALID, "gem_costmap_mark_map: not available on tiled handles");
     Lock lk(m->mu);
     SetDev sd(m->dev);
-    if (source == GEM_GRID_SNAPSHOT && !m->prev_valid)
-        return fail(m, GEM_ERR_INVALID, "gem_costmap_mark_map: no snapshot (call gem_snapshot_shown first)");
-    int rc = flush_for_observer(m);
-    if (rc) return rc;
     CostGridSrc src;
-    const MapGeom &g = source == GEM_GRID_SHOWN ? m->geom : m->prev_geom;
-    src.g.s = source == GEM_GRID_SHOWN ? live_cells(m->ml) : snapshot_cells(m->prev_ev, m->prev_ci, m->prev_tr);
-    src.g.f = grid_frame(m, g.cx, g.cy, g.sx, g.sy);
-    src.g.out = nullptr;
+    const int rc = grid_source(m, source, "gem_costmap_mark_map", &src.g);
+    if (rc) return rc;
     src.thresh = travers_thresh;
     src.mark_unknown = mark_unknown ? 1 : 0;
     src.nch = (m->L + 31) / 32;
@@ -2012,7 +2059,7 @@ int gem_costmap_update_origin(gem_map *m, gem_costmap_window *w, double new_orig
     SetDev sd(m->dev);
     const size_t ncells = (size_t)w->size_x * w->size_y;
     int rc;
-    if ((rc = cost_grow(m, ncells))) return rc;
+    if ((rc = scratch_grow(m, m->cost_scratch, ncells, "costmap scratch", m->stream))) return rc;
     // the copy, then the gather of k_costmap_roll, both ordered on the stream
     GEM_CUDA(m, cudaMemcpyAsync(m->cost_scratch.p, cost_device, ncells, cudaMemcpyDefault, m->stream));
     // |cell_ox| >= size_x leaves nothing of the old grid: clamp, so that the kernel's index sums cannot overflow
@@ -2133,12 +2180,12 @@ int gem_costmap_inflate(gem_map *m, const gem_costmap_window *w, const gem_costm
     // stale before `tab` may be replaced, and a replaced key buffer stays marked until its clearing memset is enqueued.
     if (!same) S.r = -1;
     void *old_key = S.key.p;
-    int rc = scratch_grow(m, S.key, ncells * 8, "gem_costmap_inflate");
+    int rc = scratch_grow(m, S.key, ncells * 8, "gem_costmap_inflate", m->stream);
     if (S.key.p != old_key) S.key_dirty = true;
-    if (rc || (rc = scratch_grow(m, S.pops, ncells * 8, "gem_costmap_inflate")) ||
-        (rc = scratch_grow(m, S.tab, tab_bytes, "gem_costmap_inflate")) ||
-        (rc = scratch_grow(m, S.gstart, ((size_t)nbins + 1) * sizeof(int), "gem_costmap_inflate")) ||
-        (rc = scratch_grow(m, S.blk, (size_t)S.blocks * sizeof(int), "gem_costmap_inflate")))
+    if (rc || (rc = scratch_grow(m, S.pops, ncells * 8, "gem_costmap_inflate", m->stream)) ||
+        (rc = scratch_grow(m, S.tab, tab_bytes, "gem_costmap_inflate", m->stream)) ||
+        (rc = scratch_grow(m, S.gstart, ((size_t)nbins + 1) * sizeof(int), "gem_costmap_inflate", m->stream)) ||
+        (rc = scratch_grow(m, S.blk, (size_t)S.blocks * sizeof(int), "gem_costmap_inflate", m->stream)))
         return rc;
     if (S.key_dirty) {
         GEM_CUDA(m, cudaMemsetAsync(S.key.p, 0xFF, S.key.cap, m->stream)); // every cell unseen
@@ -2177,9 +2224,8 @@ int gem_voxel_grid(gem_map *m, const void *xyzi_device, int n, const gem_voxel_g
         if (!std::isfinite(p->leaf_size[a]) || !(p->leaf_size[a] > 0.0f))
             return fail(m, GEM_ERR_INVALID, "gem_voxel_grid: every leaf size must be finite and positive");
     // V9: input and output ranges may not overlap (chained calls alternate between two buffers)
-    const uintptr_t i0 = (uintptr_t)xyzi_device, i1 = i0 + (size_t)n * sizeof(float4);
-    const uintptr_t o0 = (uintptr_t)out_xyzi_device, o1 = o0 + (size_t)capacity * sizeof(float4);
-    if (n > 0 && capacity > 0 && i0 < o1 && o0 < i1) return fail(m, GEM_ERR_INVALID, "gem_voxel_grid: the input and output ranges overlap");
+    if (ranges_meet(xyzi_device, (size_t)n * sizeof(float4), out_xyzi_device, (size_t)capacity * sizeof(float4)))
+        return fail(m, GEM_ERR_INVALID, "gem_voxel_grid: the input and output ranges overlap");
     Lock lk(m->mu);
     SetDev sd(m->dev);
     gem_voxel_grid_info r{};
@@ -2199,19 +2245,10 @@ int gem_voxel_grid(gem_map *m, const void *xyzi_device, int n, const gem_voxel_g
     const size_t N = (size_t)n;
     cudaStream_t st = m->stream;
     VoxScratch &S = m->vox;
-    // every buffer is sized before the first write (the sort's temporary for the widest key), so that a failed growth
-    // writes nothing
-    size_t t_sort = 0, t_rle = 0, t_scan = 0;
-    GEM_CUDA(m, cub::DeviceRadixSort::SortPairs(nullptr, t_sort, (u64 *)nullptr, (u64 *)nullptr, (int *)nullptr, (int *)nullptr, n, 0, 64, st));
-    GEM_CUDA(m, cub::DeviceRunLengthEncode::Encode(nullptr, t_rle, (u64 *)nullptr, (u64 *)nullptr, (int *)nullptr, (int *)nullptr, n, st));
-    GEM_CUDA(m, cub::DeviceScan::ExclusiveSum(nullptr, t_scan, (int *)nullptr, (int *)nullptr, n, st));
+    // every buffer is sized before the first write, so that a failed growth writes nothing
     const char *what = "gem_voxel_grid";
     int rc;
-    if ((rc = scratch_grow(m, S.key[0], N * 8, what)) || (rc = scratch_grow(m, S.key[1], N * 8, what)) ||
-        (rc = scratch_grow(m, S.idx[0], N * 4, what)) || (rc = scratch_grow(m, S.idx[1], N * 4, what)) ||
-        (rc = scratch_grow(m, S.cnt, N * 4, what)) || (rc = scratch_grow(m, S.off, N * 4, what)) ||
-        (rc = scratch_grow(m, S.temp, std::max(t_sort, std::max(t_rle, t_scan)), what)) || (rc = scratch_grow(m, S.acc, sizeof(VoxAcc), what)))
-        return rc;
+    if ((rc = key_runs_grow(m, S.kr, n, 0, what)) || (rc = scratch_grow(m, S.acc, sizeof(VoxAcc), what, st))) return rc;
     const float4 *in = static_cast<const float4 *>(xyzi_device);
     float4 *out = static_cast<float4 *>(out_xyzi_device);
     VoxAcc *acc = S.acc.as<VoxAcc>();
@@ -2271,20 +2308,13 @@ int gem_voxel_grid(gem_map *m, const void *xyzi_device, int n, const gem_voxel_g
     G.cut_key = G.div01 * div[2]; // one past the largest voxel key: the cut points' run sorts last
     int bits = 1;
     while ((1ull << bits) <= G.cut_key) bits++;
-    u64 *key0 = S.key[0].as<u64>(), *key1 = S.key[1].as<u64>();
-    int *idx0 = S.idx[0].as<int>(), *idx1 = S.idx[1].as<int>(), *cnt = S.cnt.as<int>(), *off = S.off.as<int>();
-    size_t tcap = S.temp.cap;
-    // the run-length encoding writes nruns <= n counts; the scan runs over all n, so the rest must be defined
-    GEM_CUDA(m, cudaMemsetAsync(cnt, 0, N * sizeof(int), st));
-    GEM_LAUNCH(m, GEM_PROF_OTHER, k_vox_keys<<<(unsigned)((N + VOX_BLOCK - 1) / VOX_BLOCK), VOX_BLOCK, 0, st>>>(in, n, P, G, key0, idx0));
+    GEM_LAUNCH(m, GEM_PROF_OTHER, k_vox_keys<<<(unsigned)((N + VOX_BLOCK - 1) / VOX_BLOCK), VOX_BLOCK, 0, st>>>(in, n, P, G, S.kr.key[0].as<u64>(), S.kr.idx[0].as<int>()));
     GEM_CUDA(m, cudaGetLastError());
     // V7: the stable sort keeps each voxel's points in input order
-    GEM_CUDA(m, cub::DeviceRadixSort::SortPairs(S.temp.p, tcap, key0, key1, idx0, idx1, n, 0, bits, st));
-    GEM_CUDA(m, cub::DeviceRunLengthEncode::Encode(S.temp.p, tcap, key1, key0, cnt, &acc->nruns, n, st));
-    GEM_CUDA(m, cub::DeviceScan::ExclusiveSum(S.temp.p, tcap, cnt, off, n, st));
+    if ((rc = key_runs_enqueue(m, S.kr, n, bits, S.kr.key[0].as<u64>(), &acc->nruns))) return rc;
     const int drop = h.used < n ? 1 : 0;
     GEM_LAUNCH(m, GEM_PROF_OTHER, k_vox_centroids<<<(unsigned)(((size_t)h.used + VOX_BLOCK - 1) / VOX_BLOCK), VOX_BLOCK, 0, st>>>(
-                                      in, idx1, cnt, off, acc, drop, out, capacity));
+                                      in, S.kr.idx[1].as<int>(), S.kr.cnt.as<int>(), S.kr.off.as<int>(), acc, drop, out, capacity));
     GEM_CUDA(m, cudaGetLastError());
     // synchronisation 2: the voxel count
     GEM_CUDA(m, cudaMemcpyAsync(&h.nruns, &acc->nruns, sizeof(int), cudaMemcpyDeviceToHost, st));
@@ -2306,9 +2336,8 @@ int gem_mls_upsample(gem_map *m, const void *points32_device, int n, const gem_m
     if (p->upsampling != GEM_MLS_NONE && p->upsampling != GEM_MLS_RANDOM_UNIFORM_DENSITY)
         return fail(m, GEM_ERR_INVALID, "gem_mls_upsample: unknown upsampling method");
     if (p->point_density < 0) return fail(m, GEM_ERR_INVALID, "gem_mls_upsample: point_density < 0");
-    const uintptr_t i0 = (uintptr_t)points32_device, i1 = i0 + (size_t)n * 32;
-    const uintptr_t o0 = (uintptr_t)out_points32_device, o1 = o0 + (size_t)capacity * 32;
-    if (n > 0 && capacity > 0 && i0 < o1 && o0 < i1) return fail(m, GEM_ERR_INVALID, "gem_mls_upsample: the input and output ranges overlap");
+    if (ranges_meet(points32_device, (size_t)n * 32, out_points32_device, (size_t)capacity * 32))
+        return fail(m, GEM_ERR_INVALID, "gem_mls_upsample: the input and output ranges overlap");
     Lock lk(m->mu);
     SetDev sd(m->dev);
     gem_mls_info r{};
@@ -2336,47 +2365,36 @@ int gem_mls_upsample(gem_map *m, const void *points32_device, int n, const gem_m
     cudaStream_t st = m->stream;
     MlsScratch &S = m->mls;
     // every buffer the first synchronisation needs is sized before the first launch, so that a failed growth writes nothing
-    size_t t_sort = 0, t_rle = 0, t_scan = 0, t_scan64 = 0;
-    GEM_CUDA(m, cub::DeviceRadixSort::SortPairs(nullptr, t_sort, (u64 *)nullptr, (u64 *)nullptr, (int *)nullptr, (int *)nullptr, n, 0, 64, st));
-    GEM_CUDA(m, cub::DeviceRunLengthEncode::Encode(nullptr, t_rle, (u64 *)nullptr, (u64 *)nullptr, (int *)nullptr, (int *)nullptr, n, st));
-    GEM_CUDA(m, cub::DeviceScan::ExclusiveSum(nullptr, t_scan, (int *)nullptr, (int *)nullptr, n, st));
+    size_t t_scan64 = 0;
     GEM_CUDA(m, cub::DeviceScan::ExclusiveSum(nullptr, t_scan64, (long long *)nullptr, (long long *)nullptr, n, st));
     const char *what = "gem_mls_upsample";
     int rc;
-    if ((rc = scratch_grow(m, S.key[0], N * 8, what)) || (rc = scratch_grow(m, S.key[1], N * 8, what)) ||
-        (rc = scratch_grow(m, S.idx[0], N * 4, what)) || (rc = scratch_grow(m, S.idx[1], N * 4, what)) ||
-        (rc = scratch_grow(m, S.spts, N * 16, what)) || (rc = scratch_grow(m, S.ukey, N * 8, what)) ||
-        (rc = scratch_grow(m, S.ucnt, N * 4, what)) || (rc = scratch_grow(m, S.uoff, N * 4, what)) ||
-        (rc = scratch_grow(m, S.nbr, N * 4, what)) || (rc = scratch_grow(m, S.ocnt, N * 8, what)) ||
-        (rc = scratch_grow(m, S.ooff, N * 8, what)) || (rc = scratch_grow(m, S.longs, N * 4, what)) ||
-        (rc = scratch_grow(m, S.temp, std::max(std::max(t_sort, t_rle), std::max(t_scan, t_scan64)), what)) ||
-        (rc = scratch_grow(m, S.acc, sizeof(MlsAcc), what)))
+    if ((rc = key_runs_grow(m, S.kr, n, t_scan64, what)) || (rc = scratch_grow(m, S.spts, N * 16, what, st)) ||
+        (rc = scratch_grow(m, S.ukey, N * 8, what, st)) || (rc = scratch_grow(m, S.nbr, N * 4, what, st)) ||
+        (rc = scratch_grow(m, S.ocnt, N * 8, what, st)) || (rc = scratch_grow(m, S.ooff, N * 8, what, st)) ||
+        (rc = scratch_grow(m, S.longs, N * 4, what, st)) || (rc = scratch_grow(m, S.acc, sizeof(MlsAcc), what, st)))
         return rc;
     const float4 *in = static_cast<const float4 *>(points32_device);
     float4 *out = static_cast<float4 *>(out_points32_device);
     MlsAcc *acc = S.acc.as<MlsAcc>();
-    u64 *key0 = S.key[0].as<u64>(), *key1 = S.key[1].as<u64>(), *ukey = S.ukey.as<u64>();
-    int *idx0 = S.idx[0].as<int>(), *idx1 = S.idx[1].as<int>(), *ucnt = S.ucnt.as<int>(), *uoff = S.uoff.as<int>();
+    u64 *ukey = S.ukey.as<u64>();
+    int *idx1 = S.kr.idx[1].as<int>(), *ucnt = S.kr.cnt.as<int>(), *uoff = S.kr.off.as<int>();
     int *nbr = S.nbr.as<int>(), *longs = S.longs.as<int>();
     long long *ocnt = S.ocnt.as<long long>(), *ooff = S.ooff.as<long long>();
     float4 *spts = S.spts.as<float4>();
-    size_t tcap = S.temp.cap;
     MlsAcc h{};
     h.mn[0] = h.mn[1] = h.mn[2] = 0xffffffffu;
     GEM_CUDA(m, cudaMemcpyAsync(acc, &h, sizeof h, cudaMemcpyHostToDevice, st));
-    // the run-length encoding writes nruns <= n counts; the scan runs over all n, so the rest must be defined
-    GEM_CUDA(m, cudaMemsetAsync(ucnt, 0, N * sizeof(int), st));
     const unsigned gb = (unsigned)((N + VOX_BLOCK - 1) / VOX_BLOCK), gq = (unsigned)((N + MLS_WARPS - 1) / MLS_WARPS);
     GEM_LAUNCH(m, GEM_PROF_OTHER, k_mls_bounds<<<blocks_for(N, VOX_BLOCK, NUM_SMS * 8), VOX_BLOCK, 0, st>>>(in, n, acc));
-    GEM_LAUNCH(m, GEM_PROF_OTHER, k_mls_keys<<<gb, VOX_BLOCK, 0, st>>>(in, n, P, acc, key0, idx0));
+    GEM_LAUNCH(m, GEM_PROF_OTHER, k_mls_keys<<<gb, VOX_BLOCK, 0, st>>>(in, n, P, acc, S.kr.key[0].as<u64>(), S.kr.idx[0].as<int>()));
     GEM_CUDA(m, cudaGetLastError());
-    GEM_CUDA(m, cub::DeviceRadixSort::SortPairs(S.temp.p, tcap, key0, key1, idx0, idx1, n, 0, 64, st));
-    GEM_CUDA(m, cub::DeviceRunLengthEncode::Encode(S.temp.p, tcap, key1, ukey, ucnt, &acc->nruns, n, st));
-    GEM_CUDA(m, cub::DeviceScan::ExclusiveSum(S.temp.p, tcap, ucnt, uoff, n, st));
+    if ((rc = key_runs_enqueue(m, S.kr, n, 64, ukey, &acc->nruns))) return rc;
     GEM_LAUNCH(m, GEM_PROF_OTHER, k_mls_stage<<<gb, VOX_BLOCK, 0, st>>>(in, n, idx1, spts));
     GEM_LAUNCH(m, GEM_PROF_OTHER, k_mls_count<<<gq, MLS_BLOCK, 0, st>>>(in, n, P, acc, spts, ukey, uoff, ucnt, nbr, ocnt, longs));
     GEM_CUDA(m, cudaGetLastError());
-    GEM_CUDA(m, cub::DeviceScan::ExclusiveSum(S.temp.p, tcap, ocnt, ooff, n, st));
+    size_t tcap = S.kr.temp.cap;
+    GEM_CUDA(m, cub::DeviceScan::ExclusiveSum(S.kr.temp.p, tcap, ocnt, ooff, n, st));
     // synchronisation 1: the output count (last offset + last count), the longest list and the number of long lists
     long long tail[2] = {0, 0};
     GEM_CUDA(m, cudaMemcpyAsync(&tail[0], ooff + (N - 1), sizeof(long long), cudaMemcpyDeviceToHost, st));
@@ -2394,7 +2412,7 @@ int gem_mls_upsample(gem_map *m, const void *points32_device, int n, const gem_m
         w = std::min(w, (size_t)NUM_SMS * 16);
         w = std::min(w, ((size_t)h.nlong + MLS_WARPS - 1) / MLS_WARPS * MLS_WARPS);
         lwarps = (int)w;
-        if ((rc = scratch_grow(m, S.lkeys, w * per, what))) return rc;
+        if ((rc = scratch_grow(m, S.lkeys, w * per, what, st))) return rc;
     }
     if (capacity == 0) { // a size query stops here: the fits are not run
         r.processed = h.processed;
@@ -2812,7 +2830,7 @@ int gem_refuse_submaps(gem_map *m, void *new_points32, int *n_new, void *old_poi
     Lock lk(m->mu);
     SetDev sd(m->dev);
     const int nn = *n_new, no = *n_old;
-    int rc = scratch_grow(m, m->refuse, pair_bytes(nn, no), "gem_refuse_submaps");
+    int rc = scratch_grow(m, m->refuse, pair_bytes(nn, no), "gem_refuse_submaps", m->stream);
     if (rc) return rc;
     const PairScratch s = pair_layout(m->refuse.p, nn, no);
     int h[4] = {0, nn, no, 0}; // fused, n_new, n_old
@@ -2840,19 +2858,6 @@ static int gmap_ready(gem_map *m)
     GlobalStore &g = m->gmap;
     if (!g.stream) GEM_CUDA(m, cudaStreamCreateWithFlags(&g.stream, cudaStreamNonBlocking));
     if (!g.ev) GEM_CUDA(m, cudaEventCreateWithFlags(&g.ev, cudaEventDisableTiming));
-    return GEM_OK;
-}
-// a scratch buffer of the stack: like scratch_grow, but drained on the stack's stream
-static int gmap_grow(gem_map *m, OctBuf &b, size_t bytes, const char *what)
-{
-    if (b.cap >= bytes) return GEM_OK;
-    bytes = std::max(std::max(bytes, 2 * b.cap), (size_t)4096);
-    void *q = nullptr;
-    const cudaError_t e = cudaMalloc(&q, bytes);
-    if (e != cudaSuccess) { cudaGetLastError(); return fail(m, GEM_ERR_NOMEM, std::string(what) + ": cudaMalloc: " + cudaGetErrorString(e)); }
-    if (b.p) { cudaStreamSynchronize(m->gmap.stream); cudaFree(b.p); }
-    b.p = q;
-    b.cap = bytes;
     return GEM_OK;
 }
 // room for `need` records in both arena buffers (capacity doubles from 1024).  Both are allocated before anything is
@@ -2900,7 +2905,7 @@ static int gmap_reserve_meta(gem_map *m, int K)
     if (K <= g.meta_submaps) return GEM_OK;
     int cap = std::max(g.meta_submaps * 2, 64);
     while (cap < K) cap *= 2;
-    const int rc = gmap_grow(m, g.meta, gmap_meta_ints(cap) * 4 + (size_t)cap * sizeof(Rigid), "global map");
+    const int rc = scratch_grow(m, g.meta, gmap_meta_ints(cap) * 4 + (size_t)cap * sizeof(Rigid), "global map", g.stream);
     if (rc == GEM_OK) g.meta_submaps = cap;
     return rc;
 }
@@ -2928,7 +2933,7 @@ int gem_global_map_reserve(gem_map *m, long long records, int submaps)
     if ((rc = gmap_ready(m)) || (rc = gmap_reserve_records(m, records)) || (rc = gmap_reserve_meta(m, submaps))) return rc;
     // one pair of the largest submaps the arena can hold
     const int big = (int)std::min<long long>(records, g.cap);
-    return gmap_grow(m, g.pair, pair_bytes(big, big), "gem_global_map_reserve");
+    return scratch_grow(m, g.pair, pair_bytes(big, big), "gem_global_map_reserve", g.stream);
 }
 
 int gem_global_map_push(gem_map *m, const void *records_device, int n, const float pose[16])
@@ -2986,7 +2991,7 @@ int gem_global_map_update(gem_map *m, const float *opt_poses, int k, double reso
     gem_gmap::pair_schedule(g.centres.data(), Kp, radius, pairs);
     int big = 0;
     for (int i = 0; i < Kp; i++) big = std::max(big, g.cnt[i]);
-    if ((rc = gmap_reserve_meta(m, std::max(K, 1))) || (rc = gmap_grow(m, g.pair, pair_bytes(big, big), "gem_global_map_update"))) return rc;
+    if ((rc = gmap_reserve_meta(m, std::max(K, 1))) || (rc = scratch_grow(m, g.pair, pair_bytes(big, big), "gem_global_map_update", g.stream))) return rc;
     int *d_cnt = g.meta.as<int>(), *d_off = d_cnt + K, *d_off_new = d_off + K + 1, *d_ctr = d_off_new + K + 1;
     Rigid *d_T = (Rigid *)(g.meta.as<int>() + gmap_meta_ints(g.meta_submaps));
     std::vector<int> h((size_t)3 * K + 6, 0);
@@ -3220,12 +3225,6 @@ int gem_pointcloud2_mapping(const gem_pointcloud2 *layout, unsigned long long da
     return why ? fail(nullptr, GEM_ERR_INVALID, std::string("gem_pointcloud2_mapping: ") + why) : GEM_OK;
 }
 
-static bool ranges_meet(const void *a, size_t na, const void *b, size_t nb)
-{
-    const uintptr_t a0 = (uintptr_t)a, b0 = (uintptr_t)b;
-    return na > 0 && nb > 0 && a0 < b0 + nb && b0 < a0 + na;
-}
-
 static int launch_decode(gem_map *m, const gem_pointcloud2 *layout, const gem_pc2_mapping &mp, const void *data, void *xyzi_out)
 {
     if (mp.points == 0) return GEM_OK;
@@ -3314,9 +3313,9 @@ int gem_add_pointcloud2_host_async(gem_map *m, const gem_pointcloud2 *layout, co
     if (m->pc2_raw[b].cap < mp.bytes || m->pc2_img[b].cap < img_bytes || m->pc2_bgr.cap < bgr_bytes) {
         GEM_CUDA(m, cudaStreamSynchronize(m->copy_stream));
         GEM_CUDA(m, cudaStreamSynchronize(m->stream));
-        if ((rc = scratch_grow(m, m->pc2_raw[b], mp.bytes, "gem_add_pointcloud2_host_async")) ||
-            (rc = scratch_grow(m, m->pc2_img[b], img_bytes, "gem_add_pointcloud2_host_async")) ||
-            (rc = scratch_grow(m, m->pc2_bgr, bgr_bytes, "gem_add_pointcloud2_host_async")))
+        if ((rc = scratch_grow(m, m->pc2_raw[b], mp.bytes, "gem_add_pointcloud2_host_async", m->stream)) ||
+            (rc = scratch_grow(m, m->pc2_img[b], img_bytes, "gem_add_pointcloud2_host_async", m->stream)) ||
+            (rc = scratch_grow(m, m->pc2_bgr, bgr_bytes, "gem_add_pointcloud2_host_async", m->stream)))
             return rc;
     }
     m->async_calls++;
@@ -3381,8 +3380,8 @@ int gem_pcd_format(gem_map *m, const void *points32_device, int n, int flags, vo
         size_t t_scan = 0;
         GEM_CUDA(m, cub::DeviceScan::InclusiveSum(nullptr, t_scan, (long long *)nullptr, (long long *)nullptr, (int)tiles, st));
         int rc;
-        if ((rc = scratch_grow(m, S.bytes, tiles * 8, what)) || (rc = scratch_grow(m, S.ends, tiles * 8, what)) ||
-            (rc = scratch_grow(m, S.temp, t_scan, what)))
+        if ((rc = scratch_grow(m, S.bytes, tiles * 8, what, m->stream)) || (rc = scratch_grow(m, S.ends, tiles * 8, what, m->stream)) ||
+            (rc = scratch_grow(m, S.temp, t_scan, what, m->stream)))
             return rc;
         long long *tb = S.bytes.as<long long>(), *te = S.ends.as<long long>();
         size_t tcap = S.temp.cap;
@@ -3438,7 +3437,7 @@ static int ros_stage(gem_map *m, unsigned char *out, long long size, bool pinned
 {
     *dst = out;
     if (!pinned) return GEM_OK;
-    const int rc = scratch_grow(m, m->ros_stage, (size_t)size + 16, "gem_ros staging");
+    const int rc = scratch_grow(m, m->ros_stage, (size_t)size + 16, "gem_ros staging", m->stream);
     if (rc) return rc;
     *dst = m->ros_stage.as<unsigned char>() + ((uintptr_t)out & 15u);
     return GEM_OK;
@@ -3454,7 +3453,7 @@ static int ros_unstage(gem_map *m, unsigned char *out, const unsigned char *dst,
 // device buffer is reused in stream order.
 static int ros_put_framing(gem_map *m, const gem_ros::Framing &f, unsigned char *out)
 {
-    const int rc = scratch_grow(m, m->ros_framing, f.bytes.size(), "gem_ros framing");
+    const int rc = scratch_grow(m, m->ros_framing, f.bytes.size(), "gem_ros framing", m->stream);
     if (rc) return rc;
     GEM_CUDA(m, cudaMemcpyAsync(m->ros_framing.p, f.bytes.data(), f.bytes.size(), cudaMemcpyHostToDevice, m->stream));
     RosSegs s{};
