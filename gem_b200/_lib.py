@@ -142,6 +142,12 @@ class GemRosPart(C.Structure):
     _fields_ = [("points32", C.c_void_p), ("n", C.c_longlong)]
 
 
+class GemCostmapPublisher(C.Structure):
+    _fields_ = [("always_send_full", C.c_int), ("saved", C.c_int), ("resolution", C.c_float), ("size_x", C.c_int),
+                ("size_y", C.c_int), ("origin_x", C.c_double), ("origin_y", C.c_double), ("x0", C.c_int), ("xn", C.c_int),
+                ("y0", C.c_int), ("yn", C.c_int)]
+
+
 COST_FREE, COST_LETHAL, COST_UNKNOWN = 0, 254, 255           # GEM_COST_*
 INFLATE_MAX_CELLS = 4094                                     # GEM_INFLATE_MAX_CELLS
 COSTMAP_MODES = {"max": 0, "overwrite": 1}                  # GEM_COSTMAP_MAX / GEM_COSTMAP_OVERWRITE
@@ -151,6 +157,7 @@ MLS_UPSAMPLING = {"none": 0, "random_uniform_density": 1}  # GEM_MLS_*
 POINTFIELD_TYPES = {"int8": 1, "uint8": 2, "int16": 3, "uint16": 4, "int32": 5, "uint32": 6, "float32": 7, "float64": 8}
 PC2_FIELDS = ["x", "y", "z", "rgb", "intensity", "covariance", "travers"]
 PCD_BINARY, PCD_RGB_UINT32 = 1, 2   # GEM_PCD_*
+COSTMAP_PUB_KINDS = {0: "none", 1: "full", 2: "update"}   # GEM_COSTMAP_PUB_*
 PCD_LINE_MAX, PCD_HEADER_MAX = 105, 512   # GEM_PCD_LINE_MAX, GEM_PCD_HEADER_MAX
 IMAGE_ENCODINGS = {"bgr8": 3, "rgb8": 3, "bgra8": 4, "rgba8": 4, "mono8": 1}   # the byte-permutation encodings: channels
 
@@ -251,6 +258,14 @@ SYMBOLS = {
     "gem_ros_cloud": (C.c_int, [_P, C.POINTER(GemRosHeader), C.POINTER(GemRosPart), C.c_int, C.c_int, _P, C.c_longlong,
                                 C.POINTER(C.c_longlong)]),
     "gem_ros_octomap": (C.c_int, [_P, C.POINTER(GemRosHeader), _P, C.c_longlong, C.POINTER(C.c_longlong)]),
+    "gem_costmap_publisher_init": (C.c_int, [C.POINTER(GemCostmapPublisher), C.c_int]),
+    "gem_costmap_publisher_bounds": (C.c_int, [C.POINTER(GemCostmapPublisher), C.c_int, C.c_int, C.c_int, C.c_int]),
+    "gem_ros_costmap": (C.c_int, [_P, C.POINTER(GemRosHeader), C.POINTER(GemCostmapWindow), _P, C.POINTER(GemCostmapPublisher),
+                                  C.c_int, _P, C.c_longlong, C.POINTER(C.c_longlong), _IP]),
+    "gem_ros_footprint": (C.c_int, [_P, C.POINTER(GemRosHeader), C.POINTER(C.c_double), C.c_int, C.c_double, C.c_double,
+                                    C.c_double, _P, C.c_longlong, C.POINTER(C.c_longlong)]),
+    "gem_costmap_footprint": (C.c_int, [_P, C.POINTER(GemCostmapWindow), C.POINTER(C.c_double), C.c_int, C.c_double, C.c_double,
+                                        C.c_double, _P, C.POINTER(GemCostmapMarks)]),
 }
 
 _lib = None

@@ -9,11 +9,19 @@ drift of the rolling window or the bounds-to-rect arithmetic.  The cell work is 
 
 GEM's global costmap also lists costmap_2d's InflationLayer after the point layer; `InflationLayer` holds its parameters
 and bounds state, and `Costmap.update(..., inflation=layer)` runs it as LayeredCostmap::updateMap does with the two
-plugins (DESIGN.md f14)."""
+plugins (DESIGN.md f14).
+
+What Costmap2DROS publishes, and ObstacleLayer's footprint clearing (DESIGN.md f17): `CostmapPublisher` is
+Costmap2DPublisher's decision between a full grid, an update and nothing, with the bytes written on the device;
+`Costmap.update(..., robot_yaw=, footprint=)` clears the footprint in the layer grid; `Costmap` keeps LayeredCostmap's
+getBounds rect and its initialized flag for the publisher."""
 from __future__ import annotations
 
 import math
 
+import ctypes as C
+
+from . import _lib
 from ._lib import COST_FREE, COST_LETHAL, COST_UNKNOWN  # noqa: F401
 
 FLT_MAX = 3.4028234663852886e38   # std::numeric_limits<float>::max(), as a double
@@ -50,6 +58,14 @@ def inscribed_radius(footprint, padding: float = 0.0) -> float:
         (x0, y0), (x1, y1) = pts[k], pts[(k + 1) % len(pts)]
         best = min(best, min(math.hypot(x0, y0), _distance_to_line(0.0, 0.0, x0, y0, x1, y1)))
     return best
+
+
+def transform_footprint(footprint, robot_x: float, robot_y: float, robot_yaw: float):
+    """footprint.cpp's transformFootprint: each vertex (fx, fy) at the pose as (x + (fx cos t - fy sin t), y + (fx sin t +
+    fy cos t)) in double, cos and sin from the host's libm.  The published footprint (W11) is these as float32."""
+    c, s = math.cos(float(robot_yaw)), math.sin(float(robot_yaw))
+    return [(float(robot_x) + (float(fx) * c - float(fy) * s), float(robot_y) + (float(fx) * s + float(fy) * c))
+            for fx, fy in footprint]
 
 
 def world_to_map_enforce_bounds(window, wx: float, wy: float):
@@ -95,6 +111,10 @@ class Costmap:
         self.fill = int(fill)
         dev = torch.device("cuda", emap._device_index())
         self.grid = torch.full((int(size_y), int(size_x)), self.fill, dtype=torch.uint8, device=dev)
+        # LayeredCostmap's getBounds rect (bx0, bxn, by0, byn) and initialized_: set by an update that reaches updateCosts;
+        # one that returns early leaves them, and a node feeds those stale bounds to the publisher again
+        self.bx0 = self.bxn = self.by0 = self.byn = 0
+        self.initialized = False
 
     def size_in_meters(self):
         """Costmap2D::getSizeInMetersX / Y: (size - 1 + 0.5) * resolution"""
@@ -115,16 +135,26 @@ class Costmap:
         """PointMapLayer::updateBounds into this grid"""
         return self.emap.costmap_mark_points(points, self.window, self.grid, travers_thresh)
 
-    def update(self, layer: "Costmap", robot_xy, mode: str, mark, inflation: "InflationLayer | None" = None):
+    def update(self, layer: "Costmap", robot_xy, mode: str, mark, inflation: "InflationLayer | None" = None,
+               robot_yaw: float | None = None, footprint=None):
         """LayeredCostmap::updateMap of this master grid with one layer: roll the master and the layer, let the layer
         mark (`mark(layer)` returns its marks, e.g. lambda l: l.mark_map(0.7)), turn the touch bounds into the rect,
         reset the rect to the master's fill and combine the layer into it ("max" for ElevationMapLayer, "overwrite" for
         PointMapLayer).  With `inflation`, that InflationLayer is the second plugin: its update_bounds follows the
-        layer's, and its update_costs follows the combine.  Returns (rect or None, marks)."""
+        layer's, and its update_costs follows the combine.  With `footprint` (the padded footprint's vertices) and
+        `robot_yaw`, the "max" layer clears it as ObstacleLayer does (DESIGN.md f17): the vertices widen the bounds and
+        the footprint's cells become FREE in the layer grid; PointMapLayer ("overwrite") has no footprint clearing, so a
+        footprint with it is refused.  Returns (rect or None, marks), the marks with the footprint's bounds merged in."""
         import torch
+        if footprint is not None and (mode != "max" or robot_yaw is None):
+            raise ValueError("update: footprint clearing needs mode \"max\" (ElevationMapLayer) and robot_yaw")
         self.roll(robot_xy)
         layer.roll(robot_xy)
         marks = mark(layer)
+        if footprint is not None:
+            fm = self.emap.costmap_footprint(layer.window, footprint, robot_xy[0], robot_xy[1], robot_yaw, layer.grid)
+            marks = dict(marks, min_x=min(marks["min_x"], fm["min_x"]), min_y=min(marks["min_y"], fm["min_y"]),
+                         max_x=max(marks["max_x"], fm["max_x"]), max_y=max(marks["max_y"], fm["max_y"]))
         if inflation is None:
             rect = update_rect(self.window, marks)
         else:
@@ -140,7 +170,33 @@ class Costmap:
         self.emap.costmap_combine(mode, layer.grid, self.grid, sx, sy, rect)
         if inflation is not None:
             inflation.update_costs(self, rect)
+        self.bx0, self.bxn, self.by0, self.byn = x0, xn, y0, yn
+        self.initialized = True
         return rect, marks
+
+
+class CostmapPublisher:
+    """Costmap2DPublisher (navigation 1.14; DESIGN.md f17 P1-P4) of one costmap: the saved window and the accumulated
+    bounds in a gem_costmap_publisher, the decision and the message bytes in the library.  The subscriber gate and the
+    publish timer stay with the caller: skipping `publish` is what the reference does without subscribers."""
+
+    def __init__(self, always_send_full: bool = False):
+        self.state = _lib.GemCostmapPublisher()
+        _lib.load().gem_costmap_publisher_init(C.byref(self.state), 1 if always_send_full else 0)
+
+    def bounds(self, x0: int, xn: int, y0: int, yn: int):
+        """Costmap2DPublisher::updateBounds: the rect merged into the accumulated bounds with min / max"""
+        _lib.load().gem_costmap_publisher_bounds(C.byref(self.state), int(x0), int(xn), int(y0), int(yn))
+
+    def update_bounds(self, costmap: Costmap):
+        """what Costmap2DROS::mapUpdateLoop feeds after every update: getBounds, once the costmap is initialised"""
+        if costmap.initialized:
+            self.bounds(costmap.bx0, costmap.bxn, costmap.by0, costmap.byn)
+
+    def publish(self, master: Costmap, header, out=None, force_full: bool = False):
+        """publishCostmap of the master grid (force_full: onNewSubscription's full grid, which leaves the bounds):
+        (kind, message) with kind "full", "update" or "none"; see ElevationMap.ros_costmap"""
+        return master.emap.ros_costmap(header, master.window, master.grid, self.state, force_full, out)
 
 
 class InflationLayer:

@@ -192,6 +192,7 @@ struct gem_map {
     PcdScratch pcd;                // gem_pcd_format
     DevBuf ros_framing;            // gem_ros_*: the framing bytes of the call, staged for k_ros_framing
     DevBuf ros_stage;              // gem_ros_* map messages for pinned outputs, written here and copied over in one DMA
+    DevBuf cost_cells;             // gem_costmap_footprint: the cell indices the host listed
     InflScratch infl;              // gem_costmap_inflate
     DevBuf refuse;                 // gem_refuse_submaps: one pair's scratch (pair_layout)
     GlobalStore gmap;              // gem_global_map_*
@@ -999,7 +1000,7 @@ int gem_destroy(gem_map *m)
                           &m->mls.ooff, &m->mls.longs, &m->mls.lkeys, &m->mls.acc, &m->pc2_raw[0],
                           &m->pc2_raw[1], &m->pc2_raw[2], &m->pc2_img[0], &m->pc2_img[1], &m->pc2_img[2], &m->pc2_bgr,
                           &m->pcd.bytes, &m->pcd.ends, &m->pcd.temp, &m->infl.key, &m->infl.pops, &m->infl.tab,
-                          &m->infl.gstart, &m->infl.blk, &m->ros_framing, &m->ros_stage, &m->refuse, &m->gmap.arena[0],
+                          &m->infl.gstart, &m->infl.blk, &m->ros_framing, &m->ros_stage, &m->cost_cells, &m->refuse, &m->gmap.arena[0],
                           &m->gmap.arena[1], &m->gmap.meta, &m->gmap.pair})
             if (b->p) cudaFree(b->p);
         if (m->gmap.stream) { cudaStreamSynchronize(m->gmap.stream); cudaStreamDestroy(m->gmap.stream); }
@@ -3409,13 +3410,13 @@ int gem_pcd_format(gem_map *m, const void *points32_device, int n, int flags, vo
 // the checks every gem_ros_* call makes first.  *pinned: out is page-locked host memory (the kernels may store to
 // device, managed and pinned memory; pageable host memory is refused, since a store to it from the device faults)
 static int ros_args(gem_map *m, const gem_ros_header *h, void *out, long long capacity, long long *bytes_out, const char *what,
-                    bool *pinned)
+                    bool *pinned, bool reads_map = true)
 {
     if (bytes_out) *bytes_out = 0;
     if (!m) return GEM_ERR_INVALID;
     if (!bytes_out || capacity < 0 || (capacity > 0 && !out)) return fail(m, GEM_ERR_INVALID, std::string(what) + ": bad argument");
     if (!gem_ros::header_ok(h)) return fail(m, GEM_ERR_INVALID, std::string(what) + ": NULL header or frame_id");
-    if (m->geom.tiled) return fail(m, GEM_ERR_INVALID, std::string(what) + ": not available on tiled handles");
+    if (reads_map && m->geom.tiled) return fail(m, GEM_ERR_INVALID, std::string(what) + ": not available on tiled handles");
     *pinned = false;
     if (out) {
         cudaPointerAttributes a{};
@@ -3609,6 +3610,139 @@ int gem_ros_octomap(gem_map *m, const gem_ros_header *h, void *out, long long ca
     if ((rc = ros_put_framing(m, f, o))) return rc;
     if (bytes) GEM_CUDA(m, cudaMemcpyAsync(o + f.payload_at[0], m->oct.nrec[1].p, (size_t)bytes, cudaMemcpyDefault, m->stream));
     *bytes_out = f.size;
+    return GEM_OK;
+}
+
+
+// ---- the costmap topics and footprint clearing (gem_rosfmt.h W9-W11 and P1-P4, gem_footprint.h F1-F4; f17) --------------
+int gem_costmap_publisher_init(gem_costmap_publisher *p, int always_send_full)
+{
+    if (!p) return GEM_ERR_INVALID;
+    gem_ros::costmap_publisher_init(*p, always_send_full);
+    return GEM_OK;
+}
+
+int gem_costmap_publisher_bounds(gem_costmap_publisher *p, int x0, int xn, int y0, int yn)
+{
+    if (!p) return GEM_ERR_INVALID;
+    gem_ros::costmap_publisher_bounds(*p, x0, xn, y0, yn);
+    return GEM_OK;
+}
+
+// a footprint and pose the f17 calls accept: n >= 0 (x, y) pairs, every value finite
+static bool footprint_ok(const double *spec_xy, int n, double rx, double ry, double yaw)
+{
+    if (n < 0 || (n > 0 && !spec_xy) || !std::isfinite(rx) || !std::isfinite(ry) || !std::isfinite(yaw)) return false;
+    for (int i = 0; i < 2 * n; i++)
+        if (!std::isfinite(spec_xy[i])) return false;
+    return true;
+}
+
+int gem_ros_costmap(gem_map *m, const gem_ros_header *h, const gem_costmap_window *w, const unsigned char *master_device,
+                    gem_costmap_publisher *p, int force_full, void *out, long long capacity, long long *bytes_out, int *kind_out)
+{
+    if (kind_out) *kind_out = GEM_COSTMAP_PUB_NONE;
+    bool pinned = false;
+    int rc = ros_args(m, h, out, capacity, bytes_out, "gem_ros_costmap", &pinned, false);
+    if (rc) return rc;
+    if (!kind_out || !p || !master_device || (force_full != 0 && force_full != 1))
+        return fail(m, GEM_ERR_INVALID, "gem_ros_costmap: bad argument");
+    if (!cost_window_ok(w)) return fail(m, GEM_ERR_INVALID, "gem_ros_costmap: bad window");
+    gem_ros::CostmapPlan d;
+    gem_ros::Framing f;
+    bool writes = false;
+    if (gem_ros::costmap_message(*h, *w, *p, force_full, !out, capacity, d, f, writes))
+        return fail(m, GEM_ERR_INVALID, "gem_ros_costmap: the accumulated bounds lie outside the grid");
+    *kind_out = d.kind;
+    if (!writes) { // a size query, or too small: nothing is written and the publisher stays as it was
+        *bytes_out = f.size;
+        return GEM_OK;
+    }
+    const size_t cells = (size_t)w->size_x * w->size_y;
+    if (f.size > 0 && ranges_meet(master_device, cells, out, (size_t)f.size))
+        return fail(m, GEM_ERR_INVALID, "gem_ros_costmap: the output overlaps the master grid");
+    if (d.kind != GEM_COSTMAP_PUB_NONE) {
+        Lock lk(m->mu);
+        SetDev sd(m->dev);
+        unsigned char *o = nullptr;
+        if ((rc = ros_stage(m, static_cast<unsigned char *>(out), f.size, pinned, &o)) || (rc = ros_put_framing(m, f, o))) return rc;
+        unsigned char *data = o + f.payload_at[0];
+        const long long n = f.payload_len[0];
+        if (n > 0) {
+            const long long nwords = ((long long)((uintptr_t)data & 15u) + n + 15) / 16;
+            GEM_LAUNCH(m, GEM_PROF_OTHER, k_ros_costmap<<<(unsigned)((nwords + 255) / 256), 256, 0, m->stream>>>(
+                                              master_device, w->size_x, d.x0, d.y0, d.width, n, data, nwords));
+            GEM_CUDA(m, cudaGetLastError());
+        }
+        if ((rc = ros_unstage(m, static_cast<unsigned char *>(out), o, f.size, pinned))) return rc;
+    }
+    gem_ros::costmap_commit(*p, *w, d, force_full);
+    *bytes_out = f.size;
+    return GEM_OK;
+}
+
+int gem_ros_footprint(gem_map *m, const gem_ros_header *h, const double *spec_xy, int n, double robot_x, double robot_y,
+                      double robot_yaw, void *out, long long capacity, long long *bytes_out)
+{
+    bool pinned = false;
+    int rc = ros_args(m, h, out, capacity, bytes_out, "gem_ros_footprint", &pinned, false);
+    if (rc) return rc;
+    if (!footprint_ok(spec_xy, n, robot_x, robot_y, robot_yaw))
+        return fail(m, GEM_ERR_INVALID, "gem_ros_footprint: n < 0, no footprint, or a value that is not finite");
+    std::vector<gem_fp::Point> pts;
+    gem_fp::transform(spec_xy, n, robot_x, robot_y, robot_yaw, pts);
+    std::vector<double> xy;
+    for (const gem_fp::Point &q : pts) {
+        xy.push_back(q.x);
+        xy.push_back(q.y);
+    }
+    gem_ros::Framing f;
+    if (gem_ros::polygon_stamped(*h, xy.data(), n, f)) return fail(m, GEM_ERR_INVALID, "gem_ros_footprint: a polygon of 2^32 bytes or more");
+    if (!out || capacity < f.size) {
+        *bytes_out = f.size;
+        return GEM_OK;
+    }
+    Lock lk(m->mu);
+    SetDev sd(m->dev);
+    if ((rc = ros_put_framing(m, f, static_cast<unsigned char *>(out)))) return rc;
+    *bytes_out = f.size;
+    return GEM_OK;
+}
+
+// ObstacleLayer::updateFootprint's bounds and updateCosts' setConvexPolygonCost(FREE_SPACE) on the layer grid.  The
+// reference fills at updateCosts; this fills at bounds time, which gives the same bytes: nothing reads the layer grid in
+// between, and with a vertex touched the bounds are never empty, so LayeredCostmap::updateMap always reaches updateCosts.
+int gem_costmap_footprint(gem_map *m, const gem_costmap_window *w, const double *spec_xy, int n, double robot_x, double robot_y,
+                          double robot_yaw, unsigned char *layer_device, gem_costmap_marks *out)
+{
+    if (!m || !layer_device || !out) return fail(m, GEM_ERR_INVALID, "gem_costmap_footprint: bad argument");
+    if (!cost_window_ok(w)) return fail(m, GEM_ERR_INVALID, "gem_costmap_footprint: bad window");
+    if (!footprint_ok(spec_xy, n, robot_x, robot_y, robot_yaw))
+        return fail(m, GEM_ERR_INVALID, "gem_costmap_footprint: n < 0, no footprint, or a value that is not finite");
+    std::vector<gem_fp::Point> pts;
+    std::vector<gem_fp::Cell> cells;
+    gem_fp::transform(spec_xy, n, robot_x, robot_y, robot_yaw, pts);
+    gem_costmap_marks r{0, 0, INFINITY, INFINITY, -INFINITY, -INFINITY};
+    for (const gem_fp::Point &q : pts) { // touch(), a zero reported as +0 (f8)
+        r.min_x = std::min(r.min_x, q.x + 0.0); r.min_y = std::min(r.min_y, q.y + 0.0);
+        r.max_x = std::max(r.max_x, q.x + 0.0); r.max_y = std::max(r.max_y, q.y + 0.0);
+    }
+    gem_fp::polygon_cells(w->origin_x, w->origin_y, w->resolution, w->size_x, w->size_y, pts, cells);
+    std::vector<int> idx(cells.size());
+    for (size_t i = 0; i < cells.size(); i++) idx[i] = (int)(cells[i].y * (unsigned)w->size_x + cells[i].x);
+    if (!idx.empty()) {
+        Lock lk(m->mu);
+        SetDev sd(m->dev);
+        int rc;
+        if ((rc = scratch_grow(m, m->cost_cells, idx.size() * sizeof(int), "costmap footprint cells", m->stream))) return rc;
+        // from pageable memory the copy returns once its source is staged, so idx may go when this call returns
+        GEM_CUDA(m, cudaMemcpyAsync(m->cost_cells.p, idx.data(), idx.size() * sizeof(int), cudaMemcpyHostToDevice, m->stream));
+        GEM_LAUNCH(m, GEM_PROF_OTHER, k_costmap_cells<<<(unsigned)((idx.size() + 255) / 256), 256, 0, m->stream>>>(
+                                          m->cost_cells.as<int>(), (int)idx.size(), layer_device, COST_FREE));
+        GEM_CUDA(m, cudaGetLastError());
+    }
+    r.marked = (long long)idx.size();
+    *out = r;
     return GEM_OK;
 }
 

@@ -12,6 +12,7 @@
 #include <stdint.h>
 #include <string.h>
 
+#include "gem_footprint.h"
 #include "gem_kernels.cuh"
 
 namespace gem {
@@ -23,18 +24,10 @@ struct CostWindow {
     int sx, sy;
 };
 
-// Costmap2D::worldToMap, in double: false if wx < origin_x || wy < origin_y; otherwise mx = (int)((wx - origin_x) / res)
-// (same for my), accepted iff mx < size_x && my < size_y.  DEFINED: a non-finite coordinate is rejected, and so is a
-// quotient >= 2^31, where the reference's cast is undefined.  (NaN fails `>=`; -inf is below the origin; +inf gives an
-// infinite quotient.)
+// Costmap2D::worldToMap (f8 item 4; gem_fp::world_to_map, shared with the host's footprint clearing)
 __device__ __forceinline__ bool cm_world_to_map(const CostWindow &w, double wx, double wy, int &mx, int &my)
 {
-    if (!(wx >= w.ox) || !(wy >= w.oy)) return false;
-    const double qx = (wx - w.ox) / w.res, qy = (wy - w.oy) / w.res;
-    if (!(qx < 2147483648.0) || !(qy < 2147483648.0)) return false;
-    mx = (int)qx;
-    my = (int)qy;
-    return mx < w.sx && my < w.sy;
+    return gem_fp::world_to_map(w.ox, w.oy, w.res, w.sx, w.sy, wx, wy, mx, my);
 }
 
 // Order-preserving integer encoding of a double (for atomicMin / atomicMax on the touch bounds).  touch() keeps

@@ -18,6 +18,8 @@
 // W6 pcl::PointXYZRGB: fields x 0, y 4, z 8, rgb 16.  100 + |frame_id| + 32n.
 // W7 octomap_msgs/Octomap (fullMapToMsg): header, binary 0, id "ColorOcTree", resolution (float64), int8[] stream.
 //    44 + |frame_id| + bytes.
+// W9-W11 and the publisher's decision P1-P4 (DESIGN.md f17, costmap_2d of navigation 1.14): below and in
+//    include/gem_b200.h.
 #pragma once
 #include <stdint.h>
 #include <string.h>
@@ -28,6 +30,12 @@
 
 #if !defined(__BYTE_ORDER__) || __BYTE_ORDER__ != __ORDER_LITTLE_ENDIAN__
 #error "gem_rosfmt.h writes ROS1's little-endian wire format with host stores"
+#endif
+
+#ifdef __CUDACC__
+#define GEM_RF __host__ __device__ __forceinline__
+#else
+#define GEM_RF inline
 #endif
 
 namespace gem_ros {
@@ -175,6 +183,143 @@ inline int octomap(const gem_ros_header &h, double resolution, long long bytes, 
     f.u32((uint32_t)bytes);
     f.payload(bytes);
     return GEM_OK;
+}
+
+// ---- the costmap topics (DESIGN.md f17) ----
+// T, Costmap2DPublisher's cost_translation_table_: 0 -> 0, 253 -> 99, 254 -> 100, 255 -> -1, and 1..252 scaled into 1..98
+// in integer arithmetic (the device's too: k_ros_costmap)
+GEM_RF signed char cost_translate(unsigned c)
+{
+    if (c == 0) return 0;
+    if (c == 253) return 99;
+    if (c == 254) return 100;
+    if (c == 255) return -1;
+    return (signed char)(1 + (97 * ((int)c - 1)) / 251);
+}
+
+// W9 nav_msgs/OccupancyGrid (prepareGrid): the data (size_x size_y bytes) is the payload
+inline int occupancy_grid(const gem_ros_header &h, const gem_costmap_window &w, Framing &f)
+{
+    const long long cells = (long long)w.size_x * w.size_y;
+    if (w.size_x <= 0 || w.size_y <= 0 || cells >= U32_LIMIT) return GEM_ERR_INVALID;
+    const double res = w.resolution;
+    const double wx = w.origin_x + (0 + 0.5) * res, wy = w.origin_y + (0 + 0.5) * res; // mapToWorld(0, 0)
+    f.header(h);
+    f.u32(0); f.u32(0);          // map_load_time: never set
+    const float fres = (float)res;
+    f.put(&fres, 4);
+    f.u32((uint32_t)w.size_x);
+    f.u32((uint32_t)w.size_y);
+    f.f64(wx - res / 2); f.f64(wy - res / 2); f.f64(0.0);
+    f.f64(0.0); f.f64(0.0); f.f64(0.0); f.f64(1.0);
+    f.u32((uint32_t)cells);
+    f.payload(cells);
+    return GEM_OK;
+}
+
+// W10 map_msgs/OccupancyGridUpdate of [x0, x0 + width) x [y0, y0 + height): the data (width height bytes) is the payload
+inline int occupancy_grid_update(const gem_ros_header &h, int x0, int y0, int width, int height, Framing &f)
+{
+    const long long cells = (long long)width * height;
+    if (width < 0 || height < 0 || cells >= U32_LIMIT) return GEM_ERR_INVALID;
+    f.header(h);
+    f.u32((uint32_t)x0);
+    f.u32((uint32_t)y0);
+    f.u32((uint32_t)width);
+    f.u32((uint32_t)height);
+    f.u32((uint32_t)cells);
+    f.payload(cells);
+    return GEM_OK;
+}
+
+// W11 geometry_msgs/PolygonStamped: every byte is framing (the transformed points as float32 x, y, z = 0)
+inline int polygon_stamped(const gem_ros_header &h, const double *xy, int n, Framing &f)
+{
+    if (n < 0 || 12ll * n >= U32_LIMIT) return GEM_ERR_INVALID;
+    f.header(h);
+    f.u32((uint32_t)n);
+    for (int i = 0; i < n; i++) {
+        const float p[3] = {(float)xy[2 * i], (float)xy[2 * i + 1], 0.0f};
+        f.put(p, 12);
+    }
+    return GEM_OK;
+}
+
+// P3 what a publish sends and the rectangle of its data (the whole grid for FULL); the publisher's state is not touched
+struct CostmapPlan {
+    int kind;                 // GEM_COSTMAP_PUB_*
+    int x0, y0, width, height;
+};
+inline CostmapPlan costmap_plan(const gem_costmap_publisher &p, const gem_costmap_window &w, int force_full)
+{
+    CostmapPlan d{GEM_COSTMAP_PUB_NONE, 0, 0, 0, 0};
+    const float res = (float)w.resolution; // Costmap2DPublisher compares the resolution as a float
+    if (force_full || p.always_send_full || !p.saved || p.resolution != res || p.size_x != w.size_x || p.size_y != w.size_y ||
+        p.origin_x != w.origin_x || p.origin_y != w.origin_y) {
+        d.kind = GEM_COSTMAP_PUB_FULL;
+        d.width = w.size_x;
+        d.height = w.size_y;
+    } else if (p.x0 < p.xn) { // y is not checked: an update of height 0 is sent
+        d = CostmapPlan{GEM_COSTMAP_PUB_UPDATE, p.x0, p.y0, p.xn - p.x0, p.yn - p.y0};
+    }
+    return d;
+}
+// an UPDATE reads the grid inside the window only
+inline bool costmap_plan_ok(const CostmapPlan &d, const gem_costmap_window &w)
+{
+    return d.kind != GEM_COSTMAP_PUB_UPDATE ||
+           (d.x0 >= 0 && d.width > 0 && d.x0 + (long long)d.width <= w.size_x && d.y0 >= 0 && d.height >= 0 &&
+            d.y0 + (long long)d.height <= w.size_y);
+}
+// P4, once the message is written: a FULL one saves the window; the bounds are reset to empty (x0 = size_x, y0 = size_y,
+// xn = yn = 0; DEFINED y0 = size_y, which for GEM's square grids is also size_x), except after force_full
+// (onNewSubscription publishes without touching them)
+inline void costmap_commit(gem_costmap_publisher &p, const gem_costmap_window &w, const CostmapPlan &d, int force_full)
+{
+    if (d.kind == GEM_COSTMAP_PUB_FULL) {
+        p.saved = 1;
+        p.resolution = (float)w.resolution;
+        p.size_x = w.size_x;
+        p.size_y = w.size_y;
+        p.origin_x = w.origin_x;
+        p.origin_y = w.origin_y;
+    }
+    if (force_full) return;
+    p.x0 = w.size_x;
+    p.y0 = w.size_y;
+    p.xn = p.yn = 0;
+}
+// A publish up to its first byte: the plan (P3), its framing (W9 / W10; NONE is an empty message), and whether the call
+// writes: a size query (out NULL) or a capacity below the size writes nothing, and then the publisher must stay as it
+// was (costmap_commit is not called).  GEM_ERR_INVALID for an UPDATE of bounds outside the grid.
+inline int costmap_message(const gem_ros_header &h, const gem_costmap_window &w, const gem_costmap_publisher &p, int force_full,
+                           bool size_query, long long capacity, CostmapPlan &d, Framing &f, bool &writes)
+{
+    writes = false;
+    d = costmap_plan(p, w, force_full);
+    if (!costmap_plan_ok(d, w)) return GEM_ERR_INVALID;
+    int rc = GEM_OK;
+    if (d.kind == GEM_COSTMAP_PUB_FULL) rc = occupancy_grid(h, w, f);
+    else if (d.kind == GEM_COSTMAP_PUB_UPDATE) rc = occupancy_grid_update(h, d.x0, d.y0, d.width, d.height, f);
+    if (rc) return rc;
+    writes = !size_query && capacity >= f.size;
+    return GEM_OK;
+}
+
+// P1, P2
+inline void costmap_publisher_init(gem_costmap_publisher &p, int always_send_full)
+{
+    p = gem_costmap_publisher{};
+    p.always_send_full = always_send_full ? 1 : 0;
+    p.x0 = p.y0 = 0x7fffffff;
+    p.xn = p.yn = 0;
+}
+inline void costmap_publisher_bounds(gem_costmap_publisher &p, int x0, int xn, int y0, int yn)
+{
+    p.x0 = x0 < p.x0 ? x0 : p.x0;
+    p.xn = xn > p.xn ? xn : p.xn;
+    p.y0 = y0 < p.y0 ? y0 : p.y0;
+    p.yn = yn > p.yn ? yn : p.yn;
 }
 
 } // namespace gem_ros

@@ -104,6 +104,48 @@ __global__ void __launch_bounds__(256) k_ros_orthomosaic(MapGeom g, MapLayers ml
     }
 }
 
+// W9 / W10's data (DESIGN.md f17): T[cost] of the master grid's rectangle [x0, x0 + w) x [y0, ...) in row order, at any
+// alignment, as k_ros_orthomosaic writes its image.  Thread q owns the aligned 16-byte word q of the output range and
+// reads its 16 cells once (row by row at stride sx); the first and the last word, which the data may share with the
+// framing, are written byte by byte.  T is gem_ros::cost_translate, computed in registers.
+__device__ __forceinline__ unsigned char ros_cost_byte(const unsigned char *master, int sx, int x0, int y0, int w, long long d)
+{
+    const long long r = d / w, c = d - r * w;
+    return (unsigned char)gem_ros::cost_translate(master[(y0 + r) * sx + x0 + c]);
+}
+__global__ void __launch_bounds__(256) k_ros_costmap(const unsigned char *master, int sx, int x0, int y0, int w, long long n,
+                                                     unsigned char *data, long long nwords)
+{
+    const long long q = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (q >= nwords) return;
+    const long long a = (long long)((uintptr_t)data & 15u);
+    const long long d0 = 16 * q - a; // data byte at the word's first byte
+    if (d0 >= 0 && d0 + 16 <= n) {
+        long long r = d0 / w;
+        int c = (int)(d0 - r * w);
+        const unsigned char *row = master + (y0 + r) * sx + x0;
+        uint32_t v[4] = {0u, 0u, 0u, 0u};
+#pragma unroll
+        for (int k = 0; k < 16; k++) {
+            v[k >> 2] |= (uint32_t)(unsigned char)gem_ros::cost_translate(row[c]) << (8 * (k & 3));
+            if (++c == w) {
+                c = 0;
+                row += sx;
+            }
+        }
+        *reinterpret_cast<uint4 *>(data + d0) = make_uint4(v[0], v[1], v[2], v[3]);
+    } else {
+        for (long long d = d0 < 0 ? 0 : d0; d < d0 + 16 && d < n; d++) data[d] = ros_cost_byte(master, sx, x0, y0, w, d);
+    }
+}
+
+// ObstacleLayer's footprint clearing: `value` into the layer grid at the n cell indices the host listed (gem_footprint.h)
+__global__ void __launch_bounds__(256) k_costmap_cells(const int *cells, int n, unsigned char *grid, unsigned char value)
+{
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) grid[cells[i]] = value;
+}
+
 // W6's record of one shown cell: {x, y, z, 1.0f, b, g, r, 0xff, 12 zero bytes}, stored at any alignment (aligned
 // 4-byte words inside the record, single bytes at its two ends)
 __device__ __forceinline__ void ros_store_record(unsigned char *dst, const uint32_t (&w)[8])

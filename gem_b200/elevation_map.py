@@ -721,6 +721,57 @@ class ElevationMap:
                                                                                            "costmap_inflate"), i0, j0, i1, j1),
               self._h, "gem_costmap_inflate")
 
+    # -- what Costmap2DROS publishes, and ObstacleLayer's footprint clearing (DESIGN.md f17) ---------------------------------
+    # A footprint is a sequence of (x, y) vertices in metres (the padded footprint); the pose is the robot's x, y, yaw.
+    @staticmethod
+    def _footprint(footprint):
+        a = np.ascontiguousarray(np.asarray(footprint, np.float64).reshape(-1, 2))
+        return a, a.shape[0], (a.ctypes.data_as(C.POINTER(C.c_double)) if a.shape[0] else None)
+
+    def costmap_footprint(self, window, footprint, robot_x: float, robot_y: float, robot_yaw: float, layer) -> dict:
+        """ObstacleLayer::updateFootprint and its updateCosts' setConvexPolygonCost(FREE_SPACE) on the layer grid: the
+        footprint at the pose is written FREE (nothing when a vertex lies outside the window or there are fewer than 3);
+        returns {marked: cells written, lethal: 0, min_x, min_y, max_x, max_y: the vertices' touch bounds}.
+        Asynchronous on the library's stream (torch_stream())."""
+        w = self._cost_window(window)
+        fp, n, ptr = self._footprint(footprint)
+        mk = _lib.GemCostmapMarks()
+        check(self._lib.gem_costmap_footprint(self._h, C.byref(w), ptr, n, float(robot_x), float(robot_y), float(robot_yaw),
+                                              self._cost_grid(layer, w.size_x, w.size_y, "costmap_footprint"), C.byref(mk)),
+              self._h, "gem_costmap_footprint")
+        return self._cost_marks(mk)
+
+    def ros_footprint(self, header: RosHeader, footprint, robot_x: float, robot_y: float, robot_yaw: float, out=None):
+        """<costmap>/footprint (geometry_msgs/PolygonStamped, W11) of the footprint at the pose"""
+        h = header.c()
+        fp, n, ptr = self._footprint(footprint)
+        return self._ros_message("gem_ros_footprint", lambda p, c, nb: self._lib.gem_ros_footprint(
+            self._h, C.byref(h), ptr, n, float(robot_x), float(robot_y), float(robot_yaw), p, c, nb), out)
+
+    def ros_costmap(self, header: RosHeader, window, master, publisher, force_full: bool = False, out=None):
+        """one Costmap2DPublisher::publishCostmap (or, with force_full, onNewSubscription's message) of the master grid:
+        `publisher` is a gem_costmap_publisher (gem_b200.costmap.CostmapPublisher holds one).  Returns (kind, message) with
+        kind "full" (nav_msgs/OccupancyGrid, W9), "update" (map_msgs/OccupancyGridUpdate, W10) or "none" (an empty
+        message).  A size query or an `out` too small leaves the publisher as it was."""
+        import torch
+        w = self._cost_window(window)
+        grid = self._cost_grid(master, w.size_x, w.size_y, "ros_costmap")
+        h = header.c()
+        kind = C.c_int()
+        what = "gem_ros_costmap"
+
+        def call(p, c, nb):
+            return self._lib.gem_ros_costmap(self._h, C.byref(h), C.byref(w), grid, C.byref(publisher), 1 if force_full else 0,
+                                             p, c, nb, C.byref(kind))
+        if out is None:
+            out = torch.empty(max(self._ros_size(what, call), 1), dtype=torch.uint8,
+                              device=torch.device("cuda", self._device_index()))
+        else:
+            out = self._ros_buffer(out, what)
+        n = self._ros_write(what, call, out)
+        self.sync()
+        return _lib.COSTMAP_PUB_KINDS[kind.value], out[:n]
+
     # -- the VoxelGrid pre-filter of GEM's demo launches (DESIGN.md f9) ---------------------------------------------------
     def voxel_grid(self, xyzi, leaf_size, field=None, limits=(-3.4028234663852886e38, 3.4028234663852886e38), negative=False,
                    out=None):

@@ -383,8 +383,9 @@ int gem_color_octree_read(gem_map *m, void *out, long long capacity);
  *   layer cell that is not NO_INFORMATION is copied).  layer and master are grids of size_x * size_y.
  * update_origin and combine are asynchronous on the handle's stream and, like mark_points, work on any handle.  No call
  * modifies the map.  Every call rejects a bad window (size <= 0, size_x * size_y >= 2^31, a resolution that is <= 0 or not
- * finite); a rejected call writes nothing.  Out of scope: footprint clearing (footprint_clearing_enabled false),
- * publishing, and the elevation_map_available_ subscription gate.  InflationLayer is gem_costmap_inflate (DESIGN.md f14). */
+ * finite); a rejected call writes nothing.  Out of scope: the elevation_map_available_ subscription gate.  InflationLayer
+ * is gem_costmap_inflate (DESIGN.md f14); footprint clearing and publishing are gem_costmap_footprint and
+ * gem_ros_costmap / gem_ros_footprint (DESIGN.md f17). */
 enum { GEM_COST_FREE = 0, GEM_COST_LETHAL = 254, GEM_COST_UNKNOWN = 255 };
 enum { GEM_COSTMAP_MAX = 0, GEM_COSTMAP_OVERWRITE = 1 };
 typedef struct gem_costmap_window {
@@ -691,6 +692,76 @@ int gem_ros_visual_points(gem_map *m, const gem_ros_header *h, void *out, long l
 int gem_ros_cloud(gem_map *m, const gem_ros_header *h, const gem_ros_part *parts, int nparts, int is_dense, void *out,
                   long long capacity, long long *bytes_out);
 int gem_ros_octomap(gem_map *m, const gem_ros_header *h, void *out, long long capacity, long long *bytes_out);
+
+/* ---- what Costmap2DROS publishes, and ObstacleLayer's footprint clearing (DESIGN.md f17) ----
+ * Restated from costmap_2d of navigation 1.14 (unpinned); the wire format follows W1 (gem_b200/csrc/gem_rosfmt.h).
+ *   T  the cost translation table: T[0] = 0, T[253] = 99, T[254] = 100, T[255] = -1, T[i] = (char)(1 + (97 (i - 1)) / 251)
+ *      in integer arithmetic for 1 <= i <= 252.
+ *   W9 nav_msgs/OccupancyGrid (Costmap2DPublisher::prepareGrid): header, map_load_time (0, 0), resolution (float),
+ *      width = size_x, height = size_y, origin position (wx - res / 2, wy - res / 2, 0) with (wx, wy) = mapToWorld(0, 0) =
+ *      origin + 0.5 res, all in double (so not always bit-equal to the origin), orientation (0, 0, 0, 1), int8[] data =
+ *      T[cost] in index order my * size_x + mx.  96 + |frame_id| + size_x size_y bytes; the data field at 92 + |frame_id| (its
+ *      uint32 count, then the bytes from 96 + |frame_id|).
+ *   W10 map_msgs/OccupancyGridUpdate: header, int32 x = x0, int32 y = y0, uint32 width = xn - x0, uint32 height = yn - y0,
+ *      int8[] data = T[master(x, y)], y outer from y0, x inner from x0.  36 + |frame_id| + width height bytes.
+ *   W11 geometry_msgs/PolygonStamped (Costmap2DROS::updateMap): header, Point32[] with x = (float)(rx + (fx cos t - fy sin
+ *      t)), y = (float)(ry + (fx sin t + fy cos t)), z = 0; cos and sin in double, DEFINED as the host libm's.
+ *      20 + |frame_id| + 12 n bytes.
+ * The publisher (Costmap2DPublisher::updateBounds / publishCostmap), one gem_costmap_publisher per costmap:
+ *   P1 gem_costmap_publisher_init: nothing saved, bounds empty.  DEFINED: empty initial bounds are x0 = y0 = INT_MAX,
+ *      xn = yn = 0 (the reference starts at the grid's size, unknown here; the first message is full either way and
+ *      min(size, b) = min(INT_MAX, b) for every bound b inside the grid).
+ *   P2 gem_costmap_publisher_bounds: x0 = min(x0, b), xn = max(xn, b), likewise y (LayeredCostmap::getBounds' rect).
+ *   P3 gem_ros_costmap decides: FULL (W9) when force_full, always_send_full, nothing saved, or the saved (float
+ *      resolution, size_x, size_y, double origin_x, origin_y) differ from the window; else UPDATE (W10) of the bounds when
+ *      x0 < xn (y is not checked: a height of 0 is sent); else NONE (nothing is written, bytes 0).
+ *   P4 a FULL message saves the window.  Then the bounds are reset to empty, x0 = size_x, y0 = size_y, xn = yn = 0
+ *      (DEFINED: y0 = size_y; for square grids size_x gives the same bytes) -- except after force_full
+ *      (onNewSubscription), which leaves them.
+ *   The subscriber gate and the publish timer stay with the caller: not calling gem_ros_costmap is what the reference
+ *   does without subscribers, and the bounds keep accumulating.
+ * gem_ros_costmap: kind_out receives GEM_COSTMAP_PUB_NONE / _FULL / _UPDATE.  The state of *p changes only when the
+ *   call writes its message (a NONE message is written by any call that is not a size query); a size query (out NULL,
+ *   capacity 0) or a too-small capacity leaves *p as it was.  GEM_ERR_INVALID, with nothing written and *p unchanged: a
+ *   NULL p or master, a bad window (f8), an UPDATE whose bounds are not 0 <= x0 < xn <= size_x, 0 <= y0 <= yn <= size_y,
+ *   an output overlapping the master grid, force_full other than 0 or 1.
+ * gem_ros_footprint: W11 of the n (x, y) pairs spec_xy (the padded footprint) at the robot's pose.
+ * Common to both (f15's rules): out is device or pinned host memory at any alignment (pageable memory is GEM_ERR_INVALID);
+ *   the message is written whole or not at all; *bytes_out is always set (out NULL with capacity 0 is a size query);
+ *   a NULL header or frame_id, n < 0, a NULL spec_xy with n > 0 and a non-finite pose or spec value are GEM_ERR_INVALID.
+ *   Asynchronous on the handle's stream; the map is not read, so tiled handles are accepted.  The master grid is read
+ *   once, on the device; pinned outputs are staged on the device and copied in one DMA transfer.
+ * gem_costmap_footprint: ObstacleLayer::updateFootprint and the footprint clearing of ObstacleLayer::updateCosts
+ *   (setConvexPolygonCost(transformed footprint, FREE_SPACE)) on a layer grid of window w, on the host and one small
+ *   kernel.  The footprint is W11's transform kept in double; *out gets marked = the cells written (convexFillCells'
+ *   list, duplicates included), lethal = 0 and the touch bounds of the n vertices (+inf / -inf for n = 0).
+ *   F1 every vertex goes through worldToMap (f8); one outside the window fills nothing.
+ *   F2 fewer than 3 vertices fill nothing (convexFillCells).
+ *   F3 polygonOutlineCells: raytraceLine (bresenham2D, both end cells included) from each vertex to the next and from the
+ *      last to the first, as indexToCells of the walked offsets.
+ *   F4 the adjacent-swap sort by x (after a swap, i steps back), then the column walk: for x from the first cell's x to
+ *      the last's, cells i and i + 1 give min and max by y, i += 2, cells of the same x widen them, and the cells (x, y)
+ *      for min.y <= y < max.y are appended to the list being walked.  Literal: a column of one cell would pair it with the
+ *      next column's first, though F3's closed outline gives every column two cells or more.
+ *   Asynchronous on the handle's stream; any handle.  GEM_ERR_INVALID, writing nothing: a NULL layer or out, a bad
+ *   window, n < 0, a NULL spec_xy with n > 0, a non-finite pose or spec value. */
+enum { GEM_COSTMAP_PUB_NONE = 0, GEM_COSTMAP_PUB_FULL = 1, GEM_COSTMAP_PUB_UPDATE = 2 };
+typedef struct gem_costmap_publisher {
+    int always_send_full;              /* always_send_full_costmap                                             */
+    int saved;                         /* 0 until the first full message                                       */
+    float resolution;                  /* the saved window: grid_.info's resolution, width, height and         */
+    int size_x, size_y;                /*   saved_origin_x_ / _y_                                              */
+    double origin_x, origin_y;
+    int x0, xn, y0, yn;                /* the accumulated bounds                                               */
+} gem_costmap_publisher;
+int gem_costmap_publisher_init(gem_costmap_publisher *p, int always_send_full);
+int gem_costmap_publisher_bounds(gem_costmap_publisher *p, int x0, int xn, int y0, int yn);
+int gem_ros_costmap(gem_map *m, const gem_ros_header *h, const gem_costmap_window *w, const unsigned char *master_device,
+                    gem_costmap_publisher *p, int force_full, void *out, long long capacity, long long *bytes_out, int *kind_out);
+int gem_ros_footprint(gem_map *m, const gem_ros_header *h, const double *spec_xy, int n, double robot_x, double robot_y,
+                      double robot_yaw, void *out, long long capacity, long long *bytes_out);
+int gem_costmap_footprint(gem_map *m, const gem_costmap_window *w, const double *spec_xy, int n, double robot_x, double robot_y,
+                          double robot_yaw, unsigned char *layer_device, gem_costmap_marks *out);
 
 /* raw layer access (row-major L*L, float or int32 for the colour ids) for tests and
  * checkpoint/restore (the dead G_get_mapinfo/G_set_mapinfo of gpu.cu:457-475). */

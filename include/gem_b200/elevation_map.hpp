@@ -608,6 +608,33 @@ class ElevationMap {
         std::memcpy(&out[out.size() - 7 * sizeof(double)], pose, 7 * sizeof(double));
         return out.size();
     }
+    // What Costmap2DROS publishes (DESIGN.md f17): rosCostmap is one publishCostmap of a master grid (forceFull:
+    // onNewSubscription's full grid) through a CostmapPublisher's state -- kind GEM_COSTMAP_PUB_FULL (OccupancyGrid),
+    // _UPDATE (OccupancyGridUpdate) or _NONE (an empty message); rosFootprint is the PolygonStamped of the padded
+    // footprint (x, y pairs) at the pose.  costmapFootprint clears the footprint in an ElevationMapLayer's grid as
+    // ObstacleLayer does and returns the vertices' touch bounds.
+    template <class Buffer>
+    size_t rosCostmap(const gem_ros_header &h, const gem_costmap_window &w, const unsigned char *master_device, gem_costmap_publisher &p,
+                      Buffer &out, int *kind, bool forceFull = false)
+    {
+        return rosInto(out, 0, "gem_ros_costmap", [&](void *q, long long c, long long *nb) {
+            return gem_ros_costmap(h_, &h, &w, master_device, &p, forceFull ? 1 : 0, q, c, nb, kind);
+        });
+    }
+    template <class Buffer>
+    size_t rosFootprint(const gem_ros_header &h, const std::vector<double> &spec_xy, double x, double y, double yaw, Buffer &out)
+    {
+        return rosInto(out, 0, "gem_ros_footprint", [&](void *q, long long c, long long *nb) {
+            return gem_ros_footprint(h_, &h, spec_xy.data(), (int)(spec_xy.size() / 2), x, y, yaw, q, c, nb);
+        });
+    }
+    gem_costmap_marks costmapFootprint(const gem_costmap_window &w, const std::vector<double> &spec_xy, double x, double y, double yaw,
+                                       unsigned char *layer_device)
+    {
+        gem_costmap_marks mk;
+        check(gem_costmap_footprint(h_, &w, spec_xy.data(), (int)(spec_xy.size() / 2), x, y, yaw, layer_device, &mk), "gem_costmap_footprint");
+        return mk;
+    }
     // Loop closure (ElevationMapping::updateGlobalMap, ElevationMapping.cpp:773-905), on device-resident submaps of
     // PointXYZRGBICT records: re-pose a submap (:805), and one pass of the pairwise fuse loop (:847-883) -- both clouds
     // come back reduced to one point per cell and compacted, *n_new / *n_old updated.  compat_precedence = true evaluates
@@ -689,11 +716,14 @@ class ElevationMap {
         long long bytes = 0;
         if (resize) {
             check(call(nullptr, 0, &bytes), what);
-            out.resize((size_t)bytes);
+            out.resize((size_t)bytes > 0 ? (size_t)bytes : 1); // an empty message (rosCostmap's NONE) still has a buffer to write to
         }
         check(call(&out[0] + at, (long long)(out.size() - at), &bytes), what);
         if ((size_t)bytes > out.size() - at) throw std::runtime_error(std::string(what) + ": the buffer is too small");
-        if (resize) sync();
+        if (resize) {
+            out.resize((size_t)bytes);
+            sync();
+        }
         return (size_t)bytes;
     }
     static int pcdFlags(bool binary, bool rgbUint32) { return (binary ? GEM_PCD_BINARY : 0) | (rgbUint32 ? GEM_PCD_RGB_UINT32 : 0); }
@@ -703,6 +733,14 @@ class ElevationMap {
     }
     gem_map *h_ = nullptr;
     int length_ = 0;
+};
+
+// Costmap2DPublisher's state for one costmap (DESIGN.md f17): feed LayeredCostmap::getBounds after each update once the
+// costmap is initialised, then ElevationMap::rosCostmap(..., publisher.state, ...) at the publish rate
+struct CostmapPublisher {
+    gem_costmap_publisher state;
+    explicit CostmapPublisher(bool alwaysSendFull = false) { gem_costmap_publisher_init(&state, alwaysSendFull ? 1 : 0); }
+    void updateBounds(int x0, int xn, int y0, int yn) { gem_costmap_publisher_bounds(&state, x0, xn, y0, yn); }
 };
 
 } // namespace gem_b200
