@@ -148,6 +148,12 @@ class GemCostmapPublisher(C.Structure):
                 ("y0", C.c_int), ("yn", C.c_int)]
 
 
+class GemGridMapLayer(C.Structure):
+    _fields_ = [("resolution", C.c_double), ("position_x", C.c_double), ("position_y", C.c_double), ("length_x", C.c_double),
+                ("length_y", C.c_double), ("size_x", C.c_int), ("size_y", C.c_int), ("start_x", C.c_int), ("start_y", C.c_int),
+                ("offset", C.c_ulonglong), ("floats", C.c_longlong), ("column_major", C.c_int)]
+
+
 COST_FREE, COST_LETHAL, COST_UNKNOWN = 0, 254, 255           # GEM_COST_*
 INFLATE_MAX_CELLS = 4094                                     # GEM_INFLATE_MAX_CELLS
 COSTMAP_MODES = {"max": 0, "overwrite": 1}                  # GEM_COSTMAP_MAX / GEM_COSTMAP_OVERWRITE
@@ -266,6 +272,10 @@ SYMBOLS = {
                                     C.c_double, _P, C.c_longlong, C.POINTER(C.c_longlong)]),
     "gem_costmap_footprint": (C.c_int, [_P, C.POINTER(GemCostmapWindow), C.POINTER(C.c_double), C.c_int, C.c_double, C.c_double,
                                         C.c_double, _P, C.POINTER(GemCostmapMarks)]),
+    "gem_grid_map_msg_parse": (C.c_int, [_P, C.c_ulonglong, C.c_char_p, C.POINTER(GemGridMapLayer)]),
+    "gem_costmap_mark_grid": (C.c_int, [_P, C.POINTER(GemGridMapLayer), _P, C.POINTER(GemCostmapWindow), C.c_double, C.c_int, _P,
+                                        C.POINTER(GemCostmapMarks)]),
+    "gem_decode_pointcloud2_records": (C.c_int, [_P, C.POINTER(GemPointCloud2), _P, C.c_ulonglong, _P]),
 }
 
 _lib = None

@@ -14,12 +14,18 @@ plugins (DESIGN.md f14).
 What Costmap2DROS publishes, and ObstacleLayer's footprint clearing (DESIGN.md f17): `CostmapPublisher` is
 Costmap2DPublisher's decision between a full grid, an update and nothing, with the bytes written on the device;
 `Costmap.update(..., robot_yaw=, footprint=)` clears the footprint in the layer grid; `Costmap` keeps LayeredCostmap's
-getBounds rect and its initialized flag for the publisher."""
+getBounds rect and its initialized flag for the publisher.
+
+The two plugins as move_base runs them, fed from their subscribed messages (DESIGN.md f18): `ElevationMapLayer` takes
+the serialised grid_map_msgs/GridMap bytes of visual_map, `PointMapLayer` the PointCloud2 of history_point; either is
+passed to `Costmap.update` as its `mark`."""
 from __future__ import annotations
 
 import math
 
 import ctypes as C
+
+import numpy as np
 
 from . import _lib
 from ._lib import COST_FREE, COST_LETHAL, COST_UNKNOWN  # noqa: F401
@@ -173,6 +179,133 @@ class Costmap:
         self.bx0, self.bxn, self.by0, self.byn = x0, xn, y0, yn
         self.initialized = True
         return rect, marks
+
+
+def _host_u8(a):
+    """host bytes (bytes, bytearray, memoryview, numpy or a CPU tensor) as a flat uint8 CPU tensor sharing their memory"""
+    import torch
+    import warnings
+    if isinstance(a, torch.Tensor):
+        return a.reshape(-1).view(torch.uint8)
+    with warnings.catch_warnings():      # read-only bytes: the tensor is only ever read
+        warnings.simplefilter("ignore", UserWarning)
+        return torch.from_numpy(np.frombuffer(memoryview(a).cast("B"), np.uint8))
+
+
+NO_MARKS = {"marked": 0, "lethal": 0, "min_x": math.inf, "min_y": math.inf, "max_x": -math.inf, "max_y": -math.inf}
+
+
+class ElevationMapLayer:
+    """ElevationMapLayer (layers/src/elevationMap_layer.cpp) fed from visual_map messages.  `on_message` is
+    elevationMapCB with its elevation_map_available_ gate: a message is kept only when none is pending; keeping it is
+    gem_grid_map_msg_parse of the bytes and one H2D copy of the `layer` floats alone into a device buffer this object
+    owns (on torch's current stream, which the mark waits for).  `update_bounds` (or calling the object, as Costmap.update's `mark`) marks the layer grid
+    from the pending message and consumes it; with none pending it marks nothing.  DEFINED: a message the parser refuses
+    raises GemError and leaves the layer as it was (the reference sets elevation_map_available_ after a failed
+    fromMessage and marks whatever that left, or throws in operator[] when no message ever had the layer).
+    travers_thresh defaults to the plugin's 0.5; GEM's yaml sets 0.7."""
+
+    def __init__(self, emap, travers_thresh: float = 0.5, mark_unknown: bool = True, layer: str = "traver"):
+        self.emap = emap
+        self.travers_thresh = float(travers_thresh)
+        self.mark_unknown = bool(mark_unknown)
+        self.layer = str(layer)
+        self.desc = None           # the pending message's gem_grid_map_layer, None when none is pending
+        self._buf = None           # the pending layer's floats (uint8 CUDA tensor, grown on demand)
+
+    @property
+    def available(self) -> bool:
+        """elevation_map_available_"""
+        return self.desc is not None
+
+    def on_message(self, msg) -> bool:
+        """elevationMapCB on the serialised message (bytes, numpy or a CPU tensor, pinned or pageable); returns whether
+        it was kept"""
+        import torch
+        from .elevation_map import ElevationMap
+        if self.desc is not None:
+            return False
+        g = ElevationMap.grid_map_msg_parse(msg, self.layer)
+        src = _host_u8(msg)
+        nb = 4 * int(g.floats)
+        dev = torch.device("cuda", self.emap._device_index())
+        if self._buf is None or self._buf.numel() < nb:
+            self.emap.sync()       # the previous buffer may still be read on the map's stream
+            self._buf = torch.empty(max(nb, 4), dtype=torch.uint8, device=dev)
+        # the copy runs on torch's current stream, which costmap_mark_grid synchronises before it marks.  Not on the
+        # map's stream: torch ties a pinned source block to the stream of its copy and records an event there when the
+        # block is freed, which must not outlive the stream (the map's is destroyed with the map)
+        self._buf[:nb].copy_(src[g.offset:g.offset + nb], non_blocking=src.is_pinned())
+        self.desc = g
+        return True
+
+    def update_bounds(self, layer_costmap: "Costmap") -> dict:
+        """updateBounds into the layer grid: the marks (NO_MARKS when no message is pending)"""
+        if self.desc is None:
+            return dict(NO_MARKS)
+        g, self.desc = self.desc, None
+        if layer_costmap.emap is not self.emap:
+            self.emap.sync()       # the copy ran on this layer's handle, the mark runs on the costmap's
+        return layer_costmap.emap.costmap_mark_grid(g, self._buf, layer_costmap.window, layer_costmap.grid,
+                                                    self.travers_thresh, self.mark_unknown)
+
+    __call__ = update_bounds
+
+
+class PointMapLayer:
+    """PointMapLayer (layers/src/pointMap_layer.cpp) fed from history_point messages.  `on_message(layout, data)` is
+    pointMapCB: the cloud replaces the stored one (ob_pointCloud = *pointCloud), decoded on the device into whole
+    PointXYZRGBICT records in a buffer this object owns and grows.  `update_bounds` (or calling the object) re-marks the
+    stored cloud every time, as the reference does; before any message it marks nothing.  DEFINED: the reference races
+    the callback against updateBounds; here calls take effect in call order.  travers_thresh defaults to the plugin's
+    0.5; GEM's yaml sets 0.7."""
+
+    def __init__(self, emap, travers_thresh: float = 0.5):
+        self.emap = emap
+        self.travers_thresh = float(travers_thresh)
+        self.n = None              # points of the stored cloud, None before any message
+        self._buf = None           # (capacity, 8) float32 CUDA tensor
+
+    @property
+    def points(self):
+        """the stored cloud's records, an (n, 8) float32 CUDA tensor view (None before any message)"""
+        return None if self.n is None else self._buf[:self.n]
+
+    def on_message(self, layout, data, data_bytes: int | None = None):
+        """pointMapCB on a PointCloud2 of `layout` (an elevation_map.PointCloud2Layout) whose bytes are `data`: a CUDA
+        tensor, or host memory (bytes, numpy or a CPU tensor) that is copied to the device first.  A layout the library
+        refuses raises GemError before anything changes: the stored cloud stays as it was (DEFINED, as for
+        ElevationMapLayer)."""
+        import torch
+        from .elevation_map import ElevationMap
+        dev = torch.device("cuda", self.emap._device_index())
+        if isinstance(data, torch.Tensor) and data.is_cuda:
+            nb = int(data.numel() * data.element_size()) if data_bytes is None else int(data_bytes)
+            ElevationMap.pointcloud2_mapping(layout, nb)           # validates the layout first (raises GemError)
+        else:
+            host = _host_u8(data)
+            nb = host.numel() if data_bytes is None else int(data_bytes)
+            ElevationMap.pointcloud2_mapping(layout, nb)
+            data = host.to(dev)
+            # the decode reads this staging copy on the map's stream after on_message returns: the caching allocator
+            # must not hand its memory out before that work is done
+            data.record_stream(self.emap.torch_stream())
+        n = layout.points
+        if self._buf is None or self._buf.shape[0] < n:
+            self.emap.sync()       # the previous buffer may still be read on the map's stream
+            self._buf = torch.empty((max(n + n // 4, 1024), 8), dtype=torch.float32, device=dev)
+        self.emap.decode_pointcloud2_records(layout, data, out=self._buf, data_bytes=nb)
+        self.n = n
+
+    def update_bounds(self, layer_costmap: "Costmap") -> dict:
+        """updateBounds into the layer grid: the marks (NO_MARKS before any message)"""
+        if self.n is None:
+            return dict(NO_MARKS)
+        if layer_costmap.emap is not self.emap:
+            self.emap.sync()       # the decode ran on this layer's handle, the mark runs on the costmap's
+        return layer_costmap.mark_points(self._buf[:self.n], self.travers_thresh)
+
+    __call__ = update_bounds
 
 
 class CostmapPublisher:

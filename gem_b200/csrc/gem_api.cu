@@ -25,6 +25,7 @@
 #include "../../include/gem_b200.h"
 #include "gem_add.cuh"
 #include "gem_costmap.cuh"
+#include "gem_gridmsg.h"
 #include "gem_inflate.cuh"
 #include "gem_kernels.cuh"
 #include "gem_global.cuh"
@@ -2044,6 +2045,39 @@ int gem_costmap_mark_points(gem_map *m, const void *points32_device, int n, cons
     return cost_mark(m, src, ((long long)n + 31) / 32, w, cost_device, out);
 }
 
+// ---- the plugins fed from their subscribed messages (gem_gridmsg.h G1-G4; f18) -----------------------------------------
+int gem_grid_map_msg_parse(const void *msg, unsigned long long bytes, const char *layer, gem_grid_map_layer *out)
+{
+    const char *why = gem_gridmsg::parse(msg, bytes, layer, out);
+    return why ? fail(nullptr, GEM_ERR_INVALID, std::string("gem_grid_map_msg_parse: ") + why) : GEM_OK;
+}
+
+int gem_costmap_mark_grid(gem_map *m, const gem_grid_map_layer *g, const void *layer_device, const gem_costmap_window *w,
+                          double travers_thresh, int mark_unknown, unsigned char *cost_device, gem_costmap_marks *out)
+{
+    if (!m || !g || !cost_device || !out || (g->floats > 0 && !layer_device))
+        return fail(m, GEM_ERR_INVALID, "gem_costmap_mark_grid: bad argument");
+    if (!cost_window_ok(w)) return fail(m, GEM_ERR_INVALID, "gem_costmap_mark_grid: bad window");
+    if (!gem_gridmsg::layer_ok(*g)) return fail(m, GEM_ERR_INVALID, "gem_costmap_mark_grid: bad layer descriptor");
+    Lock lk(m->mu);
+    SetDev sd(m->dev);
+    CostMsgSrc src;
+    src.p = static_cast<const unsigned char *>(layer_device);
+    src.aligned = ((uintptr_t)layer_device & 3u) == 0;
+    src.sx = g->size_x;
+    src.sy = g->size_y;
+    src.n = (int)g->floats;
+    // G4: the start index wrapped into [0, size) once, here; the positions' constant part in double as grid_map adds it
+    src.startx = g->size_x ? (int)(((long long)g->start_x % g->size_x + g->size_x) % g->size_x) : 0;
+    src.starty = g->size_y ? (int)(((long long)g->start_y % g->size_y + g->size_y) % g->size_y) : 0;
+    src.ox = g->position_x + (0.5 * g->length_x - 0.5 * g->resolution);
+    src.oy = g->position_y + (0.5 * g->length_y - 0.5 * g->resolution);
+    src.res = g->resolution;
+    src.thresh = travers_thresh;
+    src.mark_unknown = mark_unknown ? 1 : 0;
+    return cost_mark(m, src, ((long long)src.n + 31) / 32, w, cost_device, out);
+}
+
 int gem_costmap_update_origin(gem_map *m, gem_costmap_window *w, double new_origin_x, double new_origin_y, unsigned char fill,
                               unsigned char *cost_device)
 {
@@ -3226,12 +3260,14 @@ int gem_pointcloud2_mapping(const gem_pointcloud2 *layout, unsigned long long da
     return why ? fail(nullptr, GEM_ERR_INVALID, std::string("gem_pointcloud2_mapping: ") + why) : GEM_OK;
 }
 
-static int launch_decode(gem_map *m, const gem_pointcloud2 *layout, const gem_pc2_mapping &mp, const void *data, void *xyzi_out)
+// rec 16: float4 xyzi; rec 32: whole PointXYZRGBICT records
+static int launch_decode(gem_map *m, const gem_pointcloud2 *layout, const gem_pc2_mapping &mp, const void *data, void *out, int rec = 16)
 {
     if (mp.points == 0) return GEM_OK;
     const Pc2Params p = pc2_params(layout, mp, data, mp.bytes); // the kernel reads no byte past the last point's
     const int blocks = p.tiles < (unsigned long long)NUM_SMS * 16 ? (int)p.tiles : NUM_SMS * 16;
-    GEM_LAUNCH(m, GEM_PROF_OTHER, k_decode_pc2<<<blocks, PC2_BLOCK, pc2_smem_bytes(p), m->stream>>>(p, (uint4 *)xyzi_out));
+    if (rec == 32) GEM_LAUNCH(m, GEM_PROF_OTHER, k_decode_pc2<32><<<blocks, PC2_BLOCK, pc2_smem_bytes(p), m->stream>>>(p, (uint4 *)out));
+    else GEM_LAUNCH(m, GEM_PROF_OTHER, k_decode_pc2<16><<<blocks, PC2_BLOCK, pc2_smem_bytes(p), m->stream>>>(p, (uint4 *)out));
     GEM_CUDA(m, cudaGetLastError());
     return GEM_OK;
 }
@@ -3249,6 +3285,23 @@ int gem_decode_pointcloud2(gem_map *m, const gem_pointcloud2 *layout, const void
     Lock lk(m->mu);
     SetDev sd(m->dev);
     return launch_decode(m, layout, mp, data, xyzi_out);
+}
+
+// f18: the same decode into whole 32-byte records
+int gem_decode_pointcloud2_records(gem_map *m, const gem_pointcloud2 *layout, const void *data, unsigned long long data_bytes,
+                                   void *points32_out)
+{
+    if (!m) return GEM_ERR_INVALID;
+    gem_pc2_mapping mp;
+    const char *why = pc2_map(layout, data_bytes, &mp);
+    if (why) return fail(m, GEM_ERR_INVALID, std::string("gem_decode_pointcloud2_records: ") + why);
+    if (mp.points > 0 && ((mp.bytes > 0 && !data) || !points32_out || ((uintptr_t)points32_out & 15u)))
+        return fail(m, GEM_ERR_INVALID, "gem_decode_pointcloud2_records: NULL pointer, or the output is not 16-byte aligned");
+    if (mp.points > 0 && ranges_meet(data, mp.bytes, points32_out, (size_t)mp.points * PC2_RECORD))
+        return fail(m, GEM_ERR_INVALID, "gem_decode_pointcloud2_records: the message and output ranges overlap");
+    Lock lk(m->mu);
+    SetDev sd(m->dev);
+    return launch_decode(m, layout, mp, data, points32_out, (int)PC2_RECORD);
 }
 
 static int launch_image(gem_map *m, int enc, const void *src, int width, int height, long long step, void *dst, long long dst_step)

@@ -114,6 +114,43 @@ struct CostPointSrc {
     }
 };
 
+// Message-layer source (DESIGN.md f18): the floats of one grid_map_msgs/GridMap layer at any alignment, in G4 order
+// (element k = the k-th float, buffer index (k % sx, k / sx)).  Positions are GridMapFrame's generalised to a rectangular
+// map: (position + half) - res * unwrapped, half = 0.5 * length - 0.5 * res per axis, the start index already reduced
+// into [0, size) on the host.  The cost rule and mark_unknown are CostGridSrc's.  A chunk is 32 consecutive floats.
+struct CostMsgSrc {
+    const unsigned char *p; // the layer's first float
+    int aligned;            // p is 4-byte aligned: one 32-bit load per float, else four byte loads
+    int sx, n;              // size_x, size_x * size_y
+    int startx, starty;     // in [0, size_x) / [0, size_y)
+    int sy;
+    double ox, oy, res;     // ox = position_x + half_x, oy = position_y + half_y
+    double thresh;
+    int mark_unknown;
+    __device__ __forceinline__ float value(int k) const
+    {
+        const unsigned char *q = p + 4 * (size_t)k;
+        if (aligned) return __ldg(reinterpret_cast<const float *>(q));
+        const uint32_t u = (uint32_t)__ldg(q) | ((uint32_t)__ldg(q + 1) << 8) | ((uint32_t)__ldg(q + 2) << 16) | ((uint32_t)__ldg(q + 3) << 24);
+        return __uint_as_float(u);
+    }
+    __device__ __forceinline__ bool element(long long chunk, int lane, int &order, double &wx, double &wy, unsigned char &cost) const
+    {
+        const long long k = chunk * 32 + lane;
+        if (k >= n) return false;
+        const float v = value((int)k);
+        if (v != v && !mark_unknown) return false;
+        cost = ((double)v < thresh) ? COST_LETHAL : COST_FREE;
+        const int ix = (int)(k % sx), iy = (int)(k / sx);
+        const int ux = ix >= startx ? ix - startx : ix - startx + sx, uy = iy >= starty ? iy - starty : iy - starty + sy;
+        wx = ox + res * (double)(-ux);
+        wy = oy + res * (double)(-uy);
+        order = (int)k;
+        return true;
+    }
+    __device__ __forceinline__ unsigned char cost_of(int order) const { return ((double)value(order) < thresh) ? COST_LETHAL : COST_FREE; }
+};
+
 // Pass 1 of the deterministic last-writer scatter: one lane per source element (a warp per 32-element chunk, grid
 // stride), worldToMap, then atomicMax(winner[cell], order).  Lanes of a warp hold increasing orders, so of each group of
 // lanes with equal cells (__match_any_sync) only the highest lane issues the atomic.  The counts and the four touch

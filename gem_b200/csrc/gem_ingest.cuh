@@ -14,7 +14,8 @@
 // the message bytes of up to `tile` consecutive points of one row in shared memory with aligned 16-byte loads (the
 // partial words at the two ends of the buffer bytewise), derives from the spans which message byte feeds each of the 16
 // output bytes, and each thread then assembles its float4 from shared memory and stores it (coalesced).  Points wider
-// than the shared-memory budget are gathered straight from global memory.
+// than the shared-memory budget are gathered straight from global memory.  A second instantiation (REC 32, DESIGN.md
+// f18) derives all 32 record bytes the same way and stores each point as two aligned 16-byte words.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -152,12 +153,26 @@ __device__ __forceinline__ uint4 pc2_assemble(const unsigned char *pt, const int
     return make_uint4(w[0], w[1], w[2], w[3]);
 }
 
-__global__ void __launch_bounds__(PC2_BLOCK) k_decode_pc2(const __grid_constant__ Pc2Params p, uint4 *out)
+// one decoded point at out[i]: REC 16, the float4 {x, y, z, intensity} (struct bytes 0-11, 24-27); REC 32, the whole
+// record as two aligned 16-byte stores
+template <int REC> __device__ __forceinline__ void pc2_store(uint4 *out, unsigned long long i, const unsigned char *pt, const int (&src)[REC]);
+template <> __device__ __forceinline__ void pc2_store<16>(uint4 *out, unsigned long long i, const unsigned char *pt, const int (&src)[16])
+{
+    out[i] = pc2_assemble(pt, src);
+}
+template <> __device__ __forceinline__ void pc2_store<32>(uint4 *out, unsigned long long i, const unsigned char *pt, const int (&src)[32])
+{
+    out[2 * i] = pc2_assemble(pt, *reinterpret_cast<const int(*)[16]>(&src[0]));
+    out[2 * i + 1] = pc2_assemble(pt, *reinterpret_cast<const int(*)[16]>(&src[16]));
+}
+
+// REC 16: gem_decode_pointcloud2's float4 xyzi; REC 32: gem_decode_pointcloud2_records' whole PointXYZRGBICT records (f18)
+template <int REC> __global__ void __launch_bounds__(PC2_BLOCK) k_decode_pc2(const __grid_constant__ Pc2Params p, uint4 *out)
 {
     extern __shared__ uint4 s_raw[];
-    __shared__ int s_src[16]; // per output byte: its byte in the point, or -1 (0)
-    if (threadIdx.x < 16) {
-        const unsigned sb = threadIdx.x < 12 ? threadIdx.x : threadIdx.x + 12; // struct bytes 0-11, 24-27
+    __shared__ int s_src[REC]; // per output byte: its byte in the point, or -1 (0)
+    if (threadIdx.x < REC) {
+        const unsigned sb = REC == 32 ? threadIdx.x : threadIdx.x < 12 ? threadIdx.x : threadIdx.x + 12; // struct bytes
         int src = -1;
         for (int k = 0; k < p.nspans; k++) // M3: in span order, a later span overwrites an earlier one
             if (sb >= p.spans[k].struct_offset && sb < p.spans[k].struct_offset + p.spans[k].size)
@@ -165,9 +180,9 @@ __global__ void __launch_bounds__(PC2_BLOCK) k_decode_pc2(const __grid_constant_
         s_src[threadIdx.x] = src;
     }
     __syncthreads();
-    int src[16];
+    int src[REC];
 #pragma unroll
-    for (int b = 0; b < 16; b++) src[b] = s_src[b];
+    for (int b = 0; b < REC; b++) src[b] = s_src[b];
     const uintptr_t lo = (uintptr_t)p.data, hi = lo + p.data_bytes;
     for (unsigned long long t = blockIdx.x; t < p.tiles; t += gridDim.x) {
         const unsigned long long row = t / p.tiles_per_row;
@@ -181,11 +196,11 @@ __global__ void __launch_bounds__(PC2_BLOCK) k_decode_pc2(const __grid_constant_
             for (unsigned w = threadIdx.x; w < words; w += blockDim.x) s_raw[w] = pc2_load_word(a0 + 16 * (uintptr_t)w, lo, hi);
             __syncthreads();
             if (threadIdx.x < cnt)
-                out[row * p.width + c0 + threadIdx.x] =
-                    pc2_assemble((const unsigned char *)s_raw + ((uintptr_t)base - a0) + (size_t)threadIdx.x * p.point_step, src);
+                pc2_store<REC>(out, row * p.width + c0 + threadIdx.x,
+                               (const unsigned char *)s_raw + ((uintptr_t)base - a0) + (size_t)threadIdx.x * p.point_step, src);
             __syncthreads(); // the next tile overwrites the staged bytes
         } else if (threadIdx.x < cnt) {
-            out[row * p.width + c0 + threadIdx.x] = pc2_assemble(base + (size_t)threadIdx.x * p.point_step, src);
+            pc2_store<REC>(out, row * p.width + c0 + threadIdx.x, base + (size_t)threadIdx.x * p.point_step, src);
         }
     }
 }

@@ -692,6 +692,40 @@ class ElevationMap:
                                                 float(travers_thresh), p, C.byref(mk)), self._h, "gem_costmap_mark_points")
         return self._cost_marks(mk)
 
+    # -- the plugins fed from their subscribed messages (DESIGN.md f18) -----------------------------------------------------
+    @staticmethod
+    def grid_map_msg_parse(msg, layer: str = "traver") -> _lib.GemGridMapLayer:
+        """fromMessage's geometry (G1-G3) and where `layer`'s floats are in the serialised grid_map_msgs/GridMap `msg`
+        (host bytes: bytes, numpy or a CPU tensor; host code, no GPU).  A refused message raises GemError."""
+        lib = _lib.load()
+        p, nb = _host_bytes(msg)
+        g = _lib.GemGridMapLayer()
+        rc = lib.gem_grid_map_msg_parse(p, nb, layer.encode(), C.byref(g))
+        if rc:
+            err = lib.gem_last_error(None)
+            raise _lib.GemError(f"gem_grid_map_msg_parse: {_lib.ERR_NAMES.get(rc, rc)}: {err.decode() if err else ''}")
+        return g
+
+    def costmap_mark_grid(self, g: _lib.GemGridMapLayer, data, window, cost, travers_thresh: float = 0.7,
+                          mark_unknown: bool = True, offset: int = 0) -> dict:
+        """ElevationMapLayer::updateBounds over a message layer: `data` is a CUDA tensor whose bytes from `offset` hold
+        the g.floats floats the descriptor `g` describes (any alignment: e.g. the whole message copied to the device,
+        offset = g.offset); returns the marks as costmap_mark_map does"""
+        if not _is_device(data):
+            raise ValueError("costmap_mark_grid: data must be a CUDA tensor")
+        if data.device.index != self._device_index():
+            raise ValueError(f"costmap_mark_grid: the data are on {data.device}, the map on cuda:{self._device_index()}")
+        nb = int(data.numel() * data.element_size())
+        if offset < 0 or offset + 4 * max(int(g.floats), 0) > nb:
+            raise ValueError(f"costmap_mark_grid: {nb} bytes from offset {offset} do not hold {int(g.floats)} floats")
+        w = self._cost_window(window)
+        p = self._cost_grid(cost, w.size_x, w.size_y, "costmap_mark_grid")
+        mk = _lib.GemCostmapMarks()
+        check(self._lib.gem_costmap_mark_grid(self._h, C.byref(g), C.c_void_p(data.data_ptr() + int(offset)), C.byref(w),
+                                              float(travers_thresh), 1 if mark_unknown else 0, p, C.byref(mk)), self._h,
+              "gem_costmap_mark_grid")
+        return self._cost_marks(mk)
+
     def costmap_update_origin(self, window, new_origin_x: float, new_origin_y: float, fill: int, cost):
         """Costmap2D::updateOrigin of the grid `cost` in place; returns the new window (the grid-aligned origin)"""
         w = self._cost_window(window)
@@ -837,6 +871,25 @@ class ElevationMap:
         torch.cuda.current_stream(data.device).synchronize()
         check(self._lib.gem_decode_pointcloud2(self._h, C.byref(layout.c), _ptr(data), nb, _ptr(out)), self._h,
               "gem_decode_pointcloud2")
+        return out
+
+    def decode_pointcloud2_records(self, layout: PointCloud2Layout, data, out=None, data_bytes: int | None = None):
+        """gem_decode_pointcloud2_records (DESIGN.md f18): the message bytes `data` (a CUDA tensor, any dtype and offset)
+        into `out`, a contiguous (width * height, 8) float32 CUDA tensor (new if None) of whole PointXYZRGBICT records as
+        fromPCLPointCloud2 fills them.  Asynchronous on the map's stream, as decode_pointcloud2."""
+        import torch
+        if not _is_device(data):
+            raise ValueError("decode_pointcloud2_records: data must be a CUDA tensor")
+        n = layout.points
+        if out is None:
+            out = torch.empty((n, 8), dtype=torch.float32, device=data.device)
+        elif not (_is_device(out) and out.element_size() == 4 and out.is_contiguous() and out.numel() >= 8 * n):
+            raise ValueError("decode_pointcloud2_records: out must be a contiguous CUDA tensor of 32-bit words holding "
+                             "8 * width * height of them")
+        nb = int(data.numel() * data.element_size()) if data_bytes is None else int(data_bytes)
+        torch.cuda.current_stream(data.device).synchronize()
+        check(self._lib.gem_decode_pointcloud2_records(self._h, C.byref(layout.c), _ptr(data), nb, _ptr(out)), self._h,
+              "gem_decode_pointcloud2_records")
         return out
 
     def image_to_bgr8(self, encoding: str, src, width: int, height: int, step: int | None = None, out=None,

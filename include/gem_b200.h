@@ -383,7 +383,8 @@ int gem_color_octree_read(gem_map *m, void *out, long long capacity);
  *   layer cell that is not NO_INFORMATION is copied).  layer and master are grids of size_x * size_y.
  * update_origin and combine are asynchronous on the handle's stream and, like mark_points, work on any handle.  No call
  * modifies the map.  Every call rejects a bad window (size <= 0, size_x * size_y >= 2^31, a resolution that is <= 0 or not
- * finite); a rejected call writes nothing.  Out of scope: the elevation_map_available_ subscription gate.  InflationLayer
+ * finite); a rejected call writes nothing.  The plugins fed from their messages, with the elevation_map_available_
+ * gate, are gem_grid_map_msg_parse / gem_costmap_mark_grid / gem_decode_pointcloud2_records (DESIGN.md f18).  InflationLayer
  * is gem_costmap_inflate (DESIGN.md f14); footprint clearing and publishing are gem_costmap_footprint and
  * gem_ros_costmap / gem_ros_footprint (DESIGN.md f17). */
 enum { GEM_COST_FREE = 0, GEM_COST_LETHAL = 254, GEM_COST_UNKNOWN = 255 };
@@ -762,6 +763,56 @@ int gem_ros_footprint(gem_map *m, const gem_ros_header *h, const double *spec_xy
                       double robot_yaw, void *out, long long capacity, long long *bytes_out);
 int gem_costmap_footprint(gem_map *m, const gem_costmap_window *w, const double *spec_xy, int n, double robot_x, double robot_y,
                           double robot_yaw, unsigned char *layer_device, gem_costmap_marks *out);
+
+/* ---- the costmap plugins fed from their subscribed messages (DESIGN.md f18) ----
+ * In GEM's deployment the two layers/ plugins run in move_base and subscribe: ElevationMapLayer::elevationMapCB
+ * (layers/src/elevationMap_layer.cpp:31-38) runs grid_map::GridMapRosConverter::fromMessage on a grid_map_msgs/GridMap,
+ * PointMapLayer::pointMapCB (layers/src/pointMap_layer.cpp:33-41) pcl::fromPCLPointCloud2 on a PointCloud2 of
+ * PointXYZRGBICT.  grid_map 1.6 is unpinned; restated (gem_b200/csrc/gem_gridmsg.h):
+ *   G1 setGeometry: size = (int)round(length / resolution) per axis (round half away from zero), length = size *
+ *      resolution, position = info.pose.position.{x, y} (orientation and z ignored), start index = (outer_start_index,
+ *      inner_start_index).
+ *   G2 layer i of `layers` goes with data[i]; gridMap.add replaces an existing layer, so the LAST layer of a repeated
+ *      name wins.
+ *   G3 Float32MultiArray: dim[0].label "column_index" (column-major) is the only order accepted; rows = dim[1].size,
+ *      cols = dim[0].size; data_offset is ignored; floats beyond rows * cols are ignored.
+ *   G4 GridMapIterator order is the float order of the layer: element k has buffer index (k % size_x, k / size_x) and
+ *      position (position + (0.5 length - 0.5 resolution)) + resolution * (-unwrapped index), in double, per axis; the
+ *      unwrapped index is (index - start) wrapped into [0, size) for any start value.
+ * gem_grid_map_msg_parse: host code, no handle, no GPU.  Walks the serialised GridMap msg[0, bytes) (ROS1 wire format,
+ *   W1 / W2 of gem_rosfmt.h read instead of written) and fills *out with G1's geometry and where `layer`'s floats are:
+ *   offset = the byte offset of its first float in the message, floats = size_x * size_y (G3's rows * cols).  Bytes after
+ *   the message's last field are ignored.  GEM_ERR_INVALID, *out untouched, where fromMessage throws, asserts (compiled
+ *   out) or reads out of bounds: a NULL argument, a truncated message (any string or array count running past `bytes`),
+ *   layers.size() != data.size(), the layer missing, fewer than two dims or dim[0] not "column_index", (rows, cols) not
+ *   (size_x, size_y), fewer floats than rows * cols, a resolution or length that is <= 0 or not finite, a size above
+ *   INT_MAX or size_x * size_y above INT_MAX.
+ * gem_costmap_mark_grid: ElevationMapLayer::updateBounds (:56-84) over the layer a descriptor locates: layer_device points
+ *   at its first float (device memory, any alignment; e.g. msg_device + g->offset of a message copied whole), read in G4
+ *   order with G4's positions; the cost rule, mark_unknown, the last writer and the marks are gem_costmap_mark_map's.
+ *   It reads no map, so it works on any handle (a costmap-only process creates the smallest handle gem_create accepts).
+ *   Host-synchronous; the scratch of the other mark calls.  GEM_ERR_INVALID, nothing written: NULL pointers, a bad
+ *   window, a descriptor that fails G1 / G3's checks.
+ * gem_decode_pointcloud2_records: M1-M3 (f12) into width * height whole 32-byte PointXYZRGBICT records at
+ *   points32_out_device (16-byte aligned): the seven struct fields at their struct offsets, bytes nothing writes 0, M3's
+ *   fast path copying whole points (bytes 12-15 included).  Bytes are copied, never computed on.  The records feed
+ *   gem_costmap_mark_points, gem_ros_cloud, gem_pcd_format, gem_color_octree and the global map as they are.
+ *   Otherwise as gem_decode_pointcloud2. */
+typedef struct gem_grid_map_layer {
+    double resolution;                 /* info.resolution                                                       */
+    double position_x, position_y;     /* info.pose.position                                                    */
+    double length_x, length_y;         /* size * resolution (G1)                                                */
+    int size_x, size_y;                /* (int)round(length / resolution) of the message's lengths (G1)         */
+    int start_x, start_y;              /* outer_start_index, inner_start_index as sent (any value; G4 wraps)     */
+    unsigned long long offset;         /* message byte offset of the layer's first float                        */
+    long long floats;                  /* size_x * size_y                                                       */
+    int column_major;                  /* 1: the only storage order accepted (G3)                               */
+} gem_grid_map_layer;
+int gem_grid_map_msg_parse(const void *msg, unsigned long long bytes, const char *layer, gem_grid_map_layer *out);
+int gem_costmap_mark_grid(gem_map *m, const gem_grid_map_layer *g, const void *layer_device, const gem_costmap_window *w,
+                          double travers_thresh, int mark_unknown, unsigned char *cost_device, gem_costmap_marks *out);
+int gem_decode_pointcloud2_records(gem_map *m, const gem_pointcloud2 *layout, const void *data_device, unsigned long long data_bytes,
+                                   void *points32_out_device);
 
 /* raw layer access (row-major L*L, float or int32 for the colour ids) for tests and
  * checkpoint/restore (the dead G_get_mapinfo/G_set_mapinfo of gpu.cu:457-475). */

@@ -22,6 +22,7 @@
 #include <new>
 #include <stdexcept>
 #include <string>
+#include <utility>
 #include <vector>
 
 #include "../gem_b200.h"
@@ -635,6 +636,30 @@ class ElevationMap {
         check(gem_costmap_footprint(h_, &w, spec_xy.data(), (int)(spec_xy.size() / 2), x, y, yaw, layer_device, &mk), "gem_costmap_footprint");
         return mk;
     }
+    // The costmap plugins fed from their subscribed messages (DESIGN.md f18).  gridMapMsgParse: fromMessage's geometry and
+    // where `layer`'s floats are in a serialised grid_map_msgs/GridMap (host code, throws on a refused message);
+    // costmapMarkGrid: ElevationMapLayer::updateBounds over such a layer's floats (device or pinned memory, any alignment,
+    // e.g. msg_device + g.offset); decodePointCloud2Records: fromPCLPointCloud2 into whole 32-byte PointXYZRGBICT records.
+    static gem_grid_map_layer gridMapMsgParse(const void *msg, size_t bytes, const std::string &layer = "traver")
+    {
+        gem_grid_map_layer g;
+        if (gem_grid_map_msg_parse(msg, bytes, layer.c_str(), &g) != GEM_OK)
+            throw std::runtime_error(std::string("gem_grid_map_msg_parse: ") + gem_last_error(nullptr));
+        return g;
+    }
+    gem_costmap_marks costmapMarkGrid(const gem_grid_map_layer &g, const void *layer_device, const gem_costmap_window &w,
+                                      unsigned char *cost_device, double traversThresh = 0.7, bool markUnknown = true)
+    {
+        gem_costmap_marks mk{};
+        check(gem_costmap_mark_grid(h_, &g, layer_device, &w, traversThresh, markUnknown ? 1 : 0, cost_device, &mk), "gem_costmap_mark_grid");
+        return mk;
+    }
+    void decodePointCloud2Records(const PointCloud2Layout &lay, const void *data_device, unsigned long long data_bytes,
+                                  void *points32_out_device)
+    {
+        check(gem_decode_pointcloud2_records(h_, lay.layout(), data_device, data_bytes, points32_out_device),
+              "gem_decode_pointcloud2_records");
+    }
     // Loop closure (ElevationMapping::updateGlobalMap, ElevationMapping.cpp:773-905), on device-resident submaps of
     // PointXYZRGBICT records: re-pose a submap (:805), and one pass of the pairwise fuse loop (:847-883) -- both clouds
     // come back reduced to one point per cell and compacted, *n_new / *n_old updated.  compat_precedence = true evaluates
@@ -741,6 +766,125 @@ struct CostmapPublisher {
     gem_costmap_publisher state;
     explicit CostmapPublisher(bool alwaysSendFull = false) { gem_costmap_publisher_init(&state, alwaysSendFull ? 1 : 0); }
     void updateBounds(int x0, int xn, int y0, int yn) { gem_costmap_publisher_bounds(&state, x0, xn, y0, yn); }
+};
+
+
+// The descriptor of gem_grid_map_msg_parse from an already deserialised grid_map_msgs::GridMap (or any type with its
+// field names), without ROS headers: G1-G3 of DESIGN.md f18 on the message's fields.  Returns false where
+// gem_grid_map_msg_parse refuses (msg.layers.size() != msg.data.size(), the layer missing, a layout that is not
+// column-major, sizes that do not match, too few floats, a bad resolution or length); else fills g (offset 0) and
+// *floats with the layer's host floats, which the caller copies to the device for costmapMarkGrid.
+template <class GridMapMsg>
+bool gridMapLayerFromFields(const GridMapMsg &msg, const std::string &layer, gem_grid_map_layer &g, const float **floats)
+{
+    const double res = msg.info.resolution, lx = msg.info.length_x, ly = msg.info.length_y;
+    if (msg.layers.size() != msg.data.size() || !(std::isfinite(res) && res > 0.0)) return false;
+    long long found = -1;
+    for (size_t i = 0; i < msg.layers.size(); i++)
+        if (msg.layers[i] == layer) found = (long long)i; // G2: the last of a repeated name
+    if (found < 0) return false;
+    const auto &a = msg.data[(size_t)found];
+    if (a.layout.dim.size() < 2 || a.layout.dim[0].label != "column_index") return false;
+    int size[2];
+    const double len[2] = {lx, ly};
+    for (int k = 0; k < 2; k++) {
+        if (!(std::isfinite(len[k]) && len[k] > 0.0)) return false;
+        const double q = std::round(len[k] / res);
+        if (!(q <= 2147483647.0)) return false;
+        size[k] = (int)q;
+    }
+    const unsigned long long rows = a.layout.dim[1].size, cols = a.layout.dim[0].size;
+    if ((long long)size[0] * size[1] > 2147483647ll || rows != (unsigned long long)size[0] || cols != (unsigned long long)size[1] ||
+        (unsigned long long)a.data.size() < rows * cols)
+        return false;
+    std::memset(&g, 0, sizeof g);
+    g.resolution = res;
+    g.position_x = msg.info.pose.position.x;
+    g.position_y = msg.info.pose.position.y;
+    g.size_x = size[0];
+    g.size_y = size[1];
+    g.length_x = (double)size[0] * res;
+    g.length_y = (double)size[1] * res;
+    g.start_x = (int)msg.outer_start_index;
+    g.start_y = (int)msg.inner_start_index;
+    g.floats = (long long)size[0] * size[1];
+    g.column_major = 1;
+    if (floats) *floats = a.data.data();
+    return true;
+}
+
+// layers/src/elevationMap_layer.cpp's ElevationMapLayer fed from serialised visual_map bytes (e.g. a
+// topic_tools::ShapeShifter's): onMessage is elevationMapCB with its elevation_map_available_ gate (a message is kept only
+// when none is pending; keeping it copies the layer's floats alone into a pinned buffer the device reads); updateBounds
+// marks the layer grid from the pending message and consumes it, or marks nothing.  A refused message throws and leaves
+// the layer as it was.  travers_thresh: the plugin's default 0.5; GEM's yaml sets 0.7.
+class ElevationMapLayer {
+  public:
+    explicit ElevationMapLayer(ElevationMap &map, double traversThresh = 0.5, bool markUnknown = true, std::string layer = "traver")
+        : map_(map), thresh_(traversThresh), markUnknown_(markUnknown), layer_(std::move(layer)) {}
+    bool available() const { return pending_; }
+    bool onMessage(const void *msg, size_t bytes)
+    {
+        if (pending_) return false;
+        g_ = ElevationMap::gridMapMsgParse(msg, bytes, layer_);
+        floats_.resize((size_t)g_.floats * 4 + 4);
+        std::memcpy(&floats_[0], static_cast<const uint8_t *>(msg) + g_.offset, (size_t)g_.floats * 4);
+        pending_ = true;
+        return true;
+    }
+    gem_costmap_marks updateBounds(const gem_costmap_window &w, unsigned char *layer_grid_device)
+    {
+        if (!pending_) return noMarks();
+        pending_ = false;
+        return map_.costmapMarkGrid(g_, &floats_[0], w, layer_grid_device, thresh_, markUnknown_);
+    }
+    static gem_costmap_marks noMarks()
+    {
+        const double inf = std::numeric_limits<double>::infinity();
+        return gem_costmap_marks{0, 0, inf, inf, -inf, -inf};
+    }
+
+  private:
+    ElevationMap &map_;
+    double thresh_;
+    bool markUnknown_;
+    std::string layer_;
+    bool pending_ = false;
+    gem_grid_map_layer g_{};
+    PinnedBytes floats_;
+};
+
+// layers/src/pointMap_layer.cpp's PointMapLayer fed from history_point: onMessage is pointMapCB (the cloud, given by its
+// layout and bytes in device or pinned memory, replaces the stored one, decoded into whole PointXYZRGBICT records in a
+// pinned buffer); updateBounds re-marks the stored cloud every time, nothing before the first message.  Calls take effect
+// in call order.  The records stay in pinned host memory, so each re-mark reads them across PCIe (32 bytes per point);
+// for clouds of millions of points keep the records in device memory and call costmapMarkPoints on them instead.
+class PointMapLayer {
+  public:
+    explicit PointMapLayer(ElevationMap &map, double traversThresh = 0.5) : map_(map), thresh_(traversThresh) {}
+    void onMessage(const PointCloud2Layout &lay, const void *data, unsigned long long bytes)
+    {
+        gem_pc2_mapping mp;
+        if (gem_pointcloud2_mapping(lay.layout(), bytes, &mp) != GEM_OK)
+            throw std::runtime_error(std::string("gem_pointcloud2_mapping: ") + gem_last_error(nullptr));
+        map_.sync(); // the stored records may still be read
+        records_.resize((size_t)mp.points > 0 ? (size_t)mp.points : 1);
+        map_.decodePointCloud2Records(lay, data, bytes, records_.data());
+        n_ = (long long)mp.points;
+    }
+    gem_costmap_marks updateBounds(const gem_costmap_window &w, unsigned char *layer_grid_device)
+    {
+        if (n_ < 0) return ElevationMapLayer::noMarks();
+        return map_.costmapMarkPoints(records_.data(), (size_t)n_, w, layer_grid_device, thresh_);
+    }
+    long long points() const { return n_; }
+    const PointXYZRGBICT *records() const { return records_.data(); }
+
+  private:
+    ElevationMap &map_;
+    double thresh_;
+    long long n_ = -1;
+    std::vector<PointXYZRGBICT, PinnedAllocator<PointXYZRGBICT>> records_;
 };
 
 } // namespace gem_b200
