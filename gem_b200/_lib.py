@@ -165,6 +165,7 @@ PC2_FIELDS = ["x", "y", "z", "rgb", "intensity", "covariance", "travers"]
 PCD_BINARY, PCD_RGB_UINT32 = 1, 2   # GEM_PCD_*
 COSTMAP_PUB_KINDS = {0: "none", 1: "full", 2: "update"}   # GEM_COSTMAP_PUB_*
 PCD_LINE_MAX, PCD_HEADER_MAX = 105, 512   # GEM_PCD_LINE_MAX, GEM_PCD_HEADER_MAX
+COLOUR_LOOKUPS = {"image": 0, "node": 1}   # GEM_COLOUR_LOOKUP_IMAGE / _NODE (gem_set_colour_lookup)
 IMAGE_ENCODINGS = {"bgr8": 3, "rgb8": 3, "bgra8": 4, "rgba8": 4, "mono8": 1}   # the byte-permutation encodings: channels
 
 PROF_CLASSES = ["bin", "fold_long", "unused", "fold", "clear_floor", "features", "raytrace", "other", "route"]
@@ -198,6 +199,7 @@ SYMBOLS = {
     "gem_opt_move": (C.c_int, [_P, _FP, C.c_float, _FP]),
     "gem_closeloop": (C.c_int, [_P, _FP, C.c_float]),
     "gem_colourise_points": (C.c_int, [_P, _P, C.c_int, C.POINTER(C.c_double), C.POINTER(C.c_double), _P, C.c_int, C.c_int, C.c_int, _P]),
+    "gem_set_colour_lookup": (C.c_int, [_P, C.c_int]),
     "gem_export_layers": (C.c_int, [_P, C.POINTER(_P)]),
     "gem_export_layers_begin": (C.c_int, [_P, C.POINTER(_P)]),
     "gem_export_layers_end": (C.c_int, [_P]),

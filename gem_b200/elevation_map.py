@@ -438,6 +438,14 @@ class ElevationMap:
         p = (C.c_float * 2)(*[float(v) for v in update_position])
         check(self._lib.gem_closeloop(self._h, p, float(height_update)), self._h, "gem_closeloop")
 
+    def set_colour_lookup(self, mode: str):
+        """gem_set_colour_lookup: "image" (the default) reads every point's own pixel of the unmodified image; "node"
+        reproduces the node's loop, where each in-image point paints its colour into its four neighbour pixels for the
+        points after it (DESIGN.md f19).  Applies to colourise and to add_pointcloud2_host_async's image."""
+        if mode not in _lib.COLOUR_LOOKUPS:
+            raise ValueError(f"set_colour_lookup: mode {mode!r} is not one of {sorted(_lib.COLOUR_LOOKUPS)}")
+        check(self._lib.gem_set_colour_lookup(self._h, _lib.COLOUR_LOOKUPS[mode]), self._h, "gem_set_colour_lookup")
+
     def colourise(self, xyzi, T_camera, T_lidar, bgr, rgba_out):
         """ElevationMapping.cpp:331-381 on the device: xyzi (n,4) float32 device tensor (intensity zeroed for
         points outside the image), bgr (H,W,3) uint8 device tensor, rgba_out (n,4) uint8 device tensor"""

@@ -233,7 +233,20 @@ int gem_closeloop(gem_map *m, const float update_position[2], float height_updat
  * right before the fusion path.  T_camera: row-major 3x4 "T.camera", T_lidar: row-major 4x4 "T.lidar"
  * (kitti_intrinsic.yaml / yq_intrinsic.yaml), bgr: device BGR8 image.  Writes rgba_out (r,g,b,255 or
  * 0,0,0,0) and zeroes the intensity of points that do not project into the image, exactly like the
- * reference loop; the reference's debug circle drawing into the image (:372) is not reproduced. */
+ * reference loop.  The bgr image is never written.  Which pixel a point's colour comes from is the handle's
+ * colour lookup mode (gem_set_colour_lookup):
+ *   GEM_COLOUR_LOOKUP_IMAGE (the default): every point reads its own pixel of the unmodified image.
+ *   GEM_COLOUR_LOOKUP_NODE: the node's loop (DESIGN.md f19).  It takes the points in array order against a working copy
+ *     of the image; an in-image point reads its working pixel (mx, my), then cv::circle(img, midPoint, 1, colour) (:370)
+ *     paints that colour into whichever of (mx +- 1, my) and (mx, my +- 1) lie inside the image (no diagonals).  So a
+ *     point's colour is the image pixel of the root of its chain of parents, parent(i) being the largest j < i in the
+ *     image whose pixel is a 4-neighbour of i's.  Unpinned (restated: OpenCV is not available).  Runs on the handle's
+ *     stream with device scratch that grows on demand (GEM_ERR_NOMEM, nothing written, when it cannot).
+ * gem_set_colour_lookup: the mode of one handle, used by gem_colourise_points and the image path of
+ *   gem_add_pointcloud2_host_async from the next call on.  Another value is GEM_ERR_INVALID and leaves the mode as it
+ *   was.  Tiled handles are accepted (the lookup reads no map). */
+enum { GEM_COLOUR_LOOKUP_IMAGE = 0, GEM_COLOUR_LOOKUP_NODE = 1 };
+int gem_set_colour_lookup(gem_map *m, int mode);
 int gem_colourise_points(gem_map *m, void *xyzi_device, int n, const double T_camera[12], const double T_lidar[16],
                          const unsigned char *bgr_device, int width, int height, int row_stride_bytes,
                          void *rgba_out_device);
@@ -573,11 +586,13 @@ int gem_mls_upsample(gem_map *m, const void *points32_device, int n, const gem_m
  *   channels * width / 3 * width); src and dst may not overlap.  Asynchronous on the handle's stream.
  * gem_add_pointcloud2_host_async: Callback's lines 311-381 plus processpoints in one call: the message bytes (and the
  *   image, when img != NULL) go to the device on the copy stream, are decoded into the staging set of
- *   gem_add_points_host_async, colourised there by gem_colourise_points' kernel (img != NULL: intensities of points that
- *   do not project are zeroed before the add reads them; img == NULL: no colour, like rgba NULL) and added pipelined.
+ *   gem_add_points_host_async, colourised there as gem_colourise_points does by the handle's colour lookup mode (img !=
+ *   NULL: intensities of points that do not project are zeroed before the add reads them; img == NULL: no colour, like
+ *   rgba NULL) and added pipelined.
  *   It shares the three-slot ring of gem_add_points_host_async (staging sets, events, counters): the two calls may be
- *   interleaved on one handle.  Its own message and image staging buffers grow on demand, after synchronising the
- *   handle's streams and before anything is enqueued (a failed growth is GEM_ERR_NOMEM and changes nothing).  Host
+ *   interleaved on one handle.  Its own message and image staging buffers, and the NODE lookup's scratch, grow on demand,
+ *   after synchronising the handle's streams and before anything is enqueued (a failed growth is GEM_ERR_NOMEM and
+ *   changes nothing).  Host
  *   buffers: pinned memory must stay untouched until the call after next (or gem_sync); pageable memory is accepted and
  *   may be reused as soon as the call returns (CUDA stages it before the copy call returns), so a ROS message's data can
  *   be passed as it is.  width * height > max_points is refused; width * height == 0 flushes. */

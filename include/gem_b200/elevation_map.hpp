@@ -270,6 +270,9 @@ class ElevationMap {
         check(gem_colourise_points(h_, xyzi_device, (int)n, T_camera, T_lidar, bgr_device, width, height, row_stride_bytes,
                                    rgba_out_device), "gem_colourise_points");
     }
+    // which pixel colourise and addPointCloud2HostAsync's image give a point: GEM_COLOUR_LOOKUP_IMAGE (the default, its
+    // own pixel of the unmodified image) or GEM_COLOUR_LOOKUP_NODE (the node's loop with its circle painting; DESIGN.md f19)
+    void setColourLookup(int mode) { check(gem_set_colour_lookup(h_, mode), "gem_set_colour_lookup"); }
     // RobotMotionMapUpdater::update -> Mapvar_update (RobotMotionMapUpdater.cpp:81)
     void update(float variance_increment) { check(gem_var_update(h_, variance_increment), "gem_var_update"); }
     // upstream ElevationMap::fuse: Map_feature + show's write-back into grid_map layers
