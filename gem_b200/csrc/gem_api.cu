@@ -411,12 +411,10 @@ FrameParams make_frame(const gem_frame *f)
     memset(&p, 0, sizeof p);
     for (int i = 0; i < 12; i++) p.T[i] = f->T[i];
     for (int i = 0; i < 3; i++) { p.sJ[i] = f->sensor_jacobian[i]; p.P[i] = f->P_mul_C_BM_transpose[i]; }
-    p.has_rot = 0;
     for (int i = 0; i < 9; i++) {
         p.rotVar[i] = f->rotation_variance[i];
         p.CSBT[i] = f->C_SB_transpose[i];
         p.Bskew[i] = f->B_r_BS_skew[i];
-        if (f->rotation_variance[i] != 0.0f) p.has_rot = 1;
     }
     p.lo = f->rel_lower;
     p.hi = f->rel_upper;

@@ -12,15 +12,25 @@ from gem_b200 import build
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
-def compile_with_shim(out_dir, name, extra_flags=()):
-    """tests/cxx/<name>.cpp + the shim, linked against libgem_b200.so, built into out_dir (the tree may be read-only)"""
+def compile_with_shim(out_dir, name, extra_flags=(), shared=False):
+    """tests/cxx/<name>.cpp + the shim, linked against libgem_b200.so, built into out_dir (the tree may be read-only):
+    a program, or with shared=True the shared library lib<name>.so"""
     lib = build.build()
-    exe = os.path.join(str(out_dir), name)
+    exe = os.path.join(str(out_dir), f"lib{name}.so" if shared else name)
     srcs = [os.path.join(ROOT, "tests", "cxx", name + ".cpp"), os.path.join(ROOT, "compat", "gpu_process_shim.cpp")]
-    cmd = ["g++", "-O2", "-std=c++14", "-Wall", *extra_flags, "-I", os.path.join(ROOT, "include"), "-I", os.path.join(ROOT, "oracle", "mini_eigen"),
+    cmd = ["g++", "-O2", "-std=c++14", "-Wall", *extra_flags, *(("-shared", "-fPIC") if shared else ()),
+           "-I", os.path.join(ROOT, "include"), "-I", os.path.join(ROOT, "oracle", "mini_eigen"),
            "-o", exe] + srcs + ["-L", os.path.dirname(lib), "-lgem_b200", "-Wl,-rpath," + os.path.dirname(lib)]
     subprocess.run(cmd, check=True)
     return exe
+
+
+def test_shim_harness_builds_with_the_nine_entry_points(tmp_path):
+    so = compile_with_shim(tmp_path, "shim_harness", shared=True)
+    out = subprocess.run(["nm", "-D", "--defined-only", so], capture_output=True, text=True).stdout
+    for sym in ("ref_init", "ref_move", "ref_process_points", "ref_fuse", "ref_var_update", "ref_map_feature",
+                "ref_raytracing", "ref_optmove", "ref_closeloop"):
+        assert f" {sym}" in out, sym
 
 
 def test_three_thread_program_compiles(tmp_path):

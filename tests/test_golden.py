@@ -20,6 +20,7 @@ import gem_b200
 from gem_b200 import synth
 import ref_lib
 from oracle_lib import OracleMap
+from shim_lib import shim  # noqa: F401  (a fixture)
 
 GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "gem_golden_v2.npz")
 L, RES, NFRAMES, STRIDE = 96, 0.2, 3, 11
@@ -131,13 +132,16 @@ def test_oracle_reproduces_reference_golden(gold, frames):
 
 
 @pytest.mark.gpu
-def test_cuda_path_reproduces_reference_golden(gold, frames):
+def test_cuda_path_reproduces_reference_golden(gold, frames, shim):
+    """through the C ABI and through the drop-in shim's nine entry points (compat/gpu_process_shim.cpp)"""
     oracle_out = drive(OracleMap(L, RES, compat_box_filter=True), frames)
     ref = reference(gold, oracle_out)
-    out = drive(gem_b200.ElevationMap(L, RES, compat_box_filter=True), frames)
-    check_against_reference(out, ref, "gem_b200 CUDA path")
-    for k in range(NFRAMES):   # bit-exact vs the oracle incl. the feature layers
-        for name in ("feat_traver", "feat_rough", "feat_slope"):
-            a, b = out[f"f{k}_{name}"], oracle_out[f"f{k}_{name}"]
-            same = (bits(a) == bits(b)) | (np.isnan(a) & np.isnan(b))
-            assert same.all(), f"frame {k} {name}"
+    for what, m in (("gem_b200 CUDA path", gem_b200.ElevationMap(L, RES, compat_box_filter=True)),
+                    ("the drop-in shim", shim(L, RES))):
+        out = drive(m, frames)
+        check_against_reference(out, ref, what)
+        for k in range(NFRAMES):   # bit-exact vs the oracle incl. the feature layers
+            for name in ("feat_traver", "feat_rough", "feat_slope"):
+                a, b = out[f"f{k}_{name}"], oracle_out[f"f{k}_{name}"]
+                same = (bits(a) == bits(b)) | (np.isnan(a) & np.isnan(b))
+                assert same.all(), f"{what}: frame {k} {name}"

@@ -7,6 +7,7 @@ arithmetic definition, the tests assert the stronger property: every layer bit-i
 import numpy as np
 import pytest
 
+import frame_cases as fc
 import gem_b200
 from gem_b200 import synth
 from helpers import assert_layers_equal, split_rgb
@@ -235,17 +236,17 @@ def test_structured_light_c3_small():
 
 
 def test_rotation_variance_term():
-    c = synth.random_cloud(20000, seed=11, extent=9.0)
-    T = synth.pose_matrix(0.0, 0.0, 0.0, 0.7)
-    rv = np.diag([1e-4, 2e-4, 3e-4]).astype(np.float32)
-    rv[0, 1] = rv[1, 0] = 5e-5
-    csb = synth.pose_matrix(0, 0, 0, 0.2)[:3, :3].T
-    f = laser_frame(T, rotation_variance=rv, C_SB_transpose=csb, P_mul_C_BM_transpose=[0.01, -0.02, 0.99],
-                    B_r_BS_skew=[0, -0.3, 0.1, 0.3, 0, -0.2, -0.1, 0.2, 0])
-    g, o = both(200, 0.1, compat_box_filter=False)
-    for m in (g, o):
-        m.add(c["xyzi"], c["rgba"], f)
-    assert_layers_equal(g, o, what="rotation variance")
+    """the fused add path on the frames whose rotation term tests/test_reference_pin_frames.py pins the oracle to the
+    reference with (device = oracle = reference): every constant non-trivial, the rotation term alone, and a rotation
+    Jacobian that overflows under a zero rotation variance (NaN variances, as in the reference)"""
+    for c in fc.frame_cases():
+        g, o = both(c.L, c.res, compat_box_filter=True)
+        for m in (g, o):
+            m.move(c.position)
+            m.add(c.xyzi, c.rgba, c.frame)
+        assert_layers_equal(g, o, what=f"rotation variance, {c.name}")
+        if c.name == "overflow":
+            assert np.isnan(o.get_layer("variance")).sum() > 20
 
 
 def test_odd_length_and_edges():
