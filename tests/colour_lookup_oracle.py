@@ -8,14 +8,12 @@ All three take xyzi (n, 4) float32, the two transforms and a BGR8 image of shape
 pixels in the first 3 * width bytes of each row, and return (xyzi with intensities zeroed outside the image, rgba)."""
 from __future__ import annotations
 
-import atexit
 import ctypes as C
 import os
-import shutil
-import subprocess
-import tempfile
 
 import numpy as np
+
+import native
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 SRC = os.path.join(HERE, "orc_colour_lookup.c")
@@ -25,12 +23,7 @@ _lib = None
 def load():
     global _lib
     if _lib is None:
-        tmp = tempfile.mkdtemp(prefix="gem_orc_colour_")
-        atexit.register(shutil.rmtree, tmp, True)
-        so = os.path.join(tmp, "liborc_colour_lookup.so")
-        subprocess.run(["gcc", "-O2", "-std=gnu11", "-fPIC", "-ffp-contract=off", "-fno-fast-math", "-Wall", "-Wextra",
-                        "-shared", "-o", so, SRC], check=True)
-        lib = C.CDLL(so)
+        lib = native.shared_library("orc_colour_lookup", [SRC], native.ORACLE_C)
         P = C.c_void_p
         lib.orc_colourise_node.restype = C.c_int
         lib.orc_colourise_node.argtypes = [P, C.c_int, P, P, P, C.c_int, C.c_int, C.c_int, P]

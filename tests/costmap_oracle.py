@@ -5,14 +5,12 @@ A window is (origin_x, origin_y, resolution, size_x, size_y); a grid a (size_y, 
 {marked, lethal, min_x, min_y, max_x, max_y}."""
 from __future__ import annotations
 
-import atexit
 import ctypes as C
 import os
-import shutil
-import subprocess
-import tempfile
 
 import numpy as np
+
+import native
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 SRC = os.path.join(HERE, "orc_costmap.c")
@@ -32,12 +30,7 @@ class Marks(C.Structure):
 def load():
     global _lib
     if _lib is None:
-        tmp = tempfile.mkdtemp(prefix="gem_orc_costmap_")
-        atexit.register(shutil.rmtree, tmp, True)
-        so = os.path.join(tmp, "liborc_costmap.so")
-        subprocess.run(["gcc", "-O2", "-std=gnu11", "-fPIC", "-ffp-contract=off", "-fno-fast-math", "-Wall", "-Wextra",
-                        "-shared", "-o", so, SRC, "-lm"], check=True)
-        lib = C.CDLL(so)
+        lib = native.shared_library("orc_costmap", [SRC], native.ORACLE_C, ["-lm"])
         P = C.c_void_p
         lib.orc_mark_map.argtypes = [C.c_int, C.c_double, P, P, P, C.POINTER(Window), C.c_double, C.c_int, P, C.POINTER(Marks)]
         lib.orc_mark_map.restype = None

@@ -12,22 +12,17 @@ All compiled into temporary directories (the checkout may be read-only).
 """
 from __future__ import annotations
 
-import atexit
 import ctypes as C
 import math
 import os
-import shutil
 import struct
-import subprocess
-import tempfile
 
 import numpy as np
 
+import native
 import rosmsg_oracle as ro
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-CSRC = os.path.join(os.path.dirname(HERE), "gem_b200", "csrc")
-INCLUDE = os.path.join(os.path.dirname(HERE), "include")
 INT_MAX = 2**31 - 1
 GEM_FOOTPRINT = ((-0.64, -0.40), (-0.64, 0.40), (0.64, 0.40), (0.64, -0.40))
 
@@ -268,19 +263,10 @@ class PublisherState(C.Structure):   # gem_costmap_publisher
 _orc = _host = None
 
 
-def _tmp(prefix):
-    d = tempfile.mkdtemp(prefix=prefix)
-    atexit.register(shutil.rmtree, d, True)
-    return d
-
-
 def orc():
     global _orc
     if _orc is None:
-        so = os.path.join(_tmp("gem_orc_footprint_"), "liborc_footprint.so")
-        subprocess.run(["gcc", "-O2", "-std=gnu11", "-fPIC", "-ffp-contract=off", "-fno-fast-math", "-Wall", "-shared", "-o", so,
-                        os.path.join(HERE, "orc_footprint.c"), "-lm"], check=True)
-        lib = C.CDLL(so)
+        lib = native.shared_library("orc_footprint", [os.path.join(HERE, "orc_footprint.c")], native.ORACLE_C, ["-lm"])
         P = C.c_void_p
         lib.orc_footprint.argtypes = [P, P, P, C.c_int, C.c_double, C.c_double, C.c_double, P, P, C.c_long]
         lib.orc_footprint.restype = C.c_long
@@ -293,10 +279,7 @@ def orc():
 def host():
     global _host
     if _host is None:
-        so = os.path.join(_tmp("gem_costmap_pub_"), "libcostmap_pub_host.so")
-        subprocess.run(["g++", "-O2", "-std=c++14", "-fPIC", "-ffp-contract=off", "-Wall", "-Wextra", "-shared", "-I", CSRC, "-o", so,
-                        os.path.join(HERE, "costmap_pub_host.cpp")], check=True)
-        lib = C.CDLL(so)
+        lib = native.shared_library("costmap_pub_host", [os.path.join(HERE, "costmap_pub_host.cpp")], native.HOST_CXX)
         P, ll = C.c_void_p, C.c_longlong
         hdr = [C.c_uint, C.c_uint, C.c_uint, C.c_char_p]
         lib.cp_translate.argtypes, lib.cp_translate.restype = [C.c_uint], C.c_int

@@ -8,15 +8,12 @@ gem_b200.ElevationMap (reset, push, update) and report their state as `state()`:
 (keyframes, 4, 4) poses, (keyframes, 2) centres)."""
 from __future__ import annotations
 
-import atexit
 import ctypes as C
 import os
-import shutil
-import subprocess
-import tempfile
 
 import numpy as np
 
+import native
 import oracle_lib
 import refuse_cases as rc
 from gem_b200 import submaps as sm
@@ -31,13 +28,9 @@ def load():
     global _lib
     if _lib is None:
         oracle_lib.load()  # builds oracle/libgem_oracle.so
-        tmp = tempfile.mkdtemp(prefix="gem_orc_global_map_")
-        atexit.register(shutil.rmtree, tmp, True)
-        so = os.path.join(tmp, "liborc_global_map.so")
-        subprocess.run(["gcc", "-O2", "-std=gnu11", "-fPIC", "-ffp-contract=off", "-fno-fast-math", "-Wall", "-Wextra",
-                        "-shared", "-I", oracle_lib.ODIR, "-o", so, SRC, "-L", oracle_lib.ODIR, "-lgem_oracle",
-                        "-Wl,-rpath," + oracle_lib.ODIR, "-lm"], check=True)
-        lib = C.CDLL(so)
+        odir = oracle_lib.ODIR
+        lib = native.shared_library("orc_global_map", [SRC], native.ORACLE_C + ["-I", odir],
+                                    ["-L", odir, "-lgem_oracle", "-Wl,-rpath," + odir, "-lm"])
         P = C.c_void_p
         lib.orc_gmap_create.restype = P
         lib.orc_gmap_destroy.argtypes = [P]

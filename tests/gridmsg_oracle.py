@@ -10,21 +10,17 @@
 - cases(): the crafted messages."""
 from __future__ import annotations
 
-import atexit
 import ctypes as C
 import math
 import os
-import shutil
 import struct
-import subprocess
-import tempfile
 
 import numpy as np
 
 import costmap_oracle as co
+import native
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-CSRC = os.path.join(os.path.dirname(HERE), "gem_b200", "csrc")
 FIELDS = ("resolution", "position_x", "position_y", "length_x", "length_y", "size_x", "size_y", "start_x", "start_y",
           "offset", "floats", "column_major")
 INT_MAX = 2**31 - 1
@@ -201,19 +197,10 @@ def co_lethal():
 _orc = _host = None
 
 
-def _tmp(prefix):
-    t = tempfile.mkdtemp(prefix=prefix)
-    atexit.register(shutil.rmtree, t, True)
-    return t
-
-
 def orc():
     global _orc
     if _orc is None:
-        so = os.path.join(_tmp("gem_orc_gridmsg_"), "liborc_gridmsg.so")
-        subprocess.run(["gcc", "-O2", "-std=gnu11", "-fPIC", "-ffp-contract=off", "-fno-fast-math", "-Wall", "-shared", "-I", HERE,
-                        "-o", so, os.path.join(HERE, "orc_gridmsg.c"), "-lm"], check=True)
-        lib = C.CDLL(so)
+        lib = native.shared_library("orc_gridmsg", [os.path.join(HERE, "orc_gridmsg.c")], native.ORACLE_C + ["-I", HERE], ["-lm"])
         P = C.c_void_p
         lib.orc_grid_map_parse.argtypes = [C.c_char_p, C.c_ulonglong, C.c_char_p, C.POINTER(Layer)]
         lib.orc_grid_map_parse.restype = C.c_int
@@ -228,10 +215,7 @@ def orc():
 def host():
     global _host
     if _host is None:
-        so = os.path.join(_tmp("gem_gridmsg_host_"), "libgridmsg_host.so")
-        subprocess.run(["g++", "-O2", "-std=c++14", "-fPIC", "-ffp-contract=off", "-Wall", "-Wextra", "-shared", "-I", CSRC, "-o", so,
-                        os.path.join(HERE, "gridmsg_host.cpp")], check=True)
-        lib = C.CDLL(so)
+        lib = native.shared_library("gridmsg_host", [os.path.join(HERE, "gridmsg_host.cpp")], native.HOST_CXX)
         lib.gm_parse.argtypes = [C.c_char_p, C.c_ulonglong, C.c_char_p, C.POINTER(Layer)]
         lib.gm_parse.restype = C.c_int
         lib.gm_layer_ok.argtypes = [C.POINTER(Layer)]

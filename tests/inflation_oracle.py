@@ -6,15 +6,13 @@ A grid is a (size_y, size_x) uint8 array; params a dict {inflation_radius, cost_
 inflate_unknown}; a rect (min_i, min_j, max_i, max_j)."""
 from __future__ import annotations
 
-import atexit
 import ctypes as C
 import math
 import os
-import shutil
-import subprocess
-import tempfile
 
 import numpy as np
+
+import native
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 SRC = os.path.join(HERE, "orc_inflate.c")
@@ -26,12 +24,7 @@ FREE, INSCRIBED, LETHAL, UNKNOWN = 0, 253, 254, 255
 def load():
     global _lib
     if _lib is None:
-        tmp = tempfile.mkdtemp(prefix="gem_orc_inflate_")
-        atexit.register(shutil.rmtree, tmp, True)
-        so = os.path.join(tmp, "liborc_inflate.so")
-        subprocess.run(["gcc", "-O2", "-std=gnu11", "-fPIC", "-ffp-contract=off", "-fno-fast-math", "-Wall", "-Wextra",
-                        "-shared", "-o", so, SRC, "-lm"], check=True)
-        lib = C.CDLL(so)
+        lib = native.shared_library("orc_inflate", [SRC], native.ORACLE_C, ["-lm"])
         lib.orc_inflate.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_double, C.c_double, C.c_double, C.c_double, C.c_int,
                                     C.c_int, C.c_int, C.c_int, C.c_int]
         lib.orc_inflate.restype = C.c_longlong

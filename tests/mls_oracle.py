@@ -7,18 +7,15 @@ written records, info a dict {count, processed, fitted, skipped, max_neighbours}
 error.  detail() returns what M2-M4 give one point."""
 from __future__ import annotations
 
-import atexit
 import ctypes as C
 import os
-import shutil
-import subprocess
-import tempfile
 
 import numpy as np
 
+import native
+
 HERE = os.path.dirname(os.path.abspath(__file__))
 SRC = os.path.join(HERE, "orc_mls.c")
-CSRC = os.path.join(os.path.dirname(HERE), "gem_b200", "csrc")
 UPSAMPLING = {"none": 0, "random_uniform_density": 1}
 GEM = {"search_radius": 0.5, "sqr_gauss_param": 0.25, "polynomial_fit": True, "order": 5,
        "upsampling": "random_uniform_density", "point_density": 1000, "seed": 0}
@@ -43,12 +40,7 @@ class Detail(C.Structure):
 def load():
     global _lib
     if _lib is None:
-        tmp = tempfile.mkdtemp(prefix="gem_orc_mls_")
-        atexit.register(shutil.rmtree, tmp, True)
-        so = os.path.join(tmp, "liborc_mls.so")
-        subprocess.run(["gcc", "-O2", "-std=gnu11", "-fPIC", "-ffp-contract=off", "-fno-fast-math", "-Wall", "-Wextra",
-                        "-I", CSRC, "-shared", "-o", so, SRC, "-lm"], check=True)
-        lib = C.CDLL(so)
+        lib = native.shared_library("orc_mls", [SRC], native.ORACLE_C + ["-I", native.CSRC], ["-lm"])
         lib.orc_mls_upsample.argtypes = [C.c_void_p, C.c_int, C.POINTER(Params), C.c_void_p, C.c_longlong, C.POINTER(Info)]
         lib.orc_mls_upsample.restype = C.c_int
         lib.orc_mls_detail.argtypes = [C.c_void_p, C.c_int, C.POINTER(Params), C.c_int, C.POINTER(Detail), C.c_void_p]

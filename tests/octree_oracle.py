@@ -2,14 +2,12 @@
 temporary directory (the checkout may be read-only).  TEST INFRASTRUCTURE ONLY."""
 from __future__ import annotations
 
-import atexit
 import ctypes as C
 import os
-import shutil
-import subprocess
-import tempfile
 
 import numpy as np
+
+import native
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 SRC = os.path.join(HERE, "orc_color_octree.c")
@@ -19,12 +17,7 @@ _lib = None
 def load():
     global _lib
     if _lib is None:
-        tmp = tempfile.mkdtemp(prefix="gem_orc_color_octree_")
-        atexit.register(shutil.rmtree, tmp, True)
-        so = os.path.join(tmp, "liborc_color_octree.so")
-        subprocess.run(["gcc", "-O2", "-std=gnu11", "-fPIC", "-ffp-contract=off", "-fno-fast-math", "-Wall", "-Wextra",
-                        "-shared", "-o", so, SRC, "-lm"], check=True)
-        lib = C.CDLL(so)
+        lib = native.shared_library("orc_color_octree", [SRC], native.ORACLE_C, ["-lm"])
         P = C.c_void_p
         lib.orc_octree_build.argtypes = [C.c_int, P, C.c_double, P]
         lib.orc_octree_build.restype = P

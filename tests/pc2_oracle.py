@@ -6,14 +6,12 @@ fills them (stale bytes DEFINED as 0), mapping a dict {spans, fast_path, matched
 layout.  xyzi(records) is what the device decode writes: struct bytes 0-11 and 24-27 as an (n, 4) float32 array."""
 from __future__ import annotations
 
-import atexit
 import ctypes as C
 import os
-import shutil
-import subprocess
-import tempfile
 
 import numpy as np
+
+import native
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 SRC = os.path.join(HERE, "orc_pointcloud2.c")
@@ -41,11 +39,7 @@ class Mapping(C.Structure):
 def load():
     global _lib
     if _lib is None:
-        tmp = tempfile.mkdtemp(prefix="gem_orc_pc2_")
-        atexit.register(shutil.rmtree, tmp, True)
-        so = os.path.join(tmp, "liborc_pointcloud2.so")
-        subprocess.run(["gcc", "-O2", "-std=gnu11", "-fPIC", "-Wall", "-Wextra", "-shared", "-o", so, SRC], check=True)
-        lib = C.CDLL(so)
+        lib = native.shared_library("orc_pointcloud2", [SRC], native.FORMAT_C)
         lib.orc_pc2_decode.argtypes = [C.POINTER(Cloud), C.c_void_p, C.c_ulonglong, C.c_void_p, C.POINTER(Mapping)]
         lib.orc_pc2_decode.restype = C.c_int
         _lib = lib

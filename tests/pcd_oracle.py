@@ -10,42 +10,27 @@ Both libraries are compiled into a temporary directory (the checkout may be read
 uint32 arrays (32-byte PointXYZRGBICT records); flags are GEM_PCD_BINARY = 1 and GEM_PCD_RGB_UINT32 = 2."""
 from __future__ import annotations
 
-import atexit
 import ctypes as C
 import math
 import os
-import shutil
 import struct
-import subprocess
-import tempfile
 
 import numpy as np
 
+import native
+
 HERE = os.path.dirname(os.path.abspath(__file__))
-CSRC = os.path.join(os.path.dirname(HERE), "gem_b200", "csrc")
 BINARY, RGB_UINT32 = 1, 2
 FIELDS = ["x", "y", "z", "rgb", "intensity", "covariance", "travers"]
 WORDS = [0, 1, 2, 4, 6, 5, 7]     # each field's 32-bit word in the record, in registration order
 _orc = None
 _fmt = None
-_tmp = None
-
-
-def _tmpdir():
-    global _tmp
-    if _tmp is None:
-        _tmp = tempfile.mkdtemp(prefix="gem_orc_pcd_")
-        atexit.register(shutil.rmtree, _tmp, True)
-    return _tmp
 
 
 def load():
     global _orc
     if _orc is None:
-        so = os.path.join(_tmpdir(), "liborc_pcd.so")
-        subprocess.run(["gcc", "-O2", "-std=gnu11", "-fPIC", "-Wall", "-Wextra", "-shared", "-o", so,
-                        os.path.join(HERE, "orc_pcd.c"), "-lm"], check=True)
-        lib = C.CDLL(so)
+        lib = native.shared_library("orc_pcd", [os.path.join(HERE, "orc_pcd.c")], native.FORMAT_C, ["-lm"])
         lib.orc_pcd_header.argtypes = [C.c_longlong, C.c_int, C.c_char_p, C.c_int]
         lib.orc_pcd_header.restype = C.c_int
         lib.orc_pcd_data.argtypes = [C.c_void_p, C.c_longlong, C.c_int, C.c_void_p, C.c_longlong]
@@ -57,10 +42,7 @@ def load():
 def load_fmt():
     global _fmt
     if _fmt is None:
-        so = os.path.join(_tmpdir(), "libpcd_fmt_host.so")
-        subprocess.run(["g++", "-O2", "-std=c++14", "-fPIC", "-Wall", "-Wextra", "-I", CSRC, "-shared", "-o", so,
-                        os.path.join(HERE, "pcd_fmt_host.cpp"), "-lm"], check=True)
-        lib = C.CDLL(so)
+        lib = native.shared_library("pcd_fmt_host", [os.path.join(HERE, "pcd_fmt_host.cpp")], native.FORMAT_CXX, ["-lm"])
         lib.pcd_fmt_one.argtypes = [C.c_uint32, C.c_int, C.c_char_p]
         lib.pcd_fmt_one.restype = C.c_int
         lib.pcd_fmt_compare_range.argtypes = [C.c_uint64, C.c_uint64, C.POINTER(C.c_uint32)]

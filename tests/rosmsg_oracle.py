@@ -10,19 +10,15 @@
 """
 from __future__ import annotations
 
-import atexit
 import ctypes as C
 import os
-import shutil
 import struct
-import subprocess
-import tempfile
 
 import numpy as np
 
+import native
+
 HERE = os.path.dirname(os.path.abspath(__file__))
-CSRC = os.path.join(os.path.dirname(HERE), "gem_b200", "csrc")
-INCLUDE = os.path.join(os.path.dirname(HERE), "include")
 
 GRID_LAYERS = ["elevation", "variance", "rough", "slope", "traver", "color_r", "color_g", "color_b", "intensity"]
 ICT_FIELDS = [("x", 0), ("y", 4), ("z", 8), ("rgb", 16), ("intensity", 24), ("covariance", 20), ("travers", 28)]
@@ -212,19 +208,13 @@ def decode_submap(b: bytes, keyframe_len: int) -> dict:
 
 # ---- the library's host framing (gem_rosfmt.h) ------------------------------------------------------------------------
 _fmt = None
-_tmp = None
 
 
 def fmt_host():
     """ctypes binding of tests/rosmsg_fmt_host.cpp (g++, into a temporary directory)"""
-    global _fmt, _tmp
+    global _fmt
     if _fmt is None:
-        _tmp = tempfile.mkdtemp(prefix="gem_rosfmt_")
-        atexit.register(shutil.rmtree, _tmp, True)
-        so = os.path.join(_tmp, "librosfmt_host.so")
-        subprocess.run(["g++", "-O2", "-std=c++14", "-fPIC", "-Wall", "-Wextra", "-shared", "-I", CSRC, "-o", so,
-                        os.path.join(HERE, "rosmsg_fmt_host.cpp")], check=True)
-        lib = C.CDLL(so)
+        lib = native.shared_library("rosfmt_host", [os.path.join(HERE, "rosmsg_fmt_host.cpp")], native.FORMAT_CXX)
         ll, P = C.c_longlong, C.c_void_p
         hdr = [C.c_uint, C.c_uint, C.c_uint, C.c_char_p]
         lib.ros_fmt_grid_map.argtypes = hdr + [C.c_int, C.c_double, C.c_double, C.c_double, C.c_int, C.c_int, P, P, ll]

@@ -7,15 +7,12 @@ through OracleMap.fuse_points.  Laser and structured-light frames go to OracleMa
 """
 from __future__ import annotations
 
-import atexit
 import ctypes as C
 import os
-import shutil
-import subprocess
-import tempfile
 
 import numpy as np
 
+import native
 import oracle_lib
 
 HERE = os.path.dirname(os.path.abspath(__file__))
@@ -33,13 +30,9 @@ def load():
     global _lib
     if _lib is None:
         oracle_lib.load()  # builds oracle/libgem_oracle.so
-        tmp = tempfile.mkdtemp(prefix="gem_orc_sensor_models_")
-        atexit.register(shutil.rmtree, tmp, True)
-        so = os.path.join(tmp, "liborc_sensor_models.so")
-        subprocess.run(["gcc", "-O2", "-std=gnu11", "-fPIC", "-ffp-contract=off", "-fno-fast-math", "-Wall", "-Wextra",
-                        "-shared", "-I", oracle_lib.ODIR, "-o", so, SRC, "-L", oracle_lib.ODIR, "-lgem_oracle",
-                        "-Wl,-rpath," + oracle_lib.ODIR, "-lm"], check=True)
-        lib = C.CDLL(so)
+        odir = oracle_lib.ODIR
+        lib = native.shared_library("orc_sensor_models", [SRC], native.ORACLE_C + ["-I", odir],
+                                    ["-L", odir, "-lgem_oracle", "-Wl,-rpath," + odir, "-lm"])
         P = C.c_void_p
         lib.orc_sm_variances.restype = C.c_float
         lib.orc_sm_variances.argtypes = [C.POINTER(OrcSmSensor), C.c_float, C.c_float, C.c_float, C.c_int,

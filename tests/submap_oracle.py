@@ -7,14 +7,12 @@ dict (find, erase, insert, :740-747); a dict iterates in insertion order, which 
 """
 from __future__ import annotations
 
-import atexit
 import ctypes as C
 import os
-import shutil
-import subprocess
-import tempfile
 
 import numpy as np
+
+import native
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 SRC = os.path.join(HERE, "orc_grid_cloud.c")
@@ -24,12 +22,7 @@ _lib = None
 def load():
     global _lib
     if _lib is None:
-        tmp = tempfile.mkdtemp(prefix="gem_orc_grid_cloud_")
-        atexit.register(shutil.rmtree, tmp, True)
-        so = os.path.join(tmp, "liborc_grid_cloud.so")
-        subprocess.run(["gcc", "-O2", "-std=gnu11", "-fPIC", "-ffp-contract=off", "-fno-fast-math", "-Wall", "-Wextra",
-                        "-shared", "-o", so, SRC, "-lm"], check=True)
-        lib = C.CDLL(so)
+        lib = native.shared_library("orc_grid_cloud", [SRC], native.ORACLE_C, ["-lm"])
         P = C.c_void_p
         lib.orc_grid_cloud.argtypes = [C.c_int, C.c_double, P, P, P, P, P, P, P, P, P, P, C.POINTER(C.c_int)]
         _lib = lib

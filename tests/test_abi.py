@@ -7,6 +7,7 @@ import re
 import pytest
 
 import gem_b200
+import native
 from gem_b200 import _lib, build
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -72,30 +73,8 @@ def test_product_does_not_reference_the_oracle():
     assert "oracle" not in open(os.path.join(ROOT, "include", "gem_b200.h")).read().lower()
 
 
-def test_ctypes_struct_layouts_match_the_header(tmp_path):
+def test_ctypes_struct_layouts_match_the_header():
     """the ctypes mirrors in gem_b200/_lib.py must have the sizes and field offsets the C compiler gives the structs of
     include/gem_b200.h (a drift here corrupts every call silently)"""
-    import ctypes as C
-    import subprocess
-    from gem_b200 import _lib
-    structs = {"gem_config": _lib.GemConfig, "gem_sensor_model": _lib.GemSensorModel, "gem_frame": _lib.GemFrame,
-               "gem_stats": _lib.GemStats, "gem_profile": _lib.GemProfile}
-    lines = ['#include <stdio.h>', '#include <stddef.h>', '#include "gem_b200.h"', 'int main(void) {']
-    for cname, cls in structs.items():
-        lines.append(f'  printf("{cname} size %zu\\n", sizeof({cname}));')
-        for fname, _ in cls._fields_:
-            lines.append(f'  printf("{cname} {fname} %zu\\n", offsetof({cname}, {fname}));')
-    lines += ['  return 0;', '}']
-    src = tmp_path / "layout.c"
-    src.write_text("\n".join(lines))
-    exe = tmp_path / "layout"
-    subprocess.run(["gcc", "-std=c99", "-I", os.path.join(ROOT, "include"), "-o", str(exe), str(src)], check=True)
-    out = subprocess.run([str(exe)], capture_output=True, text=True, check=True).stdout
-    seen = 0
-    for ln in out.splitlines():
-        cname, field, val = ln.split()
-        cls = structs[cname]
-        expect = C.sizeof(cls) if field == "size" else getattr(cls, field).offset
-        assert int(val) == expect, (cname, field, int(val), expect)
-        seen += 1
-    assert seen == sum(len(c._fields_) + 1 for c in structs.values())
+    native.assert_struct_layouts({"gem_config": _lib.GemConfig, "gem_sensor_model": _lib.GemSensorModel,
+                                  "gem_frame": _lib.GemFrame, "gem_stats": _lib.GemStats, "gem_profile": _lib.GemProfile})

@@ -1,14 +1,11 @@
 """The global-map octrees, CPU side: the oracle (tests/orc_color_octree.c) against the independent Python restatement of
 tests/octree_cases.py, bit for bit, on every crafted family and on natural split clouds; the stream decoder's structure
 and O5 checks on the oracle's streams; the ctypes mirror of gem_octree; the C++ facade program compiles."""
-import ctypes as C
-import os
-import subprocess
-import tempfile
 
 import numpy as np
 import pytest
 
+import native
 import octree_cases as oc
 import octree_oracle
 import split_oracle
@@ -16,7 +13,6 @@ import submap_oracle
 from gem_b200 import synth
 from oracle_lib import OracleMap
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 CASES = oc.crafted_cases()
 
 
@@ -81,23 +77,11 @@ def test_oracle_matches_restatement_on_split_clouds(res):
         check_against_restatement(sp[part], res, (part, res))
 
 
-def test_gem_octree_struct_matches_the_header(tmp_path):
+def test_gem_octree_struct_matches_the_header():
     import gem_b200._lib as L
-    src = tmp_path / "layout.c"
-    src.write_text('#include <stdio.h>\n#include <stddef.h>\n#include "gem_b200.h"\nint main(void){gem_octree s;'
-                   'printf("%zu %zu %zu %zu %zu\\n", sizeof s, offsetof(gem_octree, nodes), offsetof(gem_octree, leaves),'
-                   ' offsetof(gem_octree, inserted), offsetof(gem_octree, skipped));return 0;}\n')
-    exe = tmp_path / "layout"
-    subprocess.run(["gcc", "-I", os.path.join(ROOT, "include"), "-o", str(exe), str(src)], check=True)
-    got = [int(v) for v in subprocess.run([str(exe)], capture_output=True, text=True, check=True).stdout.split()]
-    S = L.GemOctree
-    assert got == [C.sizeof(S), S.nodes.offset, S.leaves.offset, S.inserted.offset, S.skipped.offset]
+    assert {"nodes", "leaves", "inserted", "skipped"} <= {f for f, _ in L.GemOctree._fields_}
+    native.assert_struct_layouts({"gem_octree": L.GemOctree}, std=None)
 
 
 def test_facade_program_with_color_octree_compiles():
-    tmp = tempfile.mkdtemp(prefix="gem_color_octree_cxx_")
-    obj = os.path.join(tmp, "color_octree_smoke.o")
-    subprocess.run(["g++", "-O2", "-std=c++14", "-Wall", "-Werror", "-I", os.path.join(ROOT, "include"), "-c", "-o", obj,
-                    os.path.join(ROOT, "tests", "cxx", "color_octree_smoke.cpp")], check=True)
-    os.remove(obj)
-    os.rmdir(tmp)
+    native.facade_compiles("color_octree_smoke")

@@ -3,15 +3,14 @@ against the oracle, tests/orc_color_octree.c: the stream and every count of gem_
 tests/octree_cases.py, large random clouds, natural split clouds through global_octrees (a small map and the c2
 snapshot), the API's behaviour, and the C++ facade program run against the library."""
 import ctypes as C
-import os
 import subprocess
-import tempfile
 
 import numpy as np
 import pytest
 import torch
 
 import gem_b200
+import native
 import octree_cases as oc
 import octree_oracle
 from gem_b200 import synth
@@ -203,16 +202,7 @@ def test_tiled_handle_is_refused():
 
 
 def test_facade_color_octree_program_runs():
-    from gem_b200 import build
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    lib = build.build()
-    tmp = tempfile.mkdtemp(prefix="gem_color_octree_")
-    exe = os.path.join(tmp, "color_octree_smoke")
-    subprocess.run(["g++", "-O2", "-std=c++14", "-Wall", "-I", os.path.join(root, "include"), "-o", exe,
-                    os.path.join(root, "tests", "cxx", "color_octree_smoke.cpp"), "-L", os.path.dirname(lib), "-lgem_b200",
-                    "-Wl,-rpath," + os.path.dirname(lib)], check=True)
+    exe = native.facade_program("color_octree_smoke")
     r = subprocess.run([exe], capture_output=True, text=True, timeout=300)
-    os.remove(exe)
-    os.rmdir(tmp)
     print(r.stdout, r.stderr)
     assert r.returncode == 0 and "color_octree ok" in r.stdout, r.stdout + r.stderr

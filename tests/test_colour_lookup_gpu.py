@@ -3,7 +3,6 @@ against the literal oracle (tests/orc_colour_lookup.c) on every crafted case and
 as before, gem_add_pointcloud2_host_async in NODE mode against the oracle chain decode -> orc_colourise_node -> fuse for
 every accepted encoding, refusals, and the C++ facade."""
 import ctypes as C
-import os
 import subprocess
 
 import numpy as np
@@ -13,11 +12,12 @@ import torch
 import colour_lookup_cases as cc
 import colour_lookup_oracle as clo
 import gem_b200
+import native
 import oracle_lib
 import pc2_cases as pc
 import pc2_oracle
 import sensor_models_oracle as smo
-from gem_b200 import CameraImage, PointCloud2Layout, _lib, build, synth
+from gem_b200 import CameraImage, PointCloud2Layout, _lib, synth
 from helpers import assert_layers_equal
 from oracle_lib import OracleMap
 
@@ -242,12 +242,7 @@ def test_pointcloud2_refusals_change_nothing():
 
 
 def test_cxx_facade_program(tmp_path):
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    lib = build.build()
-    exe = str(tmp_path / "colour_lookup_smoke")
-    subprocess.run(["g++", "-O2", "-std=c++14", "-Wall", "-I", os.path.join(root, "include"), "-o", exe,
-                    os.path.join(root, "tests", "cxx", "colour_lookup_smoke.cpp"), "-L", os.path.dirname(lib), "-lgem_b200",
-                    "-Wl,-rpath," + os.path.dirname(lib)], check=True)
+    exe = native.facade_program("colour_lookup_smoke", tmp_path)
     c = cc.lidar_008()
     T, pos = synth.hdl64_pose(0)
     W, H = c["width"], c["height"]

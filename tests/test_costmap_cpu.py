@@ -2,19 +2,15 @@
 tests/costmap_cases.py, bit for bit (grids, counts, exact double bounds), on every crafted case; the ctypes mirrors of
 gem_costmap_window / gem_costmap_marks against the C compiler; the rolling-window helper's bounds and rect arithmetic; the
 C++ facade program compiles."""
-import ctypes as C
-import os
-import subprocess
-import tempfile
 
 import numpy as np
 import pytest
 
 import costmap_cases as cc
 import costmap_oracle
+import native
 from gem_b200 import costmap
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 POINTS = cc.point_cases()
 MAPS = cc.map_cases()
 ROLLS = cc.roll_cases()
@@ -132,40 +128,12 @@ def test_size_in_meters_and_roll_target():
     assert cm.size_in_meters() == ((75 - 1 + 0.5) * 0.2, (1000 - 1 + 0.5) * 0.2)
 
 
-def test_costmap_structs_match_the_header(tmp_path):
+def test_costmap_structs_match_the_header():
     import gem_b200._lib as L
-    structs = {"gem_costmap_window": L.GemCostmapWindow, "gem_costmap_marks": L.GemCostmapMarks}
-    lines = ['#include <stdio.h>', '#include <stddef.h>', '#include "gem_b200.h"', 'int main(void) {']
-    for cname, cls in structs.items():
-        lines.append(f'  printf("{cname} size %zu\\n", sizeof({cname}));')
-        for fname, _ in cls._fields_:
-            lines.append(f'  printf("{cname} {fname} %zu\\n", offsetof({cname}, {fname}));')
-    lines.append('  printf("consts %d %d %d %d %d\\n", GEM_COST_FREE, GEM_COST_LETHAL, GEM_COST_UNKNOWN, GEM_COSTMAP_MAX,'
-                 ' GEM_COSTMAP_OVERWRITE);')
-    lines += ['  return 0;', '}']
-    src = tmp_path / "layout.c"
-    src.write_text("\n".join(lines))
-    exe = tmp_path / "layout"
-    subprocess.run(["gcc", "-std=c99", "-I", os.path.join(ROOT, "include"), "-o", str(exe), str(src)], check=True)
-    out = subprocess.run([str(exe)], capture_output=True, text=True, check=True).stdout
-    seen = 0
-    for ln in out.splitlines():
-        if ln.startswith("consts"):
-            assert [int(v) for v in ln.split()[1:]] == [L.COST_FREE, L.COST_LETHAL, L.COST_UNKNOWN, L.COSTMAP_MODES["max"],
-                                                        L.COSTMAP_MODES["overwrite"]]
-            continue
-        cname, field, val = ln.split()
-        cls = structs[cname]
-        expect = C.sizeof(cls) if field == "size" else getattr(cls, field).offset
-        assert int(val) == expect, (cname, field, int(val), expect)
-        seen += 1
-    assert seen == sum(len(c._fields_) + 1 for c in structs.values())
+    consts = {"GEM_COST_FREE": L.COST_FREE, "GEM_COST_LETHAL": L.COST_LETHAL, "GEM_COST_UNKNOWN": L.COST_UNKNOWN,
+              "GEM_COSTMAP_MAX": L.COSTMAP_MODES["max"], "GEM_COSTMAP_OVERWRITE": L.COSTMAP_MODES["overwrite"]}
+    native.assert_struct_layouts({"gem_costmap_window": L.GemCostmapWindow, "gem_costmap_marks": L.GemCostmapMarks}, consts)
 
 
 def test_facade_program_with_costmaps_compiles():
-    tmp = tempfile.mkdtemp(prefix="gem_costmap_cxx_")
-    obj = os.path.join(tmp, "costmap_smoke.o")
-    subprocess.run(["g++", "-O2", "-std=c++14", "-Wall", "-Werror", "-I", os.path.join(ROOT, "include"), "-c", "-o", obj,
-                    os.path.join(ROOT, "tests", "cxx", "costmap_smoke.cpp")], check=True)
-    os.remove(obj)
-    os.rmdir(tmp)
+    native.facade_compiles("costmap_smoke")

@@ -4,9 +4,7 @@ grid_map of natural maps (both sources, scrolled so that the wrap seam runs thro
 global costmap driven through a moving robot with gem_b200.costmap, the c2 geometry, the map left unchanged, every error
 path, and the C++ facade program run against the library."""
 import ctypes as C
-import os
 import subprocess
-import tempfile
 
 import numpy as np
 import pytest
@@ -15,6 +13,7 @@ import torch
 import costmap_cases as cc
 import costmap_oracle
 import gem_b200
+import native
 from gem_b200 import _lib, costmap, synth
 
 pytestmark = pytest.mark.gpu
@@ -421,16 +420,7 @@ def test_tiled_handle():
 
 
 def test_facade_costmap_program_runs():
-    from gem_b200 import build
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    lib = build.build()
-    tmp = tempfile.mkdtemp(prefix="gem_costmap_")
-    exe = os.path.join(tmp, "costmap_smoke")
-    subprocess.run(["g++", "-O2", "-std=c++14", "-Wall", "-I", os.path.join(root, "include"), "-o", exe,
-                    os.path.join(root, "tests", "cxx", "costmap_smoke.cpp"), "-L", os.path.dirname(lib), "-lgem_b200",
-                    "-Wl,-rpath," + os.path.dirname(lib)], check=True)
+    exe = native.facade_program("costmap_smoke")
     r = subprocess.run([exe], capture_output=True, text=True, timeout=300)
-    os.remove(exe)
-    os.rmdir(tmp)
     print(r.stdout, r.stderr)
     assert r.returncode == 0 and "costmap ok" in r.stdout, r.stdout + r.stderr

@@ -5,7 +5,6 @@ map, scrolled and after gem_opt_move); the history_point round trip (gem_ros_clo
 the records back) and the f12 crafted layouts against orc_pc2_decode; the two layer classes through Costmap.update with
 inflation and a CostmapPublisher against a host model of the plugins over the oracle; refusals; the C++ facade."""
 import ctypes as C
-import os
 import subprocess
 
 import numpy as np
@@ -15,11 +14,12 @@ import torch
 import costmap_cases as cc
 import costmap_oracle
 import gridmsg_oracle as gm
+import native
 import pc2_cases as pc
 import pc2_oracle
 import rosmsg_cases as rc
 import gem_b200
-from gem_b200 import GemError, PointCloud2Layout, _lib, build, costmap, synth
+from gem_b200 import GemError, PointCloud2Layout, _lib, costmap, synth
 from gem_b200.elevation_map import RosHeader
 
 pytestmark = pytest.mark.gpu
@@ -436,12 +436,7 @@ def test_layer_classes_follow_the_robot():
 
 
 def test_cxx_facade_program(tmp_path):
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    lib = build.build()
-    exe = str(tmp_path / "costmap_ingest_smoke")
-    subprocess.run(["g++", "-O2", "-std=c++14", "-Wall", "-I", os.path.join(root, "include"), "-o", exe,
-                    os.path.join(root, "tests", "cxx", "costmap_ingest_smoke.cpp"), "-L", os.path.dirname(lib), "-lgem_b200",
-                    "-Wl,-rpath," + os.path.dirname(lib)], check=True)
+    exe = native.facade_program("costmap_ingest_smoke", tmp_path)
     prefix = str(tmp_path / "cxx")
     r = subprocess.run([exe, prefix], capture_output=True, text=True, timeout=300)
     print(r.stdout, r.stderr)

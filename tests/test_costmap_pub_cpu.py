@@ -4,17 +4,15 @@ P1-P4, gem_footprint.h F1-F4, built with g++) against the encoder, the publisher
 oracles, and the gem_costmap_publisher layout against the C compiler."""
 import ctypes as C
 import math
-import os
-import subprocess
 
 import numpy as np
 import pytest
 
 import costmap_pub_oracle as cp
+import native
 import rosmsg_oracle as ro
 from gem_b200 import _lib
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 SIZES = [(1, 1), (1, 37), (41, 1), (75, 75), (257, 33), (1000, 1000)]
 FRAME_ID_LENGTHS = list(range(21)) + [300]
 
@@ -295,16 +293,7 @@ def test_publisher_refuses_bounds_outside_the_grid():
         assert p.publish(h, W, grid)[2] == -1 and p.state() == before
 
 
-def test_publisher_struct_layout(tmp_path):
-    lines = ['#include <stdio.h>', '#include <stddef.h>', '#include "gem_b200.h"', 'int main(void) {',
-             '  printf("size %zu\\n", sizeof(gem_costmap_publisher));']
-    for f, _ in _lib.GemCostmapPublisher._fields_:
-        lines.append(f'  printf("{f} %zu\\n", offsetof(gem_costmap_publisher, {f}));')
-    lines += ['  return 0;', '}']
-    (tmp_path / "l.c").write_text("\n".join(lines))
-    subprocess.run(["gcc", "-std=c99", "-I", os.path.join(ROOT, "include"), "-o", str(tmp_path / "l"), str(tmp_path / "l.c")], check=True)
-    out = subprocess.run([str(tmp_path / "l")], capture_output=True, text=True, check=True).stdout.split()
-    got = dict(zip(out[::2], (int(v) for v in out[1::2])))
-    assert got.pop("size") == C.sizeof(_lib.GemCostmapPublisher) == C.sizeof(cp.PublisherState)
-    assert got == {f: getattr(_lib.GemCostmapPublisher, f).offset for f, _ in _lib.GemCostmapPublisher._fields_}
+def test_publisher_struct_layout():
+    native.assert_struct_layouts({"gem_costmap_publisher": _lib.GemCostmapPublisher})
+    assert C.sizeof(_lib.GemCostmapPublisher) == C.sizeof(cp.PublisherState)
     assert _lib.GemCostmapPublisher._fields_ == cp.PublisherState._fields_

@@ -5,7 +5,6 @@ changing yaws) and global costmap (inflated) through 12 moves, against the oracl
 nothing and keep the publisher; and the C++ facade program."""
 import ctypes as C
 import math
-import os
 import subprocess
 
 import numpy as np
@@ -16,9 +15,10 @@ import costmap_cases as cc
 import costmap_oracle
 import costmap_pub_oracle as cp
 import inflation_oracle as O
+import native
 import rosmsg_oracle as ro
 import gem_b200
-from gem_b200 import _lib, build, costmap, synth
+from gem_b200 import _lib, costmap, synth
 from gem_b200.elevation_map import RosHeader
 
 pytestmark = pytest.mark.gpu
@@ -301,12 +301,7 @@ def test_refusals_write_nothing_and_keep_the_publisher(emap):
 
 
 def test_cxx_facade_program(emap, tmp_path):
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    lib = build.build()
-    exe = str(tmp_path / "costmap_publish_smoke")
-    subprocess.run(["g++", "-O2", "-std=c++14", "-Wall", "-I", os.path.join(root, "include"), "-o", exe,
-                    os.path.join(root, "tests", "cxx", "costmap_publish_smoke.cpp"), "-L", os.path.dirname(lib), "-lgem_b200",
-                    "-Wl,-rpath," + os.path.dirname(lib)], check=True)
+    exe = native.facade_program("costmap_publish_smoke", tmp_path)
     r = subprocess.run([exe, str(tmp_path / "cxx")], capture_output=True, text=True, timeout=300)
     print(r.stdout, r.stderr)
     assert r.returncode == 0 and "costmap publish ok kinds=1,2,0,1" in r.stdout, r.stdout + r.stderr

@@ -7,7 +7,7 @@ import subprocess
 
 import pytest
 
-from gem_b200 import build
+import native
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
@@ -15,14 +15,9 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 def compile_with_shim(out_dir, name, extra_flags=(), shared=False):
     """tests/cxx/<name>.cpp + the shim, linked against libgem_b200.so, built into out_dir (the tree may be read-only):
     a program, or with shared=True the shared library lib<name>.so"""
-    lib = build.build()
-    exe = os.path.join(str(out_dir), f"lib{name}.so" if shared else name)
-    srcs = [os.path.join(ROOT, "tests", "cxx", name + ".cpp"), os.path.join(ROOT, "compat", "gpu_process_shim.cpp")]
-    cmd = ["g++", "-O2", "-std=c++14", "-Wall", *extra_flags, *(("-shared", "-fPIC") if shared else ()),
-           "-I", os.path.join(ROOT, "include"), "-I", os.path.join(ROOT, "oracle", "mini_eigen"),
-           "-o", exe] + srcs + ["-L", os.path.dirname(lib), "-lgem_b200", "-Wl,-rpath," + os.path.dirname(lib)]
-    subprocess.run(cmd, check=True)
-    return exe
+    srcs = [os.path.join(native.CXX, name + ".cpp"), os.path.join(ROOT, "compat", "gpu_process_shim.cpp")]
+    flags = [*extra_flags, *(("-shared", "-fPIC") if shared else ()), "-I", os.path.join(ROOT, "oracle", "mini_eigen")]
+    return native.facade_program(f"lib{name}.so" if shared else name, out_dir, flags, sources=srcs)
 
 
 def test_shim_harness_builds_with_the_nine_entry_points(tmp_path):

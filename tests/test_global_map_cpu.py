@@ -4,13 +4,13 @@ tests/global_map_cases.py, and the library's host pose arithmetic and pair sched
 against the restatement, bit for bit."""
 import ctypes as C
 import os
-import subprocess
 
 import numpy as np
 import pytest
 
 import global_map_cases as gc
 import global_map_oracle as go
+import native
 from gem_b200 import submaps as sm
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -41,12 +41,8 @@ def test_cases_reach_their_decisions():
 
 
 @pytest.fixture(scope="module")
-def host(tmp_path_factory):
-    so = str(tmp_path_factory.mktemp("gm") / "libgm_host.so")
-    subprocess.run(["g++", "-O2", "-std=c++14", "-fPIC", "-shared", "-ffp-contract=off", "-Wall", "-Wextra", "-Werror",
-                    "-I", os.path.join(ROOT, "gem_b200", "csrc"), "-o", so, os.path.join(ROOT, "tests", "global_map_host.cpp")],
-                   check=True)
-    lib = C.CDLL(so)
+def host():
+    lib = native.shared_library("gm_host", [os.path.join(ROOT, "tests", "global_map_host.cpp")], native.HOST_CXX + ["-Werror"])
     lib.gm_relative_pose.argtypes = [C.c_void_p] * 3
     lib.gm_pair_schedule.restype = C.c_int
     lib.gm_pair_schedule.argtypes = [C.c_void_p, C.c_int, C.c_double, C.c_void_p, C.c_int]

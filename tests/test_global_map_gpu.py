@@ -16,13 +16,13 @@ import torch
 import gem_b200
 import global_map_cases as gc
 import global_map_oracle as go
+import native
 import pcd_oracle
 import rosmsg_oracle as ro
 from gem_b200 import submaps as sm
 from gem_b200 import synth
 
 pytestmark = pytest.mark.gpu
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 GEM_ERR_INVALID = 1
 
 
@@ -234,12 +234,8 @@ def test_update_beside_the_add_path():
 
 
 def test_facade_global_map_program(emap, tmp_path):
-    from gem_b200 import build
-    lib = build.build()
-    exe = str(tmp_path / "global_map_smoke")
-    subprocess.run(["g++", "-O2", "-std=c++14", "-Wall", "-I", os.path.join(ROOT, "include"), "-I", "/usr/local/cuda/include",
-                    "-o", exe, os.path.join(ROOT, "tests", "cxx", "global_map_smoke.cpp"), "-L", os.path.dirname(lib), "-lgem_b200",
-                    "-L", "/usr/local/cuda/lib64", "-lcudart", "-Wl,-rpath," + os.path.dirname(lib)], check=True)
+    exe = native.facade_program("global_map_smoke", tmp_path, ["-I", "/usr/local/cuda/include"],
+                                ["-L", "/usr/local/cuda/lib64", "-lcudart"])
     subs, kf, opt = exact_chain()
     with open(tmp_path / "in.bin", "wb") as f:
         f.write(np.int32(len(subs)).tobytes())

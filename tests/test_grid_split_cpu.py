@@ -1,21 +1,16 @@
 """The global-map filter, CPU side: the oracle (tests/orc_grid_split.c) against the independent cKDTree restatement of
 tests/split_cases.py, bit for bit, on natural snapshot clouds and on every crafted family; the ctypes mirror of
 gem_grid_split; the C++ facade program compiles."""
-import ctypes as C
-import os
-import subprocess
-import tempfile
 
 import numpy as np
 import pytest
 
+import native
 import split_cases
 import split_oracle
 import submap_oracle
 from gem_b200 import synth
 from oracle_lib import OracleMap
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
 def f64bits(v):
@@ -76,23 +71,11 @@ def test_oracle_matches_restatement_on_snapshot_clouds(L):
         assert got["valid"] == rec.shape[0]
 
 
-def test_grid_split_struct_matches_the_header(tmp_path):
+def test_grid_split_struct_matches_the_header():
     import gem_b200._lib as L
-    src = tmp_path / "layout.c"
-    src.write_text('#include <stdio.h>\n#include <stddef.h>\n#include "gem_b200.h"\nint main(void){gem_grid_split s;'
-                   'printf("%zu %zu %zu %zu\\n", sizeof s, offsetof(gem_grid_split, obstacle), offsetof(gem_grid_split, mean),'
-                   ' offsetof(gem_grid_split, threshold));return 0;}\n')
-    exe = tmp_path / "layout"
-    subprocess.run(["gcc", "-I", os.path.join(ROOT, "include"), "-o", str(exe), str(src)], check=True)
-    got = [int(v) for v in subprocess.run([str(exe)], capture_output=True, text=True, check=True).stdout.split()]
-    S = L.GemGridSplit
-    assert got == [C.sizeof(S), S.obstacle.offset, S.mean.offset, S.threshold.offset]
+    assert {"obstacle", "mean", "threshold"} <= {f for f, _ in L.GemGridSplit._fields_}
+    native.assert_struct_layouts({"gem_grid_split": L.GemGridSplit}, std=None)
 
 
 def test_facade_program_with_grid_cloud_split_compiles():
-    tmp = tempfile.mkdtemp(prefix="gem_grid_split_cxx_")
-    obj = os.path.join(tmp, "grid_split_smoke.o")
-    subprocess.run(["g++", "-O2", "-std=c++14", "-Wall", "-Werror", "-I", os.path.join(ROOT, "include"), "-c", "-o", obj,
-                    os.path.join(ROOT, "tests", "cxx", "grid_split_smoke.cpp")], check=True)
-    os.remove(obj)
-    os.rmdir(tmp)
+    native.facade_compiles("grid_split_smoke")

@@ -13,6 +13,7 @@ import pytest
 import torch
 
 import gem_b200
+import native
 import split_oracle
 from gem_b200 import synth
 
@@ -274,19 +275,8 @@ def test_errors():
 
 
 def test_facade_grid_split_program_runs():
-    import os
     import subprocess
-    import tempfile
-    from gem_b200 import build
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    lib = build.build()
-    tmp = tempfile.mkdtemp(prefix="gem_grid_split_")
-    exe = os.path.join(tmp, "grid_split_smoke")
-    subprocess.run(["g++", "-O2", "-std=c++14", "-Wall", "-I", os.path.join(root, "include"), "-o", exe,
-                    os.path.join(root, "tests", "cxx", "grid_split_smoke.cpp"), "-L", os.path.dirname(lib), "-lgem_b200",
-                    "-Wl,-rpath," + os.path.dirname(lib)], check=True)
+    exe = native.facade_program("grid_split_smoke")
     r = subprocess.run([exe], capture_output=True, text=True, timeout=300)
-    os.remove(exe)
-    os.rmdir(tmp)
     print(r.stdout, r.stderr)
     assert r.returncode == 0 and "grid_split ok" in r.stdout, r.stdout + r.stderr

@@ -2,18 +2,15 @@
 restatement of tests/inflation_oracle.py on every crafted case, the witnesses shown to be witnesses, the footprint's
 inscribed radius, the bounds sequence of InflationLayer.update_bounds, Costmap.update without inflation unchanged, and
 the ctypes struct against the C compiler."""
-import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 import pytest
 
 import inflation_cases as ic
 import inflation_oracle as O
+import native
 from gem_b200 import costmap
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 CASES = {c[0]: c for c in ic.all_cases()}
 
 
@@ -152,26 +149,10 @@ def test_update_without_inflation_and_radius_zero(monkeypatch):
     assert rect2 == rect and fake.calls[-1] == ("inflate", 0.0, rect)
 
 
-def test_inflation_struct_matches_the_header(tmp_path):
+def test_inflation_struct_matches_the_header():
     import gem_b200._lib as L
-    cls = L.GemCostmapInflation
-    lines = ['#include <stdio.h>', '#include <stddef.h>', '#include "gem_b200.h"', 'int main(void) {',
-             '  printf("size %zu\\n", sizeof(gem_costmap_inflation));']
-    for fname, _ in cls._fields_:
-        lines.append(f'  printf("{fname} %zu\\n", offsetof(gem_costmap_inflation, {fname}));')
-    lines += ['  return 0;', '}']
-    src = tmp_path / "layout.c"
-    src.write_text("\n".join(lines))
-    exe = tmp_path / "layout"
-    subprocess.run(["gcc", "-std=c99", "-I", os.path.join(ROOT, "include"), "-o", str(exe), str(src)], check=True)
-    out = subprocess.run([str(exe)], capture_output=True, text=True, check=True).stdout.split()
-    got = dict(zip(out[0::2], (int(v) for v in out[1::2])))
-    assert got["size"] == C.sizeof(cls)
-    for fname, _ in cls._fields_:
-        assert got[fname] == getattr(cls, fname).offset, fname
+    native.assert_struct_layouts({"gem_costmap_inflation": L.GemCostmapInflation})
 
 
-def test_facade_program_with_inflation_compiles(tmp_path):
-    obj = tmp_path / "inflation_smoke.o"
-    subprocess.run(["g++", "-O2", "-std=c++14", "-Wall", "-Werror", "-I", os.path.join(ROOT, "include"), "-c", "-o", str(obj),
-                    os.path.join(ROOT, "tests", "cxx", "inflation_smoke.cpp")], check=True)
+def test_facade_program_with_inflation_compiles():
+    native.facade_compiles("inflation_smoke")

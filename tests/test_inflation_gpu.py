@@ -3,9 +3,7 @@ every crafted case and witness of tests/inflation_cases.py, seeded random grids 
 geometry with the c2 grid cloud marked, rolling global and local costmaps through a moving robot, back-to-back calls on one
 stream, the map left unchanged, every error path, scratch growth, and the C++ facade program."""
 import ctypes as C
-import os
 import subprocess
-import tempfile
 
 import numpy as np
 import pytest
@@ -15,6 +13,7 @@ import costmap_oracle
 import inflation_cases as ic
 import inflation_oracle as O
 import gem_b200
+import native
 from gem_b200 import _lib, costmap, synth
 
 pytestmark = pytest.mark.gpu
@@ -273,16 +272,7 @@ def test_tiled_handle():
 
 
 def test_facade_inflation_program_runs():
-    from gem_b200 import build
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    lib = build.build()
-    tmp = tempfile.mkdtemp(prefix="gem_inflation_")
-    exe = os.path.join(tmp, "inflation_smoke")
-    subprocess.run(["g++", "-O2", "-std=c++14", "-Wall", "-I", os.path.join(root, "include"), "-o", exe,
-                    os.path.join(root, "tests", "cxx", "inflation_smoke.cpp"), "-L", os.path.dirname(lib), "-lgem_b200",
-                    "-Wl,-rpath," + os.path.dirname(lib)], check=True)
+    exe = native.facade_program("inflation_smoke")
     r = subprocess.run([exe], capture_output=True, text=True, timeout=300)
-    os.remove(exe)
-    os.rmdir(tmp)
     print(r.stdout, r.stderr)
     assert r.returncode == 0 and "inflation ok" in r.stdout, r.stdout + r.stderr

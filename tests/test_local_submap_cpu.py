@@ -1,18 +1,14 @@
 """Local submaps, CPU side: the grid-cloud oracle (tests/orc_grid_cloud.c) against a numpy restatement of
 gridMaptoPointCloud (ElevationMapping.cpp:1204-1223) on show()'s masked layers, the local-map order definition, and the
 C++ facade's local-submap calls compiling and linking."""
-import os
 import subprocess
-import tempfile
 
 import numpy as np
 import pytest
 
+import native
 import submap_oracle
-from gem_b200 import build
 from oracle_lib import export_from_feature
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
 def np_grid_cloud(f, L, centre, start, res):
@@ -90,14 +86,7 @@ def test_local_map_order_definition():
 
 
 def test_local_submap_facade_compiles_and_links():
-    lib = build.build()
-    exe = os.path.join(tempfile.mkdtemp(prefix="gem_local_submap_"), "local_submap_smoke")
-    cmd = ["g++", "-O2", "-std=c++14", "-Wall", "-I", os.path.join(ROOT, "include"), "-o", exe,
-           os.path.join(ROOT, "tests", "cxx", "local_submap_smoke.cpp"), "-L", os.path.dirname(lib), "-lgem_b200",
-           "-Wl,-rpath," + os.path.dirname(lib)]
-    subprocess.run(cmd, check=True)
+    exe = native.facade_program("local_submap_smoke")
     out = subprocess.run(["nm", "-C", "--undefined-only", exe], capture_output=True, text=True).stdout
     for sym in ("gem_export_grid_cloud", "gem_harvest_to_local_map", "gem_local_map_take", "gem_local_map_clear"):
         assert sym in out, sym
-    os.remove(exe)
-    os.rmdir(os.path.dirname(exe))

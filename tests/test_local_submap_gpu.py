@@ -9,6 +9,7 @@ import pytest
 import torch
 
 import gem_b200
+import native
 import oracle_lib
 import submap_oracle
 from gem_b200 import synth
@@ -269,20 +270,9 @@ def test_f3_to_f4_end_to_end():
 
 
 def test_facade_local_submap_program_runs():
-    import os
     import subprocess
-    import tempfile
-    from gem_b200 import build
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    lib = build.build()
-    tmp = tempfile.mkdtemp(prefix="gem_local_submap_")
-    exe = os.path.join(tmp, "local_submap_smoke")
-    subprocess.run(["g++", "-O2", "-std=c++14", "-Wall", "-I", os.path.join(root, "include"), "-o", exe,
-                    os.path.join(root, "tests", "cxx", "local_submap_smoke.cpp"), "-L", os.path.dirname(lib), "-lgem_b200",
-                    "-Wl,-rpath," + os.path.dirname(lib)], check=True)
+    exe = native.facade_program("local_submap_smoke")
     r = subprocess.run([exe], capture_output=True, text=True, timeout=300)
-    os.remove(exe)
-    os.rmdir(tmp)
     print(r.stdout, r.stderr)
     assert r.returncode == 0 and "local_submap ok" in r.stdout, r.stdout + r.stderr
 

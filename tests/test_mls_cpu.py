@@ -5,8 +5,6 @@ solve), its M5 positions lie within 1e-6 m of the restatement's, its sample coun
 the disc, and the generator is reproducible and seeded.  Also: gem_mathd.h's exp against libm and its atan2 / sincos
 against the restatement of gem_math.cuh's, the ABI structs against the header, and that the facade program compiles."""
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 import pytest
@@ -14,9 +12,8 @@ from scipy.spatial import cKDTree
 
 import mls_cases as mc
 import mls_oracle
+import native
 from gem_b200 import _lib
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 f32 = np.float32
 
 
@@ -187,14 +184,10 @@ def test_abi_structs_match_header():
     assert C.sizeof(_lib.GemMlsParams) == 40 and C.sizeof(_lib.GemMlsInfo) == 24
     assert [f for f, _ in _lib.GemMlsParams._fields_] == [f for f, _ in mls_oracle.Params._fields_]
     assert [f for f, _ in _lib.GemMlsInfo._fields_] == [f for f, _ in mls_oracle.Info._fields_]
-    src = ("#include <stddef.h>\n#include \"gem_b200.h\"\n"
-           "_Static_assert(sizeof(gem_mls_params) == 40, \"p\");\n_Static_assert(sizeof(gem_mls_info) == 24, \"i\");\n"
-           "_Static_assert(offsetof(gem_mls_params, seed) == 32, \"s\");\n_Static_assert(offsetof(gem_mls_info, max_neighbours) == 20, \"m\");\n"
-           "_Static_assert(GEM_MLS_NONE == 0 && GEM_MLS_RANDOM_UNIFORM_DENSITY == 1, \"e\");\n")
-    subprocess.run(["gcc", "-std=c11", "-fsyntax-only", "-I", os.path.join(ROOT, "include"), "-x", "c", "-"], input=src, text=True,
-                   check=True)
+    assert _lib.GemMlsParams.seed.offset == 32 and _lib.GemMlsInfo.max_neighbours.offset == 20
+    native.assert_struct_layouts({"gem_mls_params": _lib.GemMlsParams, "gem_mls_info": _lib.GemMlsInfo},
+                                 {"GEM_MLS_NONE": 0, "GEM_MLS_RANDOM_UNIFORM_DENSITY": 1}, std="c11")
 
 
 def test_facade_program_compiles():
-    subprocess.run(["g++", "-std=c++14", "-Wall", "-Werror", "-fsyntax-only", "-I", os.path.join(ROOT, "include"),
-                    os.path.join(ROOT, "tests", "cxx", "mls_smoke.cpp")], check=True)
+    native.facade_compiles("mls_smoke", syntax_only=True)

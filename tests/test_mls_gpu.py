@@ -3,9 +3,7 @@ oracle, tests/orc_mls.c: output bytes and every info field on the crafted cases 
 harvested from the synthetic c2 stream at 0.05 m and at 0.2 m, a capacity below the count and the size query, every
 error path, two runs, cut_submap(dense=True) against take + oracle + grid cloud, and the C++ facade program."""
 import ctypes as C
-import os
 import subprocess
-import tempfile
 
 import numpy as np
 import pytest
@@ -14,6 +12,7 @@ import torch
 import gem_b200
 import mls_cases as mc
 import mls_oracle
+import native
 from gem_b200 import _lib, synth
 
 pytestmark = pytest.mark.gpu
@@ -216,16 +215,7 @@ def test_cut_submap_dense():
 
 
 def test_facade_mls_program_runs():
-    from gem_b200 import build
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    lib = build.build()
-    tmp = tempfile.mkdtemp(prefix="gem_mls_")
-    exe = os.path.join(tmp, "mls_smoke")
-    subprocess.run(["g++", "-O2", "-std=c++14", "-Wall", "-I", os.path.join(root, "include"), "-o", exe,
-                    os.path.join(root, "tests", "cxx", "mls_smoke.cpp"), "-L", os.path.dirname(lib), "-lgem_b200",
-                    "-Wl,-rpath," + os.path.dirname(lib)], check=True)
+    exe = native.facade_program("mls_smoke")
     r = subprocess.run([exe], capture_output=True, text=True, timeout=300)
-    os.remove(exe)
-    os.rmdir(tmp)
     print(r.stdout, r.stderr)
     assert r.returncode == 0 and "mls ok" in r.stdout, r.stdout + r.stderr

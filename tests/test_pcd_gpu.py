@@ -5,7 +5,6 @@ record cloud; the device formatter equals its host build on 2^26 random bit patt
 save_pcd's files (host and device records, chunked and one-shot) equal the oracle's; refusals write nothing; the C++
 facade's files equal Python's."""
 import ctypes as C
-import os
 import subprocess
 
 import numpy as np
@@ -13,6 +12,7 @@ import pytest
 import torch
 
 import gem_b200
+import native
 import pcd_cases as pc
 import pcd_oracle as po
 from gem_b200 import GemError, _lib, synth
@@ -152,13 +152,7 @@ def test_refusals_write_nothing(emap, tmp_path):
 
 
 def test_facade_pcd_program(emap, tmp_path):
-    from gem_b200 import build
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    lib = build.build()
-    exe = str(tmp_path / "pcd_smoke")
-    subprocess.run(["g++", "-O2", "-std=c++14", "-Wall", "-I", os.path.join(root, "include"), "-o", exe,
-                    os.path.join(root, "tests", "cxx", "pcd_smoke.cpp"), "-L", os.path.dirname(lib), "-lgem_b200",
-                    "-Wl,-rpath," + os.path.dirname(lib)], check=True)
+    exe = native.facade_program("pcd_smoke", tmp_path)
     rec = pc.harvest_like(1000, 6)
     rec[::37, :] = pc.records(pc.specials())[1]
     (tmp_path / "rec.bin").write_bytes(rec.tobytes())

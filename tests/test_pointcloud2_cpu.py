@@ -3,18 +3,15 @@ restatement of tests/pc2_cases.py, record bytes and mapping, on every crafted ca
 no GPU) against both; what the crafted cases are there to show; the ctypes mirrors of the new structs against the C
 compiler's layout of include/gem_b200.h."""
 import ctypes as C
-import os
 import subprocess
-import tempfile
 
 import numpy as np
 import pytest
 
+import native
 import pc2_cases as pc
 import pc2_oracle
 from gem_b200 import ElevationMap, GemError, PointCloud2Layout, _lib
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
 def layout(case):
@@ -131,21 +128,9 @@ STRUCTS = {
 
 
 def test_struct_layouts_match_the_header():
-    lines = ['#include <stdio.h>', '#include <stddef.h>', '#include "gem_b200.h"', "int main(void) {"]
-    for s, (_, fields) in STRUCTS.items():
-        lines.append(f'printf("{s} %zu\\n", sizeof({s}));')
-        for f in fields:
-            lines.append(f'printf("{s}.{f} %zu\\n", offsetof({s}, {f}));')
-    lines.append("return 0; }")
-    with tempfile.TemporaryDirectory() as tmp:
-        src, exe = os.path.join(tmp, "l.c"), os.path.join(tmp, "l")
-        open(src, "w").write("\n".join(lines))
-        subprocess.run(["gcc", "-I", os.path.join(ROOT, "include"), "-o", exe, src], check=True)
-        out = dict(line.rsplit(" ", 1) for line in subprocess.run([exe], capture_output=True, text=True, check=True).stdout.split("\n") if line)
     for s, (cls, fields) in STRUCTS.items():
-        assert int(out[s]) == C.sizeof(cls), s
-        for f in fields:
-            assert int(out[f"{s}.{f}"]) == getattr(cls, f).offset, (s, f)
+        assert set(fields) <= {f for f, _ in cls._fields_}, s
+    native.assert_struct_layouts({s: cls for s, (cls, _) in STRUCTS.items()}, std=None)
     # the oracle's mirrors too
     for cls, ref in ((pc2_oracle.Field, _lib.GemPointField), (pc2_oracle.Cloud, _lib.GemPointCloud2),
                      (pc2_oracle.Mapping, _lib.GemPc2Mapping)):
@@ -170,11 +155,8 @@ int main()
 
 
 def test_cxx_facade_layout_and_mapping(tmp_path):
-    from gem_b200 import build
-    lib = build.build()
-    src, exe = tmp_path / "f.cpp", tmp_path / "f"
+    src = tmp_path / "f.cpp"
     src.write_text(FACADE)
-    subprocess.run(["g++", "-std=c++14", "-Wall", "-Wextra", "-Werror", "-I", os.path.join(ROOT, "include"), str(src), "-L",
-                    os.path.dirname(lib), "-lgem_b200", f"-Wl,-rpath,{os.path.dirname(lib)}", "-o", str(exe)], check=True)
-    out = subprocess.run([str(exe)], capture_output=True, text=True, check=True).stdout.split("\n")
+    exe = native.facade_program("f", tmp_path, sources=[str(src)], flags=["-std=c++14", "-Wall", "-Wextra", "-Werror"])
+    out = subprocess.run([exe], capture_output=True, text=True, check=True).stdout.split("\n")
     assert out[0] == "2 0 0 12 12 24 4 0 23" and out[1] == "refused", out

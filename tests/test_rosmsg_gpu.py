@@ -4,7 +4,6 @@ the same state, into device and pinned host memory at every base offset 0-15, fo
 tests/rosmsg_cases.py; guard bytes around the output stay untouched by every call and refusal; size queries equal the
 written size; a c2-sized map with history_point over scrolled harvests; octrees; the SubMap; the C++ facade."""
 import ctypes as C
-import os
 import subprocess
 
 import numpy as np
@@ -12,6 +11,7 @@ import pytest
 import torch
 
 import gem_b200
+import native
 import rosmsg_cases as rc
 import rosmsg_oracle as ro
 from gem_b200 import GemError, RosHeader, _lib, synth
@@ -260,13 +260,7 @@ def test_refusals_write_nothing():
 
 
 def test_facade_rosmsg_program(tmp_path):
-    from gem_b200 import build
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    lib = build.build()
-    exe = str(tmp_path / "rosmsg_smoke")
-    subprocess.run(["g++", "-O2", "-std=c++14", "-Wall", "-I", os.path.join(root, "include"), "-o", exe,
-                    os.path.join(root, "tests", "cxx", "rosmsg_smoke.cpp"), "-L", os.path.dirname(lib), "-lgem_b200",
-                    "-Wl,-rpath," + os.path.dirname(lib)], check=True)
+    exe = native.facade_program("rosmsg_smoke", tmp_path)
     c = rc.case("L33_opt_move")
 
     class Recorder:   # the layers the case sets, for the program

@@ -4,15 +4,15 @@ DEFINITION, the twelve shipped sensor configs mapped to models, and the C++ help
 import json
 import math
 import os
-import subprocess
 import tempfile
 
 import numpy as np
 import pytest
 
+import native
 import oracle_lib
 import sensor_models_oracle as smo
-from gem_b200 import _lib, build
+from gem_b200 import _lib
 from gem_b200.elevation_map import (LaserSensorProcessor, PerfectSensorProcessor, StereoSensorProcessor,
                                     StructuredLightSensorProcessor, make_frame)
 
@@ -256,12 +256,7 @@ def test_stereo_defaults_are_the_nodes():
 
 
 def compile_sensor_models_smoke(outdir):
-    lib = build.build()
-    exe = os.path.join(outdir, "sensor_models_smoke")
-    subprocess.run(["g++", "-O2", "-std=c++14", "-Wall", "-Wextra", "-I", os.path.join(ROOT, "include"), "-o", exe,
-                    os.path.join(ROOT, "tests", "cxx", "sensor_models_smoke.cpp"), "-L", os.path.dirname(lib), "-lgem_b200",
-                    "-Wl,-rpath," + os.path.dirname(lib)], check=True)
-    return exe
+    return native.facade_program("sensor_models_smoke", outdir, ["-Wextra"])
 
 
 def test_cxx_helpers_compile():

@@ -3,17 +3,13 @@ tests/voxel_cases.py, bit for bit (output bytes and every info field), on every 
 on limits placed at float roundings; the ctypes mirrors of gem_voxel_grid_params / gem_voxel_grid_info against the C
 compiler; the C++ facade program compiles."""
 import ctypes as C
-import os
-import subprocess
-import tempfile
 
 import numpy as np
 import pytest
 
+import native
 import voxel_cases as vc
 import voxel_oracle
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
 def same(got, want, what):
@@ -112,41 +108,15 @@ def test_launch_chains_run():
     assert info["count"] == one.shape[0] > 0 and (np.abs(one[:, 0]) <= 10.0).all()
 
 
-def test_voxel_structs_match_the_header(tmp_path):
+def test_voxel_structs_match_the_header():
     import gem_b200._lib as L
-    structs = {"gem_voxel_grid_params": L.GemVoxelGridParams, "gem_voxel_grid_info": L.GemVoxelGridInfo}
-    lines = ['#include <stdio.h>', '#include <stddef.h>', '#include "gem_b200.h"', 'int main(void) {']
-    for cname, cls in structs.items():
-        lines.append(f'  printf("{cname} size %zu\\n", sizeof({cname}));')
-        for fname, _ in cls._fields_:
-            lines.append(f'  printf("{cname} {fname} %zu\\n", offsetof({cname}, {fname}));')
-    lines.append('  printf("consts %d %d %d %d %d\\n", GEM_VOXEL_FIELD_NONE, GEM_VOXEL_FIELD_X, GEM_VOXEL_FIELD_Y,'
-                 ' GEM_VOXEL_FIELD_Z, GEM_VOXEL_FIELD_INTENSITY);')
-    lines += ['  return 0;', '}']
-    src = tmp_path / "layout.c"
-    src.write_text("\n".join(lines))
-    exe = tmp_path / "layout"
-    subprocess.run(["gcc", "-std=c99", "-I", os.path.join(ROOT, "include"), "-o", str(exe), str(src)], check=True)
-    out = subprocess.run([str(exe)], capture_output=True, text=True, check=True).stdout
-    seen = 0
-    for ln in out.splitlines():
-        if ln.startswith("consts"):
-            assert [int(v) for v in ln.split()[1:]] == [L.VOXEL_FIELDS[k] for k in (None, "x", "y", "z", "intensity")]
-            continue
-        cname, field, val = ln.split()
-        cls = structs[cname]
-        expect = C.sizeof(cls) if field == "size" else getattr(cls, field).offset
-        assert int(val) == expect, (cname, field, int(val), expect)
-        seen += 1
-    assert seen == sum(len(c._fields_) + 1 for c in structs.values())
+    consts = {f"GEM_VOXEL_FIELD_{c}": L.VOXEL_FIELDS[k] for c, k in (("NONE", None), ("X", "x"), ("Y", "y"), ("Z", "z"),
+                                                                      ("INTENSITY", "intensity"))}
+    native.assert_struct_layouts({"gem_voxel_grid_params": L.GemVoxelGridParams, "gem_voxel_grid_info": L.GemVoxelGridInfo},
+                                 consts)
     # the oracle's mirror of the parameters has the library's layout too
     assert C.sizeof(voxel_oracle.Params) == C.sizeof(L.GemVoxelGridParams)
 
 
 def test_facade_program_with_voxel_grid_compiles():
-    tmp = tempfile.mkdtemp(prefix="gem_voxel_cxx_")
-    obj = os.path.join(tmp, "voxel_grid_smoke.o")
-    subprocess.run(["g++", "-O2", "-std=c++14", "-Wall", "-Werror", "-I", os.path.join(ROOT, "include"), "-c", "-o", obj,
-                    os.path.join(ROOT, "tests", "cxx", "voxel_grid_smoke.cpp")], check=True)
-    os.remove(obj)
-    os.rmdir(tmp)
+    native.facade_compiles("voxel_grid_smoke")

@@ -5,15 +5,14 @@ HDL-64 frames under filter.launch and the three-call filter_kitti.launch chain, 
 tiled handle, the C++ facade program, and raw frames filtered into gem_add_points_stream over a scrolling sequence
 against the oracle's filter and map."""
 import ctypes as C
-import os
 import subprocess
-import tempfile
 
 import numpy as np
 import pytest
 import torch
 
 import gem_b200
+import native
 import voxel_cases as vc
 import voxel_oracle
 from gem_b200 import _lib, synth
@@ -242,16 +241,7 @@ def test_filtered_stream_composition():
 
 
 def test_facade_voxel_grid_program_runs():
-    from gem_b200 import build
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    lib = build.build()
-    tmp = tempfile.mkdtemp(prefix="gem_voxel_")
-    exe = os.path.join(tmp, "voxel_grid_smoke")
-    subprocess.run(["g++", "-O2", "-std=c++14", "-Wall", "-I", os.path.join(root, "include"), "-o", exe,
-                    os.path.join(root, "tests", "cxx", "voxel_grid_smoke.cpp"), "-L", os.path.dirname(lib), "-lgem_b200",
-                    "-Wl,-rpath," + os.path.dirname(lib)], check=True)
+    exe = native.facade_program("voxel_grid_smoke")
     r = subprocess.run([exe], capture_output=True, text=True, timeout=300)
-    os.remove(exe)
-    os.rmdir(tmp)
     print(r.stdout, r.stderr)
     assert r.returncode == 0 and "voxel grid ok" in r.stdout, r.stdout + r.stderr

@@ -5,14 +5,12 @@ A call takes an (n, 4) float32 array {x, y, z, intensity} and returns (out, info
 float4 rows, info a dict {count, used, passthrough}; None where the library reports an error."""
 from __future__ import annotations
 
-import atexit
 import ctypes as C
 import os
-import shutil
-import subprocess
-import tempfile
 
 import numpy as np
+
+import native
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 SRC = os.path.join(HERE, "orc_voxel_grid.c")
@@ -33,12 +31,7 @@ class Info(C.Structure):
 def load():
     global _lib
     if _lib is None:
-        tmp = tempfile.mkdtemp(prefix="gem_orc_voxel_")
-        atexit.register(shutil.rmtree, tmp, True)
-        so = os.path.join(tmp, "liborc_voxel_grid.so")
-        subprocess.run(["gcc", "-O2", "-std=gnu11", "-fPIC", "-ffp-contract=off", "-fno-fast-math", "-Wall", "-Wextra",
-                        "-shared", "-o", so, SRC, "-lm"], check=True)
-        lib = C.CDLL(so)
+        lib = native.shared_library("orc_voxel_grid", [SRC], native.ORACLE_C, ["-lm"])
         lib.orc_voxel_grid.argtypes = [C.c_void_p, C.c_int, C.POINTER(Params), C.c_void_p, C.c_int, C.POINTER(Info)]
         lib.orc_voxel_grid.restype = C.c_int
         _lib = lib
