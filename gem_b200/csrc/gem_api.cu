@@ -20,6 +20,7 @@
 #include <map>
 #include <mutex>
 #include <string>
+#include <utility>
 #include <vector>
 
 #include "../../include/gem_b200.h"
@@ -58,6 +59,40 @@ struct PendingFold {
     const int *n_dev = nullptr;
 };
 
+// Owners of the handle's CUDA resources: each releases what it holds when it is reset, assigned over or destroyed, so
+// deleting the handle releases everything it holds.  Move-only.
+template <typename H, auto Release> struct Owned {
+    H p = nullptr;
+    Owned() = default;
+    Owned(Owned &&o) noexcept : p(std::exchange(o.p, nullptr)) {}
+    Owned &operator=(Owned &&o) noexcept { if (this != &o) { reset(); p = std::exchange(o.p, nullptr); } return *this; }
+    ~Owned() { reset(); }
+    void reset() { if (p) Release(p); p = nullptr; }
+};
+using Event = Owned<cudaEvent_t, cudaEventDestroy>;
+using Stream = Owned<cudaStream_t, cudaStreamDestroy>;
+template <typename T> using Pinned = Owned<T *, cudaFreeHost>;
+struct Graph { // a CUDA graph and its executable instance
+    Owned<cudaGraph_t, cudaGraphDestroy> graph;
+    Owned<cudaGraphExec_t, cudaGraphExecDestroy> exec;
+    void reset() { exec.reset(); graph.reset(); }
+};
+
+struct DevBuf { // a device buffer and its capacity in bytes; scratch buffers grow on demand (scratch_grow), never shrink
+    void *p = nullptr;
+    size_t cap = 0;
+    DevBuf() = default;
+    DevBuf(DevBuf &&o) noexcept : p(std::exchange(o.p, nullptr)), cap(std::exchange(o.cap, 0)) {}
+    DevBuf &operator=(DevBuf &&o) noexcept
+    {
+        if (this != &o) { reset(); p = std::exchange(o.p, nullptr); cap = std::exchange(o.cap, 0); }
+        return *this;
+    }
+    ~DevBuf() { reset(); }
+    void reset() { if (p) cudaFree(p); p = nullptr; cap = 0; }
+    template <typename T> T *as() const { return static_cast<T *>(p); }
+};
+
 struct TiledState { // gem_tiled_attach
     bool attached = false;
     int world = 0, my_rank = 0, tiles_r = 0, tiles_c = 0, cap = 0, nblk = 0;
@@ -66,16 +101,9 @@ struct TiledState { // gem_tiled_attach
     int step = 0;
     int depth = 2;                                 // 2: {route j -> bin j || fold j-1} per call; 3: {route j || bin j-1 || fold j-2}
     struct { bool active = false; int step = 0, buf = 0; } routed; // depth 3: delivered to the owners, not binned yet
-    cudaGraph_t graph = nullptr;
-    cudaGraphExec_t exec = nullptr;
+    Graph g;
     cudaGraphNode_t long_node = nullptr, fold_node = nullptr, route_node = nullptr, bin_node = nullptr;
     const void *route_func = nullptr; // the route kernel the graph was built with (k_route_peer or k_route_peer_any)
-};
-
-struct DevBuf { // a device buffer and its capacity in bytes; scratch buffers grow on demand (scratch_grow), never shrink
-    void *p = nullptr;
-    size_t cap = 0;
-    template <typename T> T *as() const { return static_cast<T *>(p); }
 };
 struct KeyRuns { // records bucketed by a 64-bit key (key_runs_grow, key_runs_enqueue): keys and record indices before /
                  // after the sort, the run lengths and their offsets, the temporary of the sort, the encoding and the scan
@@ -104,6 +132,10 @@ struct ColourScratch { // GEM_COLOUR_LOOKUP_NODE (gem_colour.cuh): the pixel key
     DevBuf ukey, up, ctl;
     int n = 0; // points every buffer is sized for
 };
+struct SplitScratch { // gem_grid_cloud_split: geographic z, row x, column y, per-cell distance, compacted distances, queue,
+                      // counters, stats
+    DevBuf zg, xg, yg, dcell, dist, queue, ctr, stats;
+};
 struct PcdScratch { // gem_pcd_format (gem_pcd.cuh): per-tile byte counts, their inclusive scan, the scan's temporary
     DevBuf bytes, ends, temp;
 };
@@ -116,7 +148,7 @@ struct OctScratch { // gem_color_octree (gem_octree.cuh); every buffer is consis
 };
 
 struct LocalStore { // localMap_ on the device (gem_harvest_to_local_map, gem_local_map_take / _clear; gem_submap.cuh)
-    void *buf = nullptr;               // one allocation: log, index keys, index positions, take scratch
+    DevBuf buf;                        // one allocation: log, index keys, index positions, take scratch
     float4 *log = nullptr;             // 2 x float4 per record, in harvest order
     unsigned long long *keys = nullptr; // open-addressing index, HASH_EMPTY = free slot
     int *latest = nullptr;             // per slot: the latest log position of its key
@@ -127,8 +159,8 @@ struct LocalStore { // localMap_ on the device (gem_harvest_to_local_map, gem_lo
 
 struct GlobalStore { // globalMap_, trajectory_ and localMapLoc_ on the device (gem_global_map_*; DESIGN.md f16)
     std::mutex mu;                     // the stack's own lock: no call on it takes the handle's mutex except a push, briefly
-    cudaStream_t stream = nullptr;     // the stack's own stream
-    cudaEvent_t ev = nullptr;          // push: the handle's stream -> the stack's stream
+    Stream stream;                     // the stack's own stream
+    Event ev;                          // push: the handle's stream -> the stack's stream
     DevBuf arena[2];                   // arena[cur]: the submaps back to back in push order; the other: the re-pack target
     int cur = 0;
     long long cap = 0;                 // records each arena buffer holds
@@ -141,8 +173,7 @@ struct GlobalStore { // globalMap_, trajectory_ and localMapLoc_ on the device (
 };
 
 struct FrameGraph { // {long lists || the other lists of the previous call || bin of this call} as one three-node CUDA graph
-    cudaGraph_t graph = nullptr;
-    cudaGraphExec_t exec = nullptr;
+    Graph g;
     cudaGraphNode_t long_node = nullptr, fold_node = nullptr, bin_node = nullptr;
 };
 
@@ -150,8 +181,8 @@ struct gem_map {
     std::recursive_mutex mu;
     gem_config cfg{};
     int dev = 0;
-    cudaStream_t stream = nullptr;
-    bool own_stream = false;
+    cudaStream_t stream = nullptr; // cfg->stream, or own_stream
+    Stream own_stream;             // the stream gem_create made when the caller gave none
     int L = 0;
     size_t nc = 0; // cells held by this handle
     int P = 0;     // per-launch point capacity
@@ -188,10 +219,7 @@ struct gem_map {
     bool prev_valid = false;
     LocalStore local;
     int *d_viscnt = nullptr;       // visual-cloud export: per (column, row chunk) counts / offsets
-    // gem_grid_cloud_split: geographic z, row x, column y, per-cell distance, compacted distances, queue, counters, stats
-    float *split_zg = nullptr, *split_xg = nullptr, *split_yg = nullptr, *split_dcell = nullptr, *split_dist = nullptr;
-    int *split_queue = nullptr, *split_ctr = nullptr;
-    SplitStats *split_stats = nullptr;
+    SplitScratch split;            // gem_grid_cloud_split
     OctScratch oct;                // gem_color_octree: scratch and the last stream
     DevBuf cost_scratch;           // costmap calls: the winner per costmap cell (int), or the copy of a rolled grid
     CostMarksDev *cost_acc = nullptr; // costmap mark calls: counts and encoded touch bounds
@@ -208,33 +236,34 @@ struct gem_map {
     GlobalStore gmap;              // gem_global_map_*
     unsigned long long *d_stamps = nullptr; // gem_debug_stamps
     int *d_raylist = nullptr;      // ray clean-up: cells that cast a ray + their count
-    uint32_t *d_bitmap = nullptr;  // ray clean-up: validity bitmap of the lowest layer (own tile / map-wide)
-    size_t bitmap_words = 0;
-    BinCounters *h_ctr = nullptr; // pinned
+    DevBuf ray_bitmap;             // ray clean-up: validity bitmap of the lowest layer (own tile / map-wide)
+    DevBuf divtest;                // gem_selftest_division: mismatch and fast-path counters
+    Pinned<BinCounters> h_ctr;
     // pipelined host ingest (gem_add_points_host_async): three staging sets (the fold of call i, issued with
     // call i+1, still reads call i's intensities)
-    cudaEvent_t ev_export = nullptr, ev_export_done = nullptr; // gem_export_layers_begin / _end
-    cudaStream_t copy_stream = nullptr;
+    Event ev_export, ev_export_done; // gem_export_layers_begin / _end
+    Stream copy_stream;
     void *d_axyzi[3] = {nullptr, nullptr, nullptr}, *d_argba[3] = {nullptr, nullptr, nullptr};
-    cudaEvent_t ev_h2d[3] = {nullptr, nullptr, nullptr}, ev_done[3] = {nullptr, nullptr, nullptr};
-    BinCounters *h_ctr_ring = nullptr; // pinned, 2 entries
+    Event ev_h2d[3], ev_done[3];
+    Pinned<BinCounters> h_ctr_ring; // 2 entries
     unsigned async_calls = 0;
     // gem_add_pointcloud2_host_async: per ring slot the message bytes and the camera image as they arrive (copy
     // stream), and one BGR8 conversion target (handle's stream); grown on demand
     DevBuf pc2_raw[3], pc2_img[3], pc2_bgr;
     // gem_add_points_multi: ring of per-call FrameParams tables (pinned host + device)
-    FrameParams *h_frames = nullptr, *d_frames = nullptr;
-    cudaEvent_t ev_frames[4] = {nullptr, nullptr, nullptr, nullptr};
+    Pinned<FrameParams> h_frames;
+    FrameParams *d_frames = nullptr;
+    Event ev_frames[4];
     unsigned multi_calls = 0;
     gem_stats stats{};
     std::string err;
-    std::vector<void *> allocs;
+    std::vector<DevBuf> allocs;
     // launch accounting / optional per-kernel CUDA-event timing (gem_profile_*)
     long long launches = 0;
     bool profiling = false;
-    struct Span { int cls; cudaEvent_t e0, e1; };
+    struct Span { int cls; Event e0, e1; };
     std::vector<Span> spans;
-    std::vector<cudaEvent_t> free_events;
+    std::vector<Event> free_events;
     double prof_ms[GEM_PROF_CLASSES] = {0};
     long long prof_count[GEM_PROF_CLASSES] = {0};
 };
@@ -266,15 +295,15 @@ int fail(gem_map *m, int code, const std::string &msg)
     return code;
 }
 
-cudaEvent_t prof_event(gem_map *m)
+Event prof_event(gem_map *m)
 {
+    Event e;
     if (!m->free_events.empty()) {
-        cudaEvent_t e = m->free_events.back();
+        e = std::move(m->free_events.back());
         m->free_events.pop_back();
-        return e;
+    } else {
+        cudaEventCreate(&e.p);
     }
-    cudaEvent_t e = nullptr;
-    cudaEventCreate(&e);
     return e;
 }
 // every kernel launch of the library goes through this macro: counts the launch and, when
@@ -284,10 +313,10 @@ cudaEvent_t prof_event(gem_map *m)
         (m)->launches++;                                         \
         if ((m)->profiling) {                                    \
             gem_map::Span sp__{(cls), prof_event(m), prof_event(m)}; \
-            cudaEventRecord(sp__.e0, (m)->stream);               \
+            cudaEventRecord(sp__.e0.p, (m)->stream);             \
             __VA_ARGS__;                                         \
-            cudaEventRecord(sp__.e1, (m)->stream);               \
-            (m)->spans.push_back(sp__);                          \
+            cudaEventRecord(sp__.e1.p, (m)->stream);             \
+            (m)->spans.push_back(std::move(sp__));               \
         } else {                                                 \
             __VA_ARGS__;                                         \
         }                                                        \
@@ -301,16 +330,29 @@ cudaEvent_t prof_event(gem_map *m)
         }                                                                                      \
     } while (0)
 
+// a buffer that lives as long as the handle (the handle keeps it in m->allocs)
 template <typename T> int dev_alloc(gem_map *m, T **p, size_t count)
 {
-    void *q = nullptr;
-    cudaError_t e = cudaMalloc(&q, count * sizeof(T) + 16);
+    DevBuf b;
+    cudaError_t e = cudaMalloc(&b.p, count * sizeof(T) + 16);
     if (e != cudaSuccess) {
         cudaGetLastError(); // a failed cudaMalloc stays recorded as the last error, which the next launch check would report
         return fail(m, GEM_ERR_NOMEM, std::string("cudaMalloc: ") + cudaGetErrorString(e));
     }
-    m->allocs.push_back(q);
-    *p = (T *)q;
+    *p = b.as<T>();
+    m->allocs.push_back(std::move(b));
+    return GEM_OK;
+}
+// pinned host memory, with dev_alloc's contract
+template <typename T> int host_alloc(gem_map *m, Pinned<T> &h, size_t count)
+{
+    void *q = nullptr;
+    cudaError_t e = cudaHostAlloc(&q, count * sizeof(T), cudaHostAllocDefault);
+    if (e != cudaSuccess) {
+        cudaGetLastError(); // as in dev_alloc
+        return fail(m, GEM_ERR_NOMEM, std::string("cudaHostAlloc: ") + cudaGetErrorString(e));
+    }
+    h.p = static_cast<T *>(q);
     return GEM_OK;
 }
 
@@ -322,18 +364,15 @@ int scratch_grow(gem_map *m, DevBuf &b, size_t bytes, const char *what, cudaStre
 {
     if (b.cap >= bytes) return GEM_OK;
     bytes = std::max(bytes + bytes / 4, (size_t)4096);
-    void *q = nullptr;
-    const cudaError_t e = cudaMalloc(&q, bytes);
+    DevBuf q;
+    const cudaError_t e = cudaMalloc(&q.p, bytes);
     if (e != cudaSuccess) {
         cudaGetLastError(); // as in dev_alloc
         return fail(m, GEM_ERR_NOMEM, std::string(what) + ": cudaMalloc: " + cudaGetErrorString(e));
     }
-    if (b.p) {
-        cudaStreamSynchronize(stream);
-        cudaFree(b.p);
-    }
-    b.p = q;
-    b.cap = bytes;
+    q.cap = bytes;
+    if (b.p) cudaStreamSynchronize(stream);
+    b = std::move(q);
     return GEM_OK;
 }
 
@@ -626,15 +665,15 @@ int read_counters(gem_map *m, long long n_in, bool accumulate)
 {
     int rc = drain(m);
     if (rc) return rc;
-    GEM_CUDA(m, cudaMemcpyAsync(m->h_ctr, m->ctr_last, sizeof(BinCounters), cudaMemcpyDeviceToHost, m->stream));
+    GEM_CUDA(m, cudaMemcpyAsync(m->h_ctr.p, m->ctr_last, sizeof(BinCounters), cudaMemcpyDeviceToHost, m->stream));
     GEM_CUDA(m, cudaStreamSynchronize(m->stream));
     if (!accumulate) memset(&m->stats, 0, sizeof m->stats);
     m->stats.points_in += n_in;
-    m->stats.points_binned += m->h_ctr->total;
-    m->stats.cells_touched += m->h_ctr->ntouched;
-    if (m->h_ctr->pool > m->bs[0].pool_cap) return fail(m, GEM_ERR_CUDA, "internal: record pool exhausted");
-    if (m->h_ctr->nlong >= m->bs[0].long_cap || m->h_ctr->nlarge >= m->bs[0].large_cap) return fail(m, GEM_ERR_CUDA, "internal: list queue overflow");
-    if (m->h_ctr->maxk > m->stats.max_points_per_cell) m->stats.max_points_per_cell = m->h_ctr->maxk;
+    m->stats.points_binned += m->h_ctr.p->total;
+    m->stats.cells_touched += m->h_ctr.p->ntouched;
+    if (m->h_ctr.p->pool > m->bs[0].pool_cap) return fail(m, GEM_ERR_CUDA, "internal: record pool exhausted");
+    if (m->h_ctr.p->nlong >= m->bs[0].long_cap || m->h_ctr.p->nlarge >= m->bs[0].large_cap) return fail(m, GEM_ERR_CUDA, "internal: list queue overflow");
+    if (m->h_ctr.p->maxk > m->stats.max_points_per_cell) m->stats.max_points_per_cell = m->h_ctr.p->maxk;
     return GEM_OK;
 }
 
@@ -663,7 +702,7 @@ int ensure_compat_staging(gem_map *m)
 }
 int ensure_out_staging(gem_map *m)
 {
-    if (m->ev_export_done) cudaStreamWaitEvent(m->stream, m->ev_export_done, 0); // an asynchronous export may still be reading the staging buffer
+    if (m->ev_export_done.p) cudaStreamWaitEvent(m->stream, m->ev_export_done.p, 0); // an asynchronous export may still be reading the staging buffer
     if (m->d_out) return GEM_OK;
     return dev_alloc(m, &m->d_out, m->nc * 9);
 }
@@ -672,12 +711,7 @@ int ensure_ray_scratch(gem_map *m, size_t bitmap_cells)
 {
     int rc;
     if (!m->d_raylist && (rc = dev_alloc(m, &m->d_raylist, m->nc + 1))) return rc; // every cell may cast a ray; [nc] = the count
-    const size_t words = bitmap_cells / 32 + 1;
-    if (!m->d_bitmap || m->bitmap_words < words) {
-        if ((rc = dev_alloc(m, &m->d_bitmap, words))) return rc;
-        m->bitmap_words = words;
-    }
-    return GEM_OK;
+    return scratch_grow(m, m->ray_bitmap, (bitmap_cells / 32 + 1) * sizeof(uint32_t), "raytracing", m->stream);
 }
 int ensure_route_scratch(gem_map *m)
 {
@@ -700,22 +734,24 @@ int ensure_route_scratch(gem_map *m)
 int launch_frame_graph(gem_map *m, BinKernel bk, void **bin_args, int bin_grid, void **fold_args, int fold_grid, void **long_args, int long_grid)
 {
     FrameGraph &fg = m->graphs[(const void *)bk];
+    Graph &g = fg.g;
     cudaKernelNodeParams kb{}, kf{}, kl{};
     kb.func = (void *)bk; kb.gridDim = dim3((unsigned)bin_grid); kb.blockDim = dim3(ADD_BLOCK); kb.sharedMemBytes = (unsigned)m->bin_smem; kb.kernelParams = bin_args;
     kf.func = (void *)k_fold; kf.gridDim = dim3((unsigned)fold_grid); kf.blockDim = dim3(ADD_BLOCK); kf.sharedMemBytes = (unsigned)m->fold_smem; kf.kernelParams = fold_args;
     kl.func = (void *)k_fold_long; kl.gridDim = dim3((unsigned)long_grid); kl.blockDim = dim3(LONG_BLOCK); kl.sharedMemBytes = (unsigned)m->long_smem; kl.kernelParams = long_args;
-    if (!fg.exec) {
-        GEM_CUDA(m, cudaGraphCreate(&fg.graph, 0));
-        GEM_CUDA(m, cudaGraphAddKernelNode(&fg.long_node, fg.graph, nullptr, 0, &kl)); // first: its blocks want empty SMs
-        GEM_CUDA(m, cudaGraphAddKernelNode(&fg.fold_node, fg.graph, nullptr, 0, &kf));
-        GEM_CUDA(m, cudaGraphAddKernelNode(&fg.bin_node, fg.graph, nullptr, 0, &kb));
-        GEM_CUDA(m, cudaGraphInstantiate(&fg.exec, fg.graph, 0));
+    if (!g.exec.p) {
+        g.reset(); // what a build that failed part way left
+        GEM_CUDA(m, cudaGraphCreate(&g.graph.p, 0));
+        GEM_CUDA(m, cudaGraphAddKernelNode(&fg.long_node, g.graph.p, nullptr, 0, &kl)); // first: its blocks want empty SMs
+        GEM_CUDA(m, cudaGraphAddKernelNode(&fg.fold_node, g.graph.p, nullptr, 0, &kf));
+        GEM_CUDA(m, cudaGraphAddKernelNode(&fg.bin_node, g.graph.p, nullptr, 0, &kb));
+        GEM_CUDA(m, cudaGraphInstantiate(&g.exec.p, g.graph.p, 0));
     } else {
-        GEM_CUDA(m, cudaGraphExecKernelNodeSetParams(fg.exec, fg.long_node, &kl));
-        GEM_CUDA(m, cudaGraphExecKernelNodeSetParams(fg.exec, fg.fold_node, &kf));
-        GEM_CUDA(m, cudaGraphExecKernelNodeSetParams(fg.exec, fg.bin_node, &kb));
+        GEM_CUDA(m, cudaGraphExecKernelNodeSetParams(g.exec.p, fg.long_node, &kl));
+        GEM_CUDA(m, cudaGraphExecKernelNodeSetParams(g.exec.p, fg.fold_node, &kf));
+        GEM_CUDA(m, cudaGraphExecKernelNodeSetParams(g.exec.p, fg.bin_node, &kb));
     }
-    GEM_CUDA(m, cudaGraphLaunch(fg.exec, m->stream));
+    GEM_CUDA(m, cudaGraphLaunch(g.exec.p, m->stream));
     m->launches += 3;
     return GEM_OK;
 }
@@ -931,9 +967,9 @@ int gem_create(const gem_config *cfg, gem_map **out)
     if (cfg->stream) {
         m->stream = (cudaStream_t)cfg->stream;
     } else {
-        e = cudaStreamCreateWithFlags(&m->stream, cudaStreamNonBlocking);
+        e = cudaStreamCreateWithFlags(&m->own_stream.p, cudaStreamNonBlocking);
         if (e != cudaSuccess) { m->err = cudaGetErrorString(e); return bail(GEM_ERR_CUDA); }
-        m->own_stream = true;
+        m->stream = m->own_stream.p;
     }
     const size_t nc = m->nc, P = (size_t)m->P;
     if ((rc = dev_alloc(m, &m->ml.cell, nc)) || (rc = dev_alloc(m, &m->ml.traver, nc)) || (rc = dev_alloc(m, &m->ml.lowest, nc)) ||
@@ -958,8 +994,7 @@ int gem_create(const gem_config *cfg, gem_map **out)
         if (e == cudaSuccess) e = cudaMemsetAsync(sc.pool, 0, ((size_t)sc.pool_cap + 1) * sizeof(uint4), m->stream);
         if (e != cudaSuccess) { m->err = cudaGetErrorString(e); return bail(GEM_ERR_CUDA); }
     }
-    e = cudaHostAlloc((void **)&m->h_ctr, sizeof(BinCounters), cudaHostAllocDefault);
-    if (e != cudaSuccess) { m->err = cudaGetErrorString(e); return bail(GEM_ERR_CUDA); }
+    if (host_alloc(m, m->h_ctr, 1)) return bail(GEM_ERR_CUDA);
     // G_Init_map gpu.cu:198-214.  A call that failed earlier on this thread (any handle; it was reported then) leaves its
     // error behind: clear it, so that the launch check below sees this handle's launches only
     cudaGetLastError();
@@ -985,46 +1020,13 @@ int gem_create(const gem_config *cfg, gem_map **out)
 int gem_destroy(gem_map *m)
 {
     if (!m) return GEM_OK;
+    SetDev sd(m->dev); // the owners release on the handle's device
     {
         Lock lk(m->mu);
-        SetDev sd(m->dev);
-        if (m->stream) cudaStreamSynchronize(m->stream);
-        for (auto &kv : m->graphs) {
-            if (kv.second.exec) cudaGraphExecDestroy(kv.second.exec);
-            if (kv.second.graph) cudaGraphDestroy(kv.second.graph);
-        }
-        if (m->tiled.exec) cudaGraphExecDestroy(m->tiled.exec);
-        if (m->tiled.graph) cudaGraphDestroy(m->tiled.graph);
-        for (auto &sp : m->spans) { cudaEventDestroy(sp.e0); cudaEventDestroy(sp.e1); }
-        for (cudaEvent_t e : m->free_events) cudaEventDestroy(e);
-        for (void *p : m->allocs) cudaFree(p);
-        if (m->local.buf) cudaFree(m->local.buf);
-        for (KeyRuns *k : {&m->oct.kr, &m->vox.kr, &m->mls.kr, &m->colour.kr})
-            for (DevBuf *b : {&k->key[0], &k->key[1], &k->idx[0], &k->idx[1], &k->cnt, &k->off, &k->temp})
-                if (b->p) cudaFree(b->p);
-        for (DevBuf *b : {&m->oct.leaf, &m->oct.level, &m->oct.ghead, &m->oct.gid, &m->oct.val, &m->oct.groups, &m->oct.ctr,
-                          &m->oct.key2[0], &m->oct.key2[1], &m->oct.nkey[0], &m->oct.nkey[1], &m->oct.nrec[0], &m->oct.nrec[1],
-                          &m->oct.dense, &m->cost_scratch, &m->vox.acc, &m->mls.spts, &m->mls.ukey, &m->mls.nbr, &m->mls.ocnt,
-                          &m->mls.ooff, &m->mls.longs, &m->mls.lkeys, &m->mls.acc, &m->pc2_raw[0],
-                          &m->pc2_raw[1], &m->pc2_raw[2], &m->pc2_img[0], &m->pc2_img[1], &m->pc2_img[2], &m->pc2_bgr,
-                          &m->pcd.bytes, &m->pcd.ends, &m->pcd.temp, &m->infl.key, &m->infl.pops, &m->infl.tab,
-                          &m->infl.gstart, &m->infl.blk, &m->ros_framing, &m->ros_stage, &m->cost_cells, &m->refuse, &m->gmap.arena[0],
-                          &m->gmap.arena[1], &m->gmap.meta, &m->gmap.pair, &m->colour.ukey, &m->colour.up, &m->colour.ctl})
-            if (b->p) cudaFree(b->p);
-        if (m->gmap.stream) { cudaStreamSynchronize(m->gmap.stream); cudaStreamDestroy(m->gmap.stream); }
-        if (m->gmap.ev) cudaEventDestroy(m->gmap.ev);
-        if (m->h_ctr) cudaFreeHost(m->h_ctr);
-        if (m->h_ctr_ring) cudaFreeHost(m->h_ctr_ring);
-        if (m->h_frames) cudaFreeHost(m->h_frames);
-        if (m->ev_export) cudaEventDestroy(m->ev_export);
-        if (m->ev_export_done) cudaEventDestroy(m->ev_export_done);
-        for (int i = 0; i < 4; i++) if (m->ev_frames[i]) cudaEventDestroy(m->ev_frames[i]);
-        for (int i = 0; i < 3; i++) {
-            if (m->ev_h2d[i]) cudaEventDestroy(m->ev_h2d[i]);
-            if (m->ev_done[i]) cudaEventDestroy(m->ev_done[i]);
-        }
-        if (m->copy_stream) { cudaStreamSynchronize(m->copy_stream); cudaStreamDestroy(m->copy_stream); }
-        if (m->own_stream && m->stream) cudaStreamDestroy(m->stream);
+        // every stream the handle issues work to is drained before any owner runs: nothing queued may still use what
+        // the owners release
+        for (cudaStream_t s : {m->stream, m->copy_stream.p, m->gmap.stream.p})
+            if (s) cudaStreamSynchronize(s);
     }
     delete m;
     return GEM_OK;
@@ -1242,14 +1244,14 @@ int gem_add_points_multi(gem_map *m, const void *xyzi, const void *rgba, int n_s
     Lock lk(m->mu);
     SetDev sd(m->dev);
     int rc = GEM_OK;
-    if (!m->h_frames) GEM_CUDA(m, cudaHostAlloc((void **)&m->h_frames, 4 * MAX_SEGMENTS * sizeof(FrameParams), cudaHostAllocDefault));
+    if (!m->h_frames.p && (rc = host_alloc(m, m->h_frames, (size_t)4 * MAX_SEGMENTS))) return rc;
     if (!m->d_frames && (rc = dev_alloc(m, &m->d_frames, (size_t)4 * MAX_SEGMENTS))) return rc;
     for (int i = 0; i < 4; i++)
-        if (!m->ev_frames[i]) GEM_CUDA(m, cudaEventCreateWithFlags(&m->ev_frames[i], cudaEventDisableTiming));
+        if (!m->ev_frames[i].p) GEM_CUDA(m, cudaEventCreateWithFlags(&m->ev_frames[i].p, cudaEventDisableTiming));
     if (n == 0) return flush_all_pending(m);
     const int slot = (int)(m->multi_calls++ & 3u);
-    if (m->multi_calls > 4) GEM_CUDA(m, cudaEventSynchronize(m->ev_frames[slot])); // pinned slot free again
-    FrameParams *hf = m->h_frames + (size_t)slot * MAX_SEGMENTS, *df = m->d_frames + (size_t)slot * MAX_SEGMENTS;
+    if (m->multi_calls > 4) GEM_CUDA(m, cudaEventSynchronize(m->ev_frames[slot].p)); // pinned slot free again
+    FrameParams *hf = m->h_frames.p + (size_t)slot * MAX_SEGMENTS, *df = m->d_frames + (size_t)slot * MAX_SEGMENTS;
     SegTable st{};
     st.n = n_segments;
     for (int s = 0; s <= n_segments; s++) st.off[s] = offsets[s];
@@ -1258,7 +1260,7 @@ int gem_add_points_multi(gem_map *m, const void *xyzi, const void *rgba, int n_s
         hf[s].idx0 = -offsets[s]; // every segment is a cloud of its own
     }
     GEM_CUDA(m, cudaMemcpyAsync(df, hf, (size_t)n_segments * sizeof(FrameParams), cudaMemcpyHostToDevice, m->stream));
-    GEM_CUDA(m, cudaEventRecord(m->ev_frames[slot], m->stream));
+    GEM_CUDA(m, cudaEventRecord(m->ev_frames[slot].p, m->stream));
     const BinSource in = xyzi_source(xyzi, rgba, 0);
     const FoldSrc fs{in.xyzi ? (const char *)in.xyzi + 12 : nullptr, 16};
     // pipelined like gem_add_points_stream: consecutive multi-sensor steps overlap bin(i+1) with fold(i)
@@ -1273,17 +1275,17 @@ int gem_add_points_multi(gem_map *m, const void *xyzi, const void *rgba, int n_s
 static int ensure_async_ring(gem_map *m)
 {
     int rc = GEM_OK;
-    if (!m->copy_stream) GEM_CUDA(m, cudaStreamCreateWithFlags(&m->copy_stream, cudaStreamNonBlocking));
+    if (!m->copy_stream.p) GEM_CUDA(m, cudaStreamCreateWithFlags(&m->copy_stream.p, cudaStreamNonBlocking));
     for (int i = 0; i < 3; i++) {
         if (!m->d_axyzi[i] && (rc = dev_alloc(m, (float4 **)&m->d_axyzi[i], (size_t)m->P))) return rc;
         if (!m->d_argba[i] && (rc = dev_alloc(m, (uchar4 **)&m->d_argba[i], (size_t)m->P))) return rc;
-        if (!m->ev_h2d[i]) GEM_CUDA(m, cudaEventCreateWithFlags(&m->ev_h2d[i], cudaEventDisableTiming));
-        if (!m->ev_done[i]) {
-            GEM_CUDA(m, cudaEventCreateWithFlags(&m->ev_done[i], cudaEventDisableTiming));
-            GEM_CUDA(m, cudaEventRecord(m->ev_done[i], m->stream));
+        if (!m->ev_h2d[i].p) GEM_CUDA(m, cudaEventCreateWithFlags(&m->ev_h2d[i].p, cudaEventDisableTiming));
+        if (!m->ev_done[i].p) {
+            GEM_CUDA(m, cudaEventCreateWithFlags(&m->ev_done[i].p, cudaEventDisableTiming));
+            GEM_CUDA(m, cudaEventRecord(m->ev_done[i].p, m->stream));
         }
     }
-    if (!m->h_ctr_ring) GEM_CUDA(m, cudaHostAlloc((void **)&m->h_ctr_ring, 2 * sizeof(BinCounters), cudaHostAllocDefault));
+    if (!m->h_ctr_ring.p) return host_alloc(m, m->h_ctr_ring, 2);
     return GEM_OK;
 }
 
@@ -1298,10 +1300,10 @@ static int async_add_slot(gem_map *m, unsigned i, int n, bool rgba, const gem_fr
     int rc = enqueue_add<SRC_XYZI>(m, in, fs, n, fp, nullptr, nullptr, true, true, true);
     if (rc) return rc;
     // the step's host-visible result: the counters of the newest call whose fold has been issued
-    GEM_CUDA(m, cudaMemcpyAsync(&m->h_ctr_ring[i & 1u], prev_ctr ? prev_ctr : m->ctr_last, sizeof(BinCounters), cudaMemcpyDeviceToHost, m->stream));
+    GEM_CUDA(m, cudaMemcpyAsync(&m->h_ctr_ring.p[i & 1u], prev_ctr ? prev_ctr : m->ctr_last, sizeof(BinCounters), cudaMemcpyDeviceToHost, m->stream));
     // staging set (i-1) % 3 was last read by the fold just issued (or by this call's own fold in the serial fallback)
-    GEM_CUDA(m, cudaEventRecord(m->ev_done[(i + 2u) % 3u], m->stream));
-    if (!m->pend.active) GEM_CUDA(m, cudaEventRecord(m->ev_done[b], m->stream));
+    GEM_CUDA(m, cudaEventRecord(m->ev_done[(i + 2u) % 3u].p, m->stream));
+    if (!m->pend.active) GEM_CUDA(m, cudaEventRecord(m->ev_done[b].p, m->stream));
     memset(&m->stats, 0, sizeof m->stats);
     m->stats.points_in = n; // the rest is fetched by gem_get_stats
     return GEM_OK;
@@ -1319,12 +1321,12 @@ int gem_add_points_host_async(gem_map *m, const void *xyzi, const void *rgba, in
     const unsigned i = m->async_calls++;
     const int b = (int)(i % 3u);
     // copy stream: wait until the fold that last read staging set b (call i-3) has been issued and is done, then H2D
-    GEM_CUDA(m, cudaStreamWaitEvent(m->copy_stream, m->ev_done[b], 0));
-    GEM_CUDA(m, cudaMemcpyAsync(m->d_axyzi[b], xyzi, (size_t)n * 16, cudaMemcpyHostToDevice, m->copy_stream));
-    if (rgba) GEM_CUDA(m, cudaMemcpyAsync(m->d_argba[b], rgba, (size_t)n * 4, cudaMemcpyHostToDevice, m->copy_stream));
-    GEM_CUDA(m, cudaEventRecord(m->ev_h2d[b], m->copy_stream));
+    GEM_CUDA(m, cudaStreamWaitEvent(m->copy_stream.p, m->ev_done[b].p, 0));
+    GEM_CUDA(m, cudaMemcpyAsync(m->d_axyzi[b], xyzi, (size_t)n * 16, cudaMemcpyHostToDevice, m->copy_stream.p));
+    if (rgba) GEM_CUDA(m, cudaMemcpyAsync(m->d_argba[b], rgba, (size_t)n * 4, cudaMemcpyHostToDevice, m->copy_stream.p));
+    GEM_CUDA(m, cudaEventRecord(m->ev_h2d[b].p, m->copy_stream.p));
     // compute stream: wait for the copy, issue {fold of the previous call || bin of this one}
-    GEM_CUDA(m, cudaStreamWaitEvent(m->stream, m->ev_h2d[b], 0));
+    GEM_CUDA(m, cudaStreamWaitEvent(m->stream, m->ev_h2d[b].p, 0));
     return async_add_slot(m, i, n, rgba != nullptr, frame);
 }
 
@@ -1518,8 +1520,8 @@ int gem_raytracing_tiled(gem_map *m, const float *global_lowest)
     MapLayers mlg = m->ml;
     mlg.lowest = const_cast<float *>(global_lowest); // rays probe the replicated, map-wide lowest layer
     GEM_LAUNCH(m, GEM_PROF_RAYTRACE, k_ray_collect<<<blocks_for(m->nc, 256, 1 << 30), 256, 0, m->stream>>>(m->geom, m->ml, m->cfg.obstacle_threshold, m->d_raylist, ray_count));
-    GEM_LAUNCH(m, GEM_PROF_RAYTRACE, k_lowest_bitmap<<<blocks_for(ng, 256, 1 << 30), 256, 0, m->stream>>>(global_lowest, (int)ng, m->d_bitmap));
-    GEM_LAUNCH(m, GEM_PROF_RAYTRACE, k_ray_trace<<<NUM_SMS * 8, 256, 0, m->stream>>>(m->geom, mlg, m->d_bitmap, m->sensorZ, m->d_raylist, ray_count));
+    GEM_LAUNCH(m, GEM_PROF_RAYTRACE, k_lowest_bitmap<<<blocks_for(ng, 256, 1 << 30), 256, 0, m->stream>>>(global_lowest, (int)ng, m->ray_bitmap.as<uint32_t>()));
+    GEM_LAUNCH(m, GEM_PROF_RAYTRACE, k_ray_trace<<<NUM_SMS * 8, 256, 0, m->stream>>>(m->geom, mlg, m->ray_bitmap.as<uint32_t>(), m->sensorZ, m->d_raylist, ray_count));
     GEM_LAUNCH(m, GEM_PROF_CLEAR, k_fill<<<blocks_for(m->nc, 256), 256, 0, m->stream>>>(m->ml.lowest, m->nc, 10.0f)); // own tile's lowest
     GEM_CUDA(m, cudaGetLastError());
     GEM_CUDA(m, cudaStreamSynchronize(m->stream));
@@ -1537,7 +1539,7 @@ int gem_raytracing(gem_map *m)
     int *ray_count = m->d_raylist + m->nc; // the list's length lives behind it
     GEM_CUDA(m, cudaMemsetAsync(ray_count, 0, sizeof(int), m->stream));
     GEM_LAUNCH(m, GEM_PROF_RAYTRACE, k_ray_collect<<<blocks_for(m->nc, 256, 1 << 30), 256, 0, m->stream>>>(m->geom, m->ml, m->cfg.obstacle_threshold, m->d_raylist, ray_count));
-    uint32_t *bitmap = m->d_bitmap;
+    uint32_t *bitmap = m->ray_bitmap.as<uint32_t>();
     GEM_LAUNCH(m, GEM_PROF_RAYTRACE, k_lowest_bitmap<<<blocks_for(m->nc, 256, 1 << 30), 256, 0, m->stream>>>(m->ml.lowest, (int)m->nc, bitmap));
     GEM_LAUNCH(m, GEM_PROF_RAYTRACE, k_ray_trace<<<NUM_SMS * 8, 256, 0, m->stream>>>(m->geom, m->ml, bitmap, m->sensorZ, m->d_raylist, ray_count));
     GEM_LAUNCH(m, GEM_PROF_CLEAR, k_fill<<<blocks_for(m->nc, 256), 256, 0, m->stream>>>(m->ml.lowest, m->nc, 10.0f)); // G_Clear_maplowest
@@ -1715,19 +1717,19 @@ int gem_export_layers_begin(gem_map *m, float *host_layers[9])
     int rc = ensure_out_staging(m);
     if (rc) return rc;
     if ((rc = flush_for_observer(m))) return rc;
-    if (!m->copy_stream) GEM_CUDA(m, cudaStreamCreateWithFlags(&m->copy_stream, cudaStreamNonBlocking));
-    if (!m->ev_export) GEM_CUDA(m, cudaEventCreateWithFlags(&m->ev_export, cudaEventDisableTiming));
-    if (!m->ev_export_done) GEM_CUDA(m, cudaEventCreateWithFlags(&m->ev_export_done, cudaEventDisableTiming));
+    if (!m->copy_stream.p) GEM_CUDA(m, cudaStreamCreateWithFlags(&m->copy_stream.p, cudaStreamNonBlocking));
+    if (!m->ev_export.p) GEM_CUDA(m, cudaEventCreateWithFlags(&m->ev_export.p, cudaEventDisableTiming));
+    if (!m->ev_export_done.p) GEM_CUDA(m, cudaEventCreateWithFlags(&m->ev_export_done.p, cudaEventDisableTiming));
     dim3 grid((m->L + 31) / 32, (m->L + 31) / 32);
-    GEM_CUDA(m, cudaStreamWaitEvent(m->stream, m->ev_export_done, 0)); // the previous export's copies have left the staging buffer
+    GEM_CUDA(m, cudaStreamWaitEvent(m->stream, m->ev_export_done.p, 0)); // the previous export's copies have left the staging buffer
     GEM_LAUNCH(m, GEM_PROF_OTHER, k_export_colmajor<<<grid, 256, 0, m->stream>>>(m->ml, m->L, m->d_out));
     GEM_CUDA(m, cudaGetLastError());
-    GEM_CUDA(m, cudaEventRecord(m->ev_export, m->stream));
-    GEM_CUDA(m, cudaStreamWaitEvent(m->copy_stream, m->ev_export, 0));
+    GEM_CUDA(m, cudaEventRecord(m->ev_export.p, m->stream));
+    GEM_CUDA(m, cudaStreamWaitEvent(m->copy_stream.p, m->ev_export.p, 0));
     for (int k = 0; k < 9; k++)
         if (host_layers[k])
-            GEM_CUDA(m, cudaMemcpyAsync(host_layers[k], m->d_out + (size_t)k * m->nc, m->nc * 4, cudaMemcpyDeviceToHost, m->copy_stream));
-    GEM_CUDA(m, cudaEventRecord(m->ev_export_done, m->copy_stream));
+            GEM_CUDA(m, cudaMemcpyAsync(host_layers[k], m->d_out + (size_t)k * m->nc, m->nc * 4, cudaMemcpyDeviceToHost, m->copy_stream.p));
+    GEM_CUDA(m, cudaEventRecord(m->ev_export_done.p, m->copy_stream.p));
     return GEM_OK;
 }
 int gem_export_layers_end(gem_map *m)
@@ -1735,7 +1737,7 @@ int gem_export_layers_end(gem_map *m)
     if (!m) return GEM_ERR_INVALID;
     Lock lk(m->mu);
     SetDev sd(m->dev);
-    if (m->ev_export_done) GEM_CUDA(m, cudaEventSynchronize(m->ev_export_done));
+    if (m->ev_export_done.p) GEM_CUDA(m, cudaEventSynchronize(m->ev_export_done.p));
     return GEM_OK;
 }
 
@@ -1874,27 +1876,26 @@ int gem_grid_cloud_split(gem_map *m, int source, int mean_k, double stddev_mul, 
     int rc = grid_source(m, source, "gem_grid_cloud_split", &g);
     if (rc) return rc;
     const int L = m->L;
-    if (!m->split_stats) { // the scratch is published only once every buffer exists (a failed call leaves it unset)
-        float *zg, *xg, *yg, *dcell, *dist;
-        int *queue, *ctr;
-        SplitStats *st;
-        if ((rc = dev_alloc(m, &zg, m->nc)) || (rc = dev_alloc(m, &xg, (size_t)L)) || (rc = dev_alloc(m, &yg, (size_t)L)) ||
-            (rc = dev_alloc(m, &dcell, m->nc)) || (rc = dev_alloc(m, &dist, m->nc)) || (rc = dev_alloc(m, &queue, m->nc)) ||
-            (rc = dev_alloc(m, &ctr, 2)) || (rc = dev_alloc(m, &st, 1)))
-            return rc;
-        m->split_zg = zg; m->split_xg = xg; m->split_yg = yg; m->split_dcell = dcell; m->split_dist = dist;
-        m->split_queue = queue; m->split_ctr = ctr; m->split_stats = st;
-    }
-    GEM_CUDA(m, cudaMemsetAsync(m->split_ctr, 0, 2 * sizeof(int), m->stream));
-    GEM_LAUNCH(m, GEM_PROF_OTHER, k_split_stage<<<blocks_for(m->nc, 256), 256, 0, m->stream>>>(g, m->split_zg, m->split_xg, m->split_yg, m->split_dcell));
+    SplitScratch &s = m->split;
+    const char *what = "gem_grid_cloud_split";
+    const size_t fn = m->nc * sizeof(float), fl = (size_t)L * sizeof(float);
+    if ((rc = scratch_grow(m, s.zg, fn, what, m->stream)) || (rc = scratch_grow(m, s.xg, fl, what, m->stream)) ||
+        (rc = scratch_grow(m, s.yg, fl, what, m->stream)) || (rc = scratch_grow(m, s.dcell, fn, what, m->stream)) ||
+        (rc = scratch_grow(m, s.dist, fn, what, m->stream)) || (rc = scratch_grow(m, s.queue, m->nc * sizeof(int), what, m->stream)) ||
+        (rc = scratch_grow(m, s.ctr, 2 * sizeof(int), what, m->stream)) || (rc = scratch_grow(m, s.stats, sizeof(SplitStats), what, m->stream)))
+        return rc;
+    float *zg = s.zg.as<float>(), *xg = s.xg.as<float>(), *yg = s.yg.as<float>(), *dcell = s.dcell.as<float>(), *dist = s.dist.as<float>();
+    int *queue = s.queue.as<int>(), *ctr = s.ctr.as<int>();
+    GEM_CUDA(m, cudaMemsetAsync(ctr, 0, 2 * sizeof(int), m->stream));
+    GEM_LAUNCH(m, GEM_PROF_OTHER, k_split_stage<<<blocks_for(m->nc, 256), 256, 0, m->stream>>>(g, zg, xg, yg, dcell));
     const int nt = (L + SPLIT_TILE - 1) / SPLIT_TILE;
     const dim3 grid(nt, nt);
     const int K = mean_k + 1;
     // the queue's length stays on the device: k_split_knn_far's fixed grid strides over it
 #define GEM_SPLIT_KNN(KC)                                                                                                              \
     do {                                                                                                                               \
-        GEM_LAUNCH(m, GEM_PROF_OTHER, k_split_knn<KC><<<grid, SPLIT_TILE * SPLIT_TILE, 0, m->stream>>>(m->split_zg, m->split_xg, m->split_yg, L, g.f.sx, g.f.sy, mean_k, m->split_dcell, m->split_queue, m->split_ctr)); \
-        GEM_LAUNCH(m, GEM_PROF_OTHER, k_split_knn_far<KC><<<NUM_SMS * 4, 128, 0, m->stream>>>(m->split_zg, m->split_xg, m->split_yg, L, g.f.sx, g.f.sy, mean_k, m->split_dcell, m->split_queue, m->split_ctr)); \
+        GEM_LAUNCH(m, GEM_PROF_OTHER, k_split_knn<KC><<<grid, SPLIT_TILE * SPLIT_TILE, 0, m->stream>>>(zg, xg, yg, L, g.f.sx, g.f.sy, mean_k, dcell, queue, ctr)); \
+        GEM_LAUNCH(m, GEM_PROF_OTHER, k_split_knn_far<KC><<<NUM_SMS * 4, 128, 0, m->stream>>>(zg, xg, yg, L, g.f.sx, g.f.sy, mean_k, dcell, queue, ctr)); \
     } while (0)
     if (K <= 8) GEM_SPLIT_KNN(8);
     else if (K <= 24) GEM_SPLIT_KNN(24);
@@ -1903,19 +1904,19 @@ int gem_grid_cloud_split(gem_map *m, int source, int mean_k, double stddev_mul, 
     GEM_CUDA(m, cudaGetLastError());
     // distances in cloud order -> statistics -> road -> obstacle, all on the stream; the three counts are copied beside
     // the statistics on the device, and the call waits once, for the one small read-back
-    SplitStats *dst = m->split_stats;
+    SplitStats *dst = s.stats.as<SplitStats>();
     int *d_total = nullptr;
-    SplitDistSrc ds{g, m->split_dcell, m->split_dist, mean_distance_device, distance_capacity};
+    SplitDistSrc ds{g, dcell, dist, mean_distance_device, distance_capacity};
     if ((rc = compact_cells_issue(m, ds, (int)m->nc, &d_total))) return rc;
     GEM_CUDA(m, cudaMemcpyAsync(&dst->points, d_total, sizeof(int), cudaMemcpyDeviceToDevice, m->stream));
-    GEM_LAUNCH(m, GEM_PROF_OTHER, k_split_stats<<<1, 32, 0, m->stream>>>(m->split_dist, &dst->points, m->split_ctr, mean_k, stddev_mul, dst,
+    GEM_LAUNCH(m, GEM_PROF_OTHER, k_split_stats<<<1, 32, 0, m->stream>>>(dist, &dst->points, ctr, mean_k, stddev_mul, dst,
                                                                          mean_distance_device, distance_capacity));
     GEM_CUDA(m, cudaGetLastError());
-    SplitSrc rs{g, m->split_dcell, dst, travers_threshold, 1};
+    SplitSrc rs{g, dcell, dst, travers_threshold, 1};
     rs.g.out = reinterpret_cast<float4 *>(road_points32_device);
     if ((rc = compact_cells_issue(m, rs, (int)std::min<size_t>((size_t)road_capacity, m->nc), &d_total))) return rc;
     GEM_CUDA(m, cudaMemcpyAsync(&dst->road, d_total, sizeof(int), cudaMemcpyDeviceToDevice, m->stream));
-    SplitSrc os{g, m->split_dcell, dst, travers_threshold, 0};
+    SplitSrc os{g, dcell, dst, travers_threshold, 0};
     os.g.out = reinterpret_cast<float4 *>(obstacle_points32_device);
     if ((rc = compact_cells_issue(m, os, (int)std::min<size_t>((size_t)obstacle_capacity, m->nc), &d_total))) return rc;
     GEM_CUDA(m, cudaMemcpyAsync(&dst->obstacle, d_total, sizeof(int), cudaMemcpyDeviceToDevice, m->stream));
@@ -2570,15 +2571,14 @@ static int local_reserve(gem_map *m, long long need)
     while (slots < 2 * (size_t)cap) slots <<= 1;
     const size_t nchunk = (size_t)cap / 32 + 1, nseg = nchunk / SCAN_SEG + 1;
     const size_t bytes = (size_t)cap * 32 + slots * (8 + 4) + (nchunk + nseg) * 4;
-    void *buf = nullptr;
-    cudaError_t e = cudaMalloc(&buf, bytes);
+    LocalStore t;
+    cudaError_t e = cudaMalloc(&t.buf.p, bytes);
     if (e != cudaSuccess) {
         cudaGetLastError();
         return fail(m, GEM_ERR_NOMEM, std::string("local map: cudaMalloc: ") + cudaGetErrorString(e));
     }
-    LocalStore t;
-    t.buf = buf;
-    t.log = (float4 *)buf;
+    t.buf.cap = bytes;
+    t.log = t.buf.as<float4>();
     t.keys = (unsigned long long *)(t.log + 2 * (size_t)cap);
     t.latest = (int *)(t.keys + slots);
     t.cnt = t.latest + slots;
@@ -2591,12 +2591,8 @@ static int local_reserve(gem_map *m, long long need)
         e = cudaGetLastError();
     }
     if (e == cudaSuccess) e = cudaStreamSynchronize(m->stream);
-    if (e != cudaSuccess) {
-        cudaFree(buf);
-        return fail(m, GEM_ERR_CUDA, std::string("local map: growth: ") + cudaGetErrorString(e));
-    }
-    if (s.buf) cudaFree(s.buf);
-    s = t;
+    if (e != cudaSuccess) return fail(m, GEM_ERR_CUDA, std::string("local map: growth: ") + cudaGetErrorString(e));
+    s = std::move(t);
     return GEM_OK;
 }
 
@@ -2605,7 +2601,7 @@ static int local_reset(gem_map *m)
 {
     LocalStore &s = m->local;
     s.n = 0;
-    if (!s.buf) return GEM_OK;
+    if (!s.buf.p) return GEM_OK;
     GEM_CUDA(m, cudaMemsetAsync(s.keys, 0xff, s.slots * 8, m->stream));
     GEM_CUDA(m, cudaMemsetAsync(s.latest, 0xff, s.slots * 4, m->stream));
     GEM_CUDA(m, cudaStreamSynchronize(m->stream));
@@ -2757,12 +2753,12 @@ int gem_profile_read(gem_map *m, gem_profile *out, int reset)
     GEM_CUDA(m, cudaStreamSynchronize(m->stream));
     for (auto &sp : m->spans) {
         float ms = 0.0f;
-        if (cudaEventElapsedTime(&ms, sp.e0, sp.e1) == cudaSuccess) {
+        if (cudaEventElapsedTime(&ms, sp.e0.p, sp.e1.p) == cudaSuccess) {
             m->prof_ms[sp.cls] += ms;
             m->prof_count[sp.cls]++;
         }
-        m->free_events.push_back(sp.e0);
-        m->free_events.push_back(sp.e1);
+        m->free_events.push_back(std::move(sp.e0));
+        m->free_events.push_back(std::move(sp.e1));
     }
     m->spans.clear();
     out->launches = m->launches;
@@ -2783,14 +2779,14 @@ int gem_selftest_division(gem_map *m, unsigned long long seed, unsigned long lon
     if (!m || !mismatches_out) return GEM_ERR_INVALID;
     Lock lk(m->mu);
     SetDev sd(m->dev);
-    unsigned long long *d = nullptr;
-    GEM_CUDA(m, cudaMalloc((void **)&d, 16));
+    const int rc = scratch_grow(m, m->divtest, 16, "gem_selftest_division", m->stream);
+    if (rc) return rc;
+    unsigned long long *d = m->divtest.as<unsigned long long>();
     GEM_CUDA(m, cudaMemsetAsync(d, 0, 16, m->stream));
     GEM_LAUNCH(m, GEM_PROF_OTHER, k_div_selftest<<<NUM_SMS * 8, 256, 0, m->stream>>>(seed, (size_t)n, d, d + 1));
     unsigned long long h[2] = {0, 0};
     GEM_CUDA(m, cudaMemcpyAsync(h, d, 16, cudaMemcpyDeviceToHost, m->stream));
     GEM_CUDA(m, cudaStreamSynchronize(m->stream));
-    cudaFree(d);
     *mismatches_out = h[0];
     if (fast_out) *fast_out = h[1];
     return GEM_OK;
@@ -2799,7 +2795,9 @@ int gem_selftest_division(gem_map *m, unsigned long long seed, unsigned long lon
 int gem_host_alloc(void **out, unsigned long long bytes)
 {
     if (!out) return GEM_ERR_INVALID;
-    return cudaHostAlloc(out, (size_t)bytes, cudaHostAllocDefault) == cudaSuccess ? GEM_OK : GEM_ERR_NOMEM;
+    if (cudaHostAlloc(out, (size_t)bytes, cudaHostAllocDefault) == cudaSuccess) return GEM_OK;
+    cudaGetLastError(); // as in dev_alloc
+    return GEM_ERR_NOMEM;
 }
 int gem_host_free(void *p) { return cudaFreeHost(p) == cudaSuccess ? GEM_OK : GEM_ERR_CUDA; }
 
@@ -2970,8 +2968,8 @@ using GLock = std::lock_guard<std::mutex>;
 static int gmap_ready(gem_map *m)
 {
     GlobalStore &g = m->gmap;
-    if (!g.stream) GEM_CUDA(m, cudaStreamCreateWithFlags(&g.stream, cudaStreamNonBlocking));
-    if (!g.ev) GEM_CUDA(m, cudaEventCreateWithFlags(&g.ev, cudaEventDisableTiming));
+    if (!g.stream.p) GEM_CUDA(m, cudaStreamCreateWithFlags(&g.stream.p, cudaStreamNonBlocking));
+    if (!g.ev.p) GEM_CUDA(m, cudaEventCreateWithFlags(&g.ev.p, cudaEventDisableTiming));
     return GEM_OK;
 }
 // room for `need` records in both arena buffers (capacity doubles from 1024).  Both are allocated before anything is
@@ -2983,29 +2981,21 @@ static int gmap_reserve_records(gem_map *m, long long need)
     long long cap = g.cap > 0 ? g.cap : 1024;
     while (cap < need) cap *= 2;
     if (cap > (1 << 30)) return fail(m, GEM_ERR_NOMEM, "global map: more than 2^30 records");
-    void *q[2] = {nullptr, nullptr};
+    DevBuf q[2];
     for (int b = 0; b < 2; b++) {
-        const cudaError_t e = cudaMalloc(&q[b], (size_t)cap * sizeof(SubPoint));
+        const cudaError_t e = cudaMalloc(&q[b].p, (size_t)cap * sizeof(SubPoint));
         if (e != cudaSuccess) {
             cudaGetLastError();
-            if (q[0]) cudaFree(q[0]);
             return fail(m, GEM_ERR_NOMEM, std::string("global map: cudaMalloc: ") + cudaGetErrorString(e));
         }
+        q[b].cap = (size_t)cap * sizeof(SubPoint);
     }
     const int total = g.off.back();
-    cudaError_t e = total ? cudaMemcpyAsync(q[0], g.arena[g.cur].p, (size_t)total * sizeof(SubPoint), cudaMemcpyDeviceToDevice, g.stream)
+    cudaError_t e = total ? cudaMemcpyAsync(q[0].p, g.arena[g.cur].p, (size_t)total * sizeof(SubPoint), cudaMemcpyDeviceToDevice, g.stream.p)
                           : cudaSuccess;
-    if (e == cudaSuccess) e = cudaStreamSynchronize(g.stream);
-    if (e != cudaSuccess) {
-        cudaFree(q[0]);
-        cudaFree(q[1]);
-        return fail(m, GEM_ERR_CUDA, std::string("global map: growth: ") + cudaGetErrorString(e));
-    }
-    for (int b = 0; b < 2; b++) {
-        if (g.arena[b].p) cudaFree(g.arena[b].p);
-        g.arena[b].p = q[b];
-        g.arena[b].cap = (size_t)cap * sizeof(SubPoint);
-    }
+    if (e == cudaSuccess) e = cudaStreamSynchronize(g.stream.p);
+    if (e != cudaSuccess) return fail(m, GEM_ERR_CUDA, std::string("global map: growth: ") + cudaGetErrorString(e));
+    for (int b = 0; b < 2; b++) g.arena[b] = std::move(q[b]);
     g.cur = 0;
     g.cap = cap;
     return GEM_OK;
@@ -3019,7 +3009,7 @@ static int gmap_reserve_meta(gem_map *m, int K)
     if (K <= g.meta_submaps) return GEM_OK;
     int cap = std::max(g.meta_submaps * 2, 64);
     while (cap < K) cap *= 2;
-    const int rc = scratch_grow(m, g.meta, gmap_meta_ints(cap) * 4 + (size_t)cap * sizeof(Rigid), "global map", g.stream);
+    const int rc = scratch_grow(m, g.meta, gmap_meta_ints(cap) * 4 + (size_t)cap * sizeof(Rigid), "global map", g.stream.p);
     if (rc == GEM_OK) g.meta_submaps = cap;
     return rc;
 }
@@ -3047,7 +3037,7 @@ int gem_global_map_reserve(gem_map *m, long long records, int submaps)
     if ((rc = gmap_ready(m)) || (rc = gmap_reserve_records(m, records)) || (rc = gmap_reserve_meta(m, submaps))) return rc;
     // one pair of the largest submaps the arena can hold
     const int big = (int)std::min<long long>(records, g.cap);
-    return scratch_grow(m, g.pair, pair_bytes(big, big), "gem_global_map_reserve", g.stream);
+    return scratch_grow(m, g.pair, pair_bytes(big, big), "gem_global_map_reserve", g.stream.p);
 }
 
 int gem_global_map_push(gem_map *m, const void *records_device, int n, const float pose[16])
@@ -3068,12 +3058,12 @@ int gem_global_map_push(gem_map *m, const void *records_device, int n, const flo
     if ((rc = gmap_ready(m)) || (rc = gmap_reserve_records(m, total + n))) return rc;
     { // a cut_submap issued just before on the handle's stream is complete before the copy reads it
         Lock hl(m->mu);
-        GEM_CUDA(m, cudaEventRecord(g.ev, m->stream));
+        GEM_CUDA(m, cudaEventRecord(g.ev.p, m->stream));
     }
-    GEM_CUDA(m, cudaStreamWaitEvent(g.stream, g.ev, 0));
+    GEM_CUDA(m, cudaStreamWaitEvent(g.stream.p, g.ev.p, 0));
     if (n) GEM_CUDA(m, cudaMemcpyAsync(g.arena[g.cur].as<SubPoint>() + total, records_device, (size_t)n * sizeof(SubPoint),
-                                       cudaMemcpyDeviceToDevice, g.stream));
-    GEM_CUDA(m, cudaStreamSynchronize(g.stream));
+                                       cudaMemcpyDeviceToDevice, g.stream.p));
+    GEM_CUDA(m, cudaStreamSynchronize(g.stream.p));
     // :636-642, then :660: the keyframe (pose, centre = its translation x, y) first, then its submap
     g.poses.insert(g.poses.end(), pose, pose + 16);
     g.centres.push_back(pose[3]);
@@ -3105,35 +3095,35 @@ int gem_global_map_update(gem_map *m, const float *opt_poses, int k, double reso
     gem_gmap::pair_schedule(g.centres.data(), Kp, radius, pairs);
     int big = 0;
     for (int i = 0; i < Kp; i++) big = std::max(big, g.cnt[i]);
-    if ((rc = gmap_reserve_meta(m, std::max(K, 1))) || (rc = scratch_grow(m, g.pair, pair_bytes(big, big), "gem_global_map_update", g.stream))) return rc;
+    if ((rc = gmap_reserve_meta(m, std::max(K, 1))) || (rc = scratch_grow(m, g.pair, pair_bytes(big, big), "gem_global_map_update", g.stream.p))) return rc;
     int *d_cnt = g.meta.as<int>(), *d_off = d_cnt + K, *d_off_new = d_off + K + 1, *d_ctr = d_off_new + K + 1;
     Rigid *d_T = (Rigid *)(g.meta.as<int>() + gmap_meta_ints(g.meta_submaps));
     std::vector<int> h((size_t)3 * K + 6, 0);
     std::copy(g.cnt.begin(), g.cnt.end(), h.begin());
     std::copy(g.off.begin(), g.off.end(), h.begin() + K);
-    GEM_CUDA(m, cudaMemcpyAsync(d_cnt, h.data(), h.size() * 4, cudaMemcpyHostToDevice, g.stream));
+    GEM_CUDA(m, cudaMemcpyAsync(d_cnt, h.data(), h.size() * 4, cudaMemcpyHostToDevice, g.stream.p));
     SubPoint *arena = g.arena[g.cur].as<SubPoint>();
     if (Kp > 1) {
-        GEM_CUDA(m, cudaMemcpyAsync(d_T, T.data(), (size_t)Kp * sizeof(Rigid), cudaMemcpyHostToDevice, g.stream));
+        GEM_CUDA(m, cudaMemcpyAsync(d_T, T.data(), (size_t)Kp * sizeof(Rigid), cudaMemcpyHostToDevice, g.stream.p));
         const int n = g.off[Kp] - g.off[1];
-        if (n > 0) k_transform_segments<<<blocks_for((size_t)n, 256, 1 << 30), 256, 0, g.stream>>>(arena, d_off + 1, d_T + 1, Kp - 1);
+        if (n > 0) k_transform_segments<<<blocks_for((size_t)n, 256, 1 << 30), 256, 0, g.stream.p>>>(arena, d_off + 1, d_T + 1, Kp - 1);
         GEM_CUDA(m, cudaGetLastError());
     }
     int launches = 0;
     for (const auto &pr : pairs) { // each pair's scratch laid out for its own two upper bounds (within pair_bytes(big, big))
         const int j = pr.first, i = pr.second;
-        const cudaError_t e = enqueue_pair(g.stream, pair_layout(g.pair.p, g.cnt[j], g.cnt[i]), arena + g.off[j], g.cnt[j], d_cnt + j, arena + g.off[i], g.cnt[i], d_cnt + i,
+        const cudaError_t e = enqueue_pair(g.stream.p, pair_layout(g.pair.p, g.cnt[j], g.cnt[i]), arena + g.off[j], g.cnt[j], d_cnt + j, arena + g.off[i], g.cnt[i], d_cnt + i,
                                            resolution, compat, d_ctr, launches);
         if (e != cudaSuccess) return fail(m, GEM_ERR_CUDA, std::string("gem_global_map_update: ") + cudaGetErrorString(e));
     }
     if (!pairs.empty()) { // the stack back to back again, into the other arena buffer
-        k_pack_offsets<<<1, 1, 0, g.stream>>>(d_cnt, K, d_off_new);
-        k_pack_segments<<<blocks_for((size_t)g.off[K], 256, 1 << 30), 256, 0, g.stream>>>(arena, g.arena[g.cur ^ 1].as<SubPoint>(), d_off,
+        k_pack_offsets<<<1, 1, 0, g.stream.p>>>(d_cnt, K, d_off_new);
+        k_pack_segments<<<blocks_for((size_t)g.off[K], 256, 1 << 30), 256, 0, g.stream.p>>>(arena, g.arena[g.cur ^ 1].as<SubPoint>(), d_off,
                                                                                           d_off_new, d_cnt, K);
         GEM_CUDA(m, cudaGetLastError());
     }
-    GEM_CUDA(m, cudaMemcpyAsync(h.data(), d_cnt, h.size() * 4, cudaMemcpyDeviceToHost, g.stream));
-    GEM_CUDA(m, cudaStreamSynchronize(g.stream));
+    GEM_CUDA(m, cudaMemcpyAsync(h.data(), d_cnt, h.size() * 4, cudaMemcpyDeviceToHost, g.stream.p));
+    GEM_CUDA(m, cudaStreamSynchronize(g.stream.p));
     if (!pairs.empty()) g.cur ^= 1;
     for (int i = 0; i < K; i++) {
         g.cnt[i] = h[i];
@@ -3193,7 +3183,7 @@ void *gem_global_map_stream(gem_map *m)
     GlobalStore &g = m->gmap;
     GLock lk(g.mu);
     SetDev sd(m->dev);
-    return gmap_ready(m) == GEM_OK ? (void *)g.stream : nullptr;
+    return gmap_ready(m) == GEM_OK ? (void *)g.stream.p : nullptr;
 }
 
 // ---- tiled maps, peer path (gem_route.cuh "Peer path, round 2") --------------------------------------------------------
@@ -3224,7 +3214,7 @@ int gem_tiled_attach(gem_map *m, const gem_tiled_peers *p)
     ts.step = 0;
     ts.routed.active = false;
     if (const char *e = getenv("GEM_B200_TILED_DEPTH")) ts.depth = (atoi(e) == 3) ? 3 : 2;
-    if (ts.exec) { cudaGraphExecDestroy(ts.exec); cudaGraphDestroy(ts.graph); ts.exec = nullptr; ts.graph = nullptr; }
+    ts.g.reset();
     ts.attached = true;
     return GEM_OK;
 }
@@ -3307,25 +3297,24 @@ int gem_tiled_step(gem_map *m, const void *xyzi, const void *rgba, int n, const 
     kf.func = (void *)k_fold; kf.gridDim = dim3((unsigned)fb); kf.blockDim = dim3(ADD_BLOCK); kf.sharedMemBytes = (unsigned)m->fold_smem; kf.kernelParams = fold_args;
     kr.func = (void *)route_kernel; kr.gridDim = dim3((unsigned)nblk); kr.blockDim = dim3(ROUTE_BLOCK); kr.sharedMemBytes = 0; kr.kernelParams = route_args;
     kb.func = (void *)k_bin_peer; kb.gridDim = dim3((unsigned)bin_peer_blocks(b.nsub)); kb.blockDim = dim3(ROUTE_BLOCK); kb.sharedMemBytes = 0; kb.kernelParams = bin_args;
-    if (ts.exec && ts.route_func != kr.func) { // a sensor model of the other kind: a node's kernel cannot be swapped
-        cudaGraphExecDestroy(ts.exec); cudaGraphDestroy(ts.graph); ts.exec = nullptr; ts.graph = nullptr;
-    }
-    if (!ts.exec) {
+    Graph &tg = ts.g;
+    if (!tg.exec.p || ts.route_func != kr.func) { // (re)build: a node's kernel cannot be swapped for the other sensor kind's
+        tg.reset();
         ts.route_func = kr.func;
-        GEM_CUDA(m, cudaGraphCreate(&ts.graph, 0));
-        GEM_CUDA(m, cudaGraphAddKernelNode(&ts.long_node, ts.graph, nullptr, 0, &kl));
-        GEM_CUDA(m, cudaGraphAddKernelNode(&ts.route_node, ts.graph, nullptr, 0, &kr));
-        GEM_CUDA(m, cudaGraphAddKernelNode(&ts.fold_node, ts.graph, nullptr, 0, &kf));
-        if (ts.depth == 2) GEM_CUDA(m, cudaGraphAddKernelNode(&ts.bin_node, ts.graph, &ts.route_node, 1, &kb));
-        else GEM_CUDA(m, cudaGraphAddKernelNode(&ts.bin_node, ts.graph, nullptr, 0, &kb));
-        GEM_CUDA(m, cudaGraphInstantiate(&ts.exec, ts.graph, 0));
+        GEM_CUDA(m, cudaGraphCreate(&tg.graph.p, 0));
+        GEM_CUDA(m, cudaGraphAddKernelNode(&ts.long_node, tg.graph.p, nullptr, 0, &kl));
+        GEM_CUDA(m, cudaGraphAddKernelNode(&ts.route_node, tg.graph.p, nullptr, 0, &kr));
+        GEM_CUDA(m, cudaGraphAddKernelNode(&ts.fold_node, tg.graph.p, nullptr, 0, &kf));
+        if (ts.depth == 2) GEM_CUDA(m, cudaGraphAddKernelNode(&ts.bin_node, tg.graph.p, &ts.route_node, 1, &kb));
+        else GEM_CUDA(m, cudaGraphAddKernelNode(&ts.bin_node, tg.graph.p, nullptr, 0, &kb));
+        GEM_CUDA(m, cudaGraphInstantiate(&tg.exec.p, tg.graph.p, 0));
     } else {
-        GEM_CUDA(m, cudaGraphExecKernelNodeSetParams(ts.exec, ts.long_node, &kl));
-        GEM_CUDA(m, cudaGraphExecKernelNodeSetParams(ts.exec, ts.route_node, &kr));
-        GEM_CUDA(m, cudaGraphExecKernelNodeSetParams(ts.exec, ts.fold_node, &kf));
-        GEM_CUDA(m, cudaGraphExecKernelNodeSetParams(ts.exec, ts.bin_node, &kb));
+        GEM_CUDA(m, cudaGraphExecKernelNodeSetParams(tg.exec.p, ts.long_node, &kl));
+        GEM_CUDA(m, cudaGraphExecKernelNodeSetParams(tg.exec.p, ts.route_node, &kr));
+        GEM_CUDA(m, cudaGraphExecKernelNodeSetParams(tg.exec.p, ts.fold_node, &kf));
+        GEM_CUDA(m, cudaGraphExecKernelNodeSetParams(tg.exec.p, ts.bin_node, &kb));
     }
-    GEM_CUDA(m, cudaGraphLaunch(ts.exec, m->stream));
+    GEM_CUDA(m, cudaGraphLaunch(tg.exec.p, m->stream));
     m->launches += 4;
     m->pend = b.fold;
     if (ts.depth != 2) { ts.routed.active = true; ts.routed.step = stepv; ts.routed.buf = bufv; }
@@ -3445,7 +3434,7 @@ int gem_add_pointcloud2_host_async(gem_map *m, const gem_pointcloud2 *layout, co
     const size_t bgr_bytes = img && enc != IMG_BGR8 ? (size_t)3 * img->width * img->height : 0;
     const bool node = img && m->colour_lookup == GEM_COLOUR_LOOKUP_NODE;
     if (m->pc2_raw[b].cap < mp.bytes || m->pc2_img[b].cap < img_bytes || m->pc2_bgr.cap < bgr_bytes || (node && m->colour.n < n)) {
-        GEM_CUDA(m, cudaStreamSynchronize(m->copy_stream));
+        GEM_CUDA(m, cudaStreamSynchronize(m->copy_stream.p));
         GEM_CUDA(m, cudaStreamSynchronize(m->stream));
         if ((rc = scratch_grow(m, m->pc2_raw[b], mp.bytes, "gem_add_pointcloud2_host_async", m->stream)) ||
             (rc = scratch_grow(m, m->pc2_img[b], img_bytes, "gem_add_pointcloud2_host_async", m->stream)) ||
@@ -3456,11 +3445,11 @@ int gem_add_pointcloud2_host_async(gem_map *m, const gem_pointcloud2 *layout, co
     m->async_calls++;
     // copy stream: the slot's last reader (call i-3) is done (see gem_add_points_host_async); pageable sources are staged
     // by CUDA before cudaMemcpyAsync returns
-    GEM_CUDA(m, cudaStreamWaitEvent(m->copy_stream, m->ev_done[b], 0));
-    if (mp.bytes > 0) GEM_CUDA(m, cudaMemcpyAsync(m->pc2_raw[b].p, data, mp.bytes, cudaMemcpyHostToDevice, m->copy_stream));
-    if (img) GEM_CUDA(m, cudaMemcpyAsync(m->pc2_img[b].p, img->data, img_bytes, cudaMemcpyHostToDevice, m->copy_stream));
-    GEM_CUDA(m, cudaEventRecord(m->ev_h2d[b], m->copy_stream));
-    GEM_CUDA(m, cudaStreamWaitEvent(m->stream, m->ev_h2d[b], 0));
+    GEM_CUDA(m, cudaStreamWaitEvent(m->copy_stream.p, m->ev_done[b].p, 0));
+    if (mp.bytes > 0) GEM_CUDA(m, cudaMemcpyAsync(m->pc2_raw[b].p, data, mp.bytes, cudaMemcpyHostToDevice, m->copy_stream.p));
+    if (img) GEM_CUDA(m, cudaMemcpyAsync(m->pc2_img[b].p, img->data, img_bytes, cudaMemcpyHostToDevice, m->copy_stream.p));
+    GEM_CUDA(m, cudaEventRecord(m->ev_h2d[b].p, m->copy_stream.p));
+    GEM_CUDA(m, cudaStreamWaitEvent(m->stream, m->ev_h2d[b].p, 0));
     // decode into staging set b, then (with an image) BGR8 and the colourisation of ElevationMapping.cpp:331-381 by the
     // handle's lookup mode
     if ((rc = launch_decode(m, layout, mp, m->pc2_raw[b].p, m->d_axyzi[b]))) return rc;
