@@ -27,6 +27,29 @@ A script is a list of steps (op, args).  Ops:
   snapshot / harvest             map_feature + snapshot_shown, then harvest_scrolled_out with the last move's centre
                                  and shift
   sync                           gem_sync, then stats() against the last add call
+
+The later readers read the shown map as it stands: the live elevation, variance, intensity and colour, with the rough,
+slope and traversability the last feature pass wrote (the oracle keeps that pass's outputs).  Their ops:
+  grid_cloud src                 gem_export_grid_cloud of the shown map or the snapshot (src: shown / snapshot)
+  split src                      gem_grid_cloud_split: road, obstacle and the filter's stats
+  octrees src                    global_octrees: the split, then the 0.2 m road and 0.1 m obstacle ColorOcTree streams
+  costmap src size               gem_costmap_update_origin of the layer grid of that window size to the map centre, then
+                                 gem_costmap_mark_map into it: grid, window and marks (each size keeps its own grid, both
+                                 calls share the handle's costmap scratch)
+  ros                            gem_ros_visual_points, gem_ros_grid_map, gem_ros_orthomosaic into device and pinned
+                                 memory at offsets that are not 16-byte aligned, guard bytes around them
+  layer_device                   gem_get_layer_device of every layer, rough, slope and the feature traversability included
+  local                          gem_harvest_to_local_map with the last move's centre and shift: records and store size
+  cut dense pose                 cut_submap (dense: the MLS points of the taken local map between it and the grid cloud),
+                                 then global_map_push of the cut: the whole global-map stack is compared
+
+Hazards (kind, step) the CPU suite checks: long_clear, wrap, overflow, full_shift_pending, boundary, var_below_floor,
+set_below_floor, pending_fold_and_clears, multi_frames and harvest (each at the step that raises it), and, in the scripts
+named readers_after_*, at a later reader placed directly after
+  reader_fold_in_flight          a pipelined add (stream, host_async) whose fold is still to be issued
+  reader_queued_clears           a move whose bands are queued (wrapping the storage edge on both axes, or the whole map)
+  reader_floor_pending           a negative var_update or a set_variance: the variance floor waits for the next Fuse
+  reader_parked                  gem_process_points with its fuse still to come (the pending operations are parked)
 """
 from __future__ import annotations
 
@@ -36,7 +59,14 @@ from dataclasses import dataclass, field
 
 import numpy as np
 
+import costmap_oracle
+import mls_oracle
 import np_reference
+import octree_oracle
+import oracle_lib
+import rosmsg_oracle
+import split_oracle
+import submap_oracle
 from oracle_lib import OracleMap
 
 f32 = np.float32
@@ -45,6 +75,28 @@ MAX_POINTS = 1 << 16                 # per-launch capacity of the device maps th
 ADD_VARIANTS = ("host", "dev", "stream", "host_async", "pcl")
 PIPELINED = ("stream", "host_async", "multi")
 EMPTY_VARIANTS = ADD_VARIANTS + ("multi",)
+READERS = ("grid_cloud", "split", "octrees", "costmap", "ros", "layer_device", "local", "cut")
+READER_HAZARDS = ("reader_fold_in_flight", "reader_queued_clears", "reader_floor_pending", "reader_parked")
+COST_RES, COST_THRESH, COST_FILL = 0.15, 0.7, 255      # costmap cells of 1.5 map cells: several map cells per costmap cell
+COST_SIZES = ((23, 19), (41, 37))                       # inside the 64-cell window, and wider than it
+ROS_HEADER = {"seq": 7, "stamp_sec": 1700000000, "stamp_nsec": 123456789, "frame_id": "map"}
+ROS_OFFSETS = {"cuda": 7, "pinned": 13}                 # destination offsets that are not 16-byte aligned
+ROS_GUARD = 64
+CUT_SEED = 11                                           # the MLS seed of the dense cuts
+
+
+def initial_window(sx, sy):
+    return (-sx * COST_RES / 2, -sy * COST_RES / 2, COST_RES, sx, sy)
+
+
+def initial_grid(sx, sy):
+    """a costmap layer grid of free, lethal and unknown cells, so that a cell left unwritten shows"""
+    return np.random.default_rng(1000 * sx + sy).choice(np.array([0, 254, 255], np.uint8), (sy, sx))
+
+
+def cost_origin(centre, sx, sy):
+    """the origin update_origin is asked for: the window centred on the map centre"""
+    return float(centre[0]) - sx * COST_RES / 2, float(centre[1]) - sy * COST_RES / 2
 
 
 # ---- gem_move's arithmetic, restated (gem_api.cu gem_move, oracle orc_move) ----------------------------------------------
@@ -238,6 +290,18 @@ class Builder:
         """a move of (dx, dy) cells (aligned positions, no rounding question)"""
         r = self.s.res
         return self.move(float(self.centre[0]) + dx * r, float(self.centre[1]) + dy * r, z)
+
+    def move_to_start(self, sx, sy):
+        """a move that leaves the storage start at (sx, sy), by a shift of less than L / 2 cells per axis"""
+        L = self.s.L
+        d = [(self.start[i] - t) % L for i, t in enumerate((sx, sy))]
+        d = [v - L if v >= L // 2 else v for v in d]
+        i = self.move_cells(d[0], d[1])
+        assert self.start == [sx, sy], (self.start, sx, sy)
+        return i
+
+    def cut(self, dense):
+        return self._step("cut", dense=dense, pose=pose(float(self.centre[0]), float(self.centre[1]), 0.5))
 
     def add(self, variant="stream", T=None, **kw):
         if variant == "multi":
@@ -484,7 +548,107 @@ def hand_written():
     b.move_cells(-9, 3)
     b.add("host")
     out.append(b.done())
+    return out + readers_after_hazards() + [node_frame_loop()]
+
+
+# ---- the later readers straight after each hazard ------------------------------------------------------------------------
+def _reader_ops(k):
+    """the readers of one readers_after_* script, in order: every op of READERS, the costmap at both sizes (its scratch
+    alternates between the marks' ints and update_origin's bytes at both sizes), both sources, dense and plain cuts"""
+    a, b = ("shown", "snapshot") if k % 2 == 0 else ("snapshot", "shown")
+    return [("grid_cloud", {"src": "shown"}), ("split", {"src": a}), ("octrees", {"src": b}),
+            ("costmap", {"src": "shown", "size": COST_SIZES[0]}), ("ros", {}), ("layer_device", {}), ("local", {}),
+            ("cut", {"dense": True}), ("costmap", {"src": "shown", "size": COST_SIZES[1]}), ("grid_cloud", {"src": "snapshot"}),
+            ("split", {"src": b}), ("octrees", {"src": a}), ("costmap", {"src": "snapshot", "size": COST_SIZES[0]}),
+            ("cut", {"dense": False})]
+
+
+def _fill(b):
+    """an add that puts a few points into every cell of flat ground, then features + snapshot: the whole window is shown
+    and traversable, so every reader has cells to read and the harvest has cells to take"""
+    b.add("stream", stripe=1, ks=(1, 2, 3), relief=0.05)
+    b.op("snapshot")
+
+
+def _reader(b, op, args):
+    return b.cut(args["dense"]) if op == "cut" else b.op(op, **args)
+
+
+def readers_after_hazards():
+    """one script per hazard: each round sets the map up, raises the hazard, and puts the next reader right after it"""
+    out = []
+    for k, (name, trigger) in enumerate((("readers_after_stream_fold", "stream"),
+                                         ("readers_after_host_async_fold", "host_async"),
+                                         ("readers_after_wrapping_clears", "wrap"), ("readers_after_full_shift", "full"),
+                                         ("readers_after_negative_var_update", "var_update"),
+                                         ("readers_after_set_variance", "set_variance"),
+                                         ("readers_after_parked_process", "process"))):
+        b = Builder(name, seed=20 + k)
+        for op, args in _reader_ops(k):
+            if trigger == "wrap":
+                b.move_to_start(2, 3)
+                _fill(b)
+                h, kind = b.move_cells(5, 6), "reader_queued_clears"     # shifts above the start: both bands wrap
+            elif trigger == "full":
+                _fill(b)
+                h, kind = b.move_cells(b.s.L + 1, -2), "reader_queued_clears"
+            else:
+                _fill(b)
+                b.move_cells(3, -2)
+                if trigger in ("stream", "host_async"):
+                    h, kind = b.add(trigger, relief=0.3), "reader_fold_in_flight"
+                elif trigger == "var_update":
+                    b.add("stream", relief=0.3)
+                    h, kind = b.op("var_update", dv=-7.5e-5), "reader_floor_pending"
+                elif trigger == "set_variance":
+                    b.add("stream", relief=0.3)
+                    h, kind = b.op("set_variance"), "reader_floor_pending"
+                else:
+                    h, kind = b.op("process", cloud=b.new_cloud(relief=0.3), T=np.eye(4)), "reader_parked"
+            i = _reader(b, op, args)
+            assert i == h + 1
+            b.hazard(kind, i)
+            if trigger == "process":
+                b.op("fuse")
+        b.add("stream")                                   # a Fuse takes the last round's pending floor and clears
+        out.append(b.done())
     return out
+
+
+NODE_FRAMES = 14
+
+
+def node_frame_loop():
+    """the node's per-frame order on one handle: Move, harvest into the local map, add, features + snapshot, the grid
+    cloud, the map topics, the local costmap; every third frame the global map's split and octrees and a keyframe cut
+    (every other one dense); then the ray clean-up.  The first frames fill the window with small moves, the later ones
+    scroll it away in long moves over sparse clouds, and the costmap window widens and narrows again: the grid cloud,
+    the harvest and the costmap each grow and later shrink."""
+    b = Builder("node_frame_loop", seed=31)
+    sizes = [(9, 7), (15, 13), (23, 19), (31, 27), (41, 37), (49, 45), (49, 45), (41, 37), (31, 27), (23, 19), (15, 13),
+             (9, 7), (9, 7), (15, 13)]
+    variants = ("stream", "stream", "host_async", "host", "stream", "dev", "stream")
+    for k in range(NODE_FRAMES):
+        if k < 6:
+            b.move_cells(1, (k % 2) - 1)
+        else:
+            b.move_cells(7, -6)
+        if k > 0:
+            b.op("local")
+        if k < 6:
+            b.add(variants[k % len(variants)], sparse=500, relief=0.25)
+        else:
+            b.add(variants[k % len(variants)], stripe=64, sparse=80, scale=0.5, relief=0.25)
+        b.op("snapshot")
+        b.op("grid_cloud", src="shown")
+        b.op("ros")
+        b.op("costmap", src="shown", size=sizes[k])
+        if k % 3 == 2:
+            b.op("split", src="snapshot")
+            b.op("octrees", src="snapshot")
+            b.cut(dense=k % 6 == 5)
+        b.op("raytracing")
+    return b.done()
 
 
 def _opt_move_centre(centre, p, res):
@@ -516,11 +680,20 @@ def random_script(seed, n_steps=28):
     L = int(rng.choice([64, 80, 96]))
     b = Builder(f"random_{seed}", L=L, seed=seed)
     vocab = ["add", "add", "add", "add", "move", "move", "move", "layers", "var_update", "set_variance", "opt_move",
-             "closeloop", "process", "empty", "export_ray", "snapshot", "sync", "multi", "raytracing"]
+             "closeloop", "process", "empty", "export_ray", "snapshot", "sync", "multi", "raytracing"] + list(READERS)
     snap = False
     for _ in range(n_steps):
         op = vocab[int(rng.integers(len(vocab)))]
-        if op == "add":
+        if op in ("grid_cloud", "split", "octrees", "costmap"):
+            args = {"src": "snapshot" if snap and rng.uniform() < 0.4 else "shown"}
+            if op == "costmap":
+                args["size"] = COST_SIZES[int(rng.integers(len(COST_SIZES)))]
+            b.op(op, **args)
+        elif op == "local":
+            b.op("local" if snap and b.last_move is not None else "layer_device")
+        elif op == "cut":
+            b.cut(dense=False)
+        elif op == "add":
             b.add(str(rng.choice(ADD_VARIANTS + ("stream", "stream"))), stripe=int(rng.choice([16, 24, 48])))
         elif op == "multi":
             b.multi(nseg=int(rng.integers(2, 9)), yaw0=float(rng.uniform(-3, 3)))
@@ -584,6 +757,12 @@ class OracleRun:
         self.proc = None
         self.last_move = None
         self.stats = None
+        n = script.L * script.L
+        # the outputs of the last feature pass (the device map starts with rough = slope = 0, traversability -10)
+        self.feat = {"rough": np.zeros(n, f32), "slope": np.zeros(n, f32), "traver": np.full(n, f32(-10))}
+        self.local = submap_oracle.LocalMapDict()
+        self.pushed = []                                 # the global map's submaps
+        self.cost = {}                                   # window size -> (window, grid) of that costmap layer
 
     def close(self):
         self.o.close()
@@ -610,6 +789,7 @@ class OracleRun:
         if op == "move":
             before = o.state()
             ops = move_model(L, self.s.res, before[0], before[1], a["pos"])[3]
+            out["band_filled"] = int((o.get_layer("elevation").reshape(-1)[band_cells(L, ops)] != f32(-10)).sum())
             out["returned"] = o.move(a["pos"])
             out["state"] = o.state()
             out["ops"] = ops
@@ -670,19 +850,22 @@ class OracleRun:
             out["layers"] = self.layers()
             out.update(self.readouts())
         elif op == "export_ray":
-            out["feature"] = o.map_feature()
+            out["feature"] = self._features()
             out["export"] = o.export_layers()            # what the node reads: taken before the ray clean-up
             o.raytracing()
         elif op == "raytracing":
             o.raytracing()
         elif op == "snapshot":
-            out["feature"] = o.map_feature()             # the node snapshots what show() just drew
+            out["feature"] = self._features()            # the node snapshots what show() just drew
             o.snapshot_shown()
         elif op == "harvest":
             centre, shift = self.last_move
             out["harvest"] = o.harvest_scrolled_out(centre, shift)
         elif op == "sync":
             out["stats"] = self.stats
+        elif op in READERS:
+            out["shown"] = self.shown_mask()
+            out.update(self.reader(op, a))
         else:
             raise ValueError(op)
         return out
@@ -690,9 +873,115 @@ class OracleRun:
     def layers(self):
         return {n: self.o.get_layer(n) for n in LAYERS}
 
+    # ---- the later readers ----------------------------------------------------------------------------------------------
+    def _features(self):
+        f = self.o.map_feature()
+        self.feat = {k: f[k].copy() for k in ("rough", "slope", "traver")}
+        return f
+
+    def shown(self):
+        """the shown map as the readers take it: live cells, the last feature pass's rough / slope / traversability"""
+        f = {n: self.o.get_layer(n).reshape(-1) for n in ("elevation", "variance", "intensity", "color_r", "color_g", "color_b")}
+        f.update(self.feat)
+        return f
+
+    def shown_mask(self):
+        f = self.shown()
+        return (f["elevation"] != f32(-10)) & (f["traver"] != f32(-10)) & ~np.isnan(f["traver"])
+
+    def grid_res(self):
+        return float(f32(self.s.res))
+
+    def grid_cloud(self, src):
+        if src == "shown":
+            centre, start, _ = self.o.state()
+            return submap_oracle.grid_cloud(self.shown(), self.s.L, centre, start, self.grid_res())
+        f, centre, start = self.o._prev
+        return submap_oracle.grid_cloud(f, self.s.L, centre, start, self.grid_res())
+
+    def show(self):
+        """orc_show of the shown map: orthomosaic, visual cloud xyz and rgb"""
+        f, L = self.shown(), self.s.L
+        img = np.empty((L, L, 3), np.uint8)
+        xyz = np.empty((L * L, 3), f32)
+        rgb = np.empty((L * L, 3), np.uint8)
+        cnt = oracle_lib.C.c_int()
+        p = oracle_lib._p
+        self.o.lib.orc_show(self.o.m, 0.0, p(f["elevation"]), p(f["traver"]), p(f["color_r"]), p(f["color_g"]), p(f["color_b"]),
+                            p(img), p(xyz), p(rgb), oracle_lib.C.byref(cnt))
+        return img, xyz[:cnt.value].copy(), rgb[:cnt.value].copy()
+
+    def cost_traver(self, src):
+        """show()'s traversability [ix, iy], NaN where the cell is not shown, and that grid's centre and start"""
+        L = self.s.L
+        if src == "shown":
+            f = self.shown()
+            centre, start, _ = self.o.state()
+            t = np.where(self.shown_mask(), f["traver"], f32(np.nan))
+        else:
+            f, centre, start = self.o._prev
+            t = oracle_lib.export_from_feature(f, L)["traver"]
+        return np.asarray(t, f32).reshape(L, L), centre, start
+
+    def reader(self, op, a):
+        o, L = self.o, self.s.L
+        if op == "grid_cloud":
+            return {"cloud": self.grid_cloud(a["src"])}
+        if op in ("split", "octrees"):
+            cloud = self.grid_cloud(a["src"])
+            sp = split_oracle.grid_split(cloud)
+            out = {"road": sp["road"], "obstacle": sp["obstacle"], "points": int(cloud.shape[0])}
+            out.update({k: sp[k] for k in ("valid", "mean", "stddev", "threshold")})
+            if op == "octrees":
+                out["road_stream"] = octree_oracle.color_octree(sp["road"], 0.2)[0]
+                out["obstacle_stream"] = octree_oracle.color_octree(sp["obstacle"], 0.1)[0]
+            return out
+        if op == "costmap":
+            sx, sy = a["size"]
+            if a["size"] not in self.cost:
+                self.cost[a["size"]] = (initial_window(sx, sy), initial_grid(sx, sy))
+            w, grid = self.cost[a["size"]]
+            nx, ny = cost_origin(o.state()[0], sx, sy)
+            w, grid = costmap_oracle.update_origin(w, nx, ny, COST_FILL, grid)
+            t, centre, start = self.cost_traver(a["src"])
+            grid, marks = costmap_oracle.mark_map(t, L, self.grid_res(), centre, start, w, grid, COST_THRESH, True)
+            self.cost[a["size"]] = (w, grid)
+            return {"window": w, "grid": grid, "marks": marks}
+        if op == "ros":
+            ro = rosmsg_oracle
+            h = ro.header(ROS_HEADER["seq"], ROS_HEADER["stamp_sec"], ROS_HEADER["stamp_nsec"], ROS_HEADER["frame_id"].encode())
+            img, xyz, rgb = self.show()
+            centre, start, _ = o.state()
+            layers = oracle_lib.export_from_feature(self.shown(), L)
+            return {"ros": {"visual_points": ro.visual_points(h, xyz, rgb),
+                            "grid_map": ro.grid_map(h, L, self.grid_res(), float(centre[0]), float(centre[1]), start, layers),
+                            "orthomosaic": ro.image(h, L, img.tobytes())}}
+        if op == "layer_device":
+            out = {n: o.get_layer(n) for n in LAYERS}
+            out.update({n: self.feat[k].reshape(L, L) for n, k in (("rough", "rough"), ("slope", "slope"),
+                                                                   ("traver_out", "traver"))})
+            return {"device_layers": out}
+        if op == "local":
+            centre, shift = self.last_move
+            rec, n = o.harvest_scrolled_out(centre, shift)
+            self.local.insert_all(rec)
+            return {"local": (rec, n), "local_size": len(self.local)}
+        if op == "cut":
+            local = self.local.records()
+            parts = [local]
+            if a["dense"] and local.shape[0]:
+                parts.append(mls_oracle.upsample(local, {"seed": CUT_SEED})[0])
+            parts.append(self.grid_cloud("shown"))
+            cut = np.concatenate(parts)
+            self.local.clear()
+            self.pushed.append(cut)
+            return {"cut": cut, "local_taken": int(local.shape[0]), "global": np.concatenate(self.pushed),
+                    "submaps": len(self.pushed)}
+        raise ValueError(op)
+
     def readouts(self):
         o = self.o
-        out = {"feature": o.map_feature(), "export": o.export_layers()}
+        out = {"feature": self._features(), "export": o.export_layers()}
         out["ortho"], out["vis_xyz"], out["vis_rgb"] = o.show()
         return out
 

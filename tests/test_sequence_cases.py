@@ -1,5 +1,6 @@
 """The call scripts of tests/sequence_cases.py on the oracle alone: every script runs, the restatement of gem_move's
-band arithmetic agrees with the oracle's Move, and every hand-written script reaches the hazard it is named after."""
+band arithmetic agrees with the oracle's Move, and every hand-written script reaches the hazard it is named after: every
+later reader straight after every hazard kind, and the node's frame loop growing and shrinking what its readers return."""
 import numpy as np
 import pytest
 
@@ -167,19 +168,141 @@ def _check_harvest(s, trace, i):
     assert trace[i][2]["harvest"][1] > 10, f"{s.name} step {i}: the harvest takes {trace[i][2]['harvest'][1]} records"
 
 
+def _check_reader(s, trace, i):
+    assert trace[i][0] in sc.READERS, f"{s.name} step {i}: {trace[i][0]} is not one of the later readers"
+
+
+def _check_reader_fold_in_flight(s, trace, i):
+    """a pipelined add right before the reader, whose fold changes cells the reader reads"""
+    _check_reader(s, trace, i)
+    op, a, out = trace[i - 1]
+    assert op == "add" and a["variant"] in ("stream", "host_async"), f"{s.name} step {i}: no pipelined add right before"
+    hit = _counts(s.L, out["keys"])[trace[i][2]["shown"]]
+    assert (hit > 0).sum() > 100, f"{s.name} step {i}: the fold in flight touches {(hit > 0).sum()} shown cells"
+
+
+def _check_reader_queued_clears(s, trace, i):
+    """a move right before the reader whose bands wrap the storage edge on both axes or clear the whole map, over cells
+    that held heights, with no fusing call since the fill before it"""
+    _check_reader(s, trace, i)
+    op, _, out = trace[i - 1]
+    assert op == "move", f"{s.name} step {i}: no move right before"
+    ops = out["ops"]
+    assert ("all",) in ops or all(sum(o[0] == k for o in ops) == 2 for k in ("rows", "cols")), f"{s.name} step {i}: {ops}"
+    assert out["band_filled"] > 100, f"{s.name} step {i}: the bands clear {out['band_filled']} cells with heights"
+
+
+def _check_reader_floor_pending(s, trace, i):
+    _check_reader(s, trace, i)
+    op, a, out = trace[i - 1]
+    assert op in ("var_update", "set_variance"), f"{s.name} step {i}: {op} right before"
+    v = out["variance"]
+    assert ((v < f32(1e-4)) & (v != f32(-10))).sum() > 100, f"{s.name} step {i}: no variance below the floor"
+    assert any(op in ("add", "multi", "empty", "fuse") for op, _, _ in trace[i + 1:]), f"{s.name} step {i}: no Fuse follows"
+
+
+def _check_reader_parked(s, trace, i):
+    """gem_process_points right before the reader, its fuse still to come, with the clears of a move parked"""
+    _check_reader(s, trace, i)
+    assert trace[i - 1][0] == "process" and trace[i - 2][0] == "move" and trace[i - 2][2]["ops"], s.name
+    j = next(j for j in range(i + 1, len(trace)) if trace[j][0] in ("add", "multi", "empty", "fuse", "process"))
+    assert trace[j][0] == "fuse", f"{s.name} step {i}: the fuse does not follow"
+
+
 CHECKS = {"harvest": _check_harvest, "long_clear": _check_long_clear, "wrap": _check_wrap, "overflow": _check_overflow,
           "full_shift_pending": _check_full_shift_pending, "boundary": _check_boundary,
           "var_below_floor": _check_var_below_floor, "set_below_floor": _check_set_below_floor,
-          "pending_fold_and_clears": _check_pending_fold_and_clears, "multi_frames": _check_multi_frames}
+          "pending_fold_and_clears": _check_pending_fold_and_clears, "multi_frames": _check_multi_frames,
+          "reader_fold_in_flight": _check_reader_fold_in_flight, "reader_queued_clears": _check_reader_queued_clears,
+          "reader_floor_pending": _check_reader_floor_pending, "reader_parked": _check_reader_parked}
 
 
 @pytest.mark.parametrize("name", sorted(HAND))
 def test_hand_written_script_reaches_its_hazard(traces, name):
     s, trace = traces[name]
     assert s.hazards or name in ("empty_call_flushes", "export_around_raytracing", "host_async_alternating",
-                                 "reader_between_pipelined")
+                                 "reader_between_pipelined", "node_frame_loop")
     for kind, i in s.hazards:
         CHECKS[kind](s, trace, i)
+
+
+def test_every_later_reader_follows_every_hazard(traces):
+    """across the readers_after_* scripts each reader op sits directly after each hazard kind, and after each way to
+    raise it: a stream and a host_async fold, wrapping bands and a full shift, a negative var_update and a set_variance"""
+    seen, ways = set(), set()
+    for s, trace in traces.values():
+        for kind, i in s.hazards:
+            if kind in sc.READER_HAZARDS:
+                op = trace[i][0]
+                seen.add((op, kind))
+                prev_op, prev_a, prev_out = trace[i - 1]
+                way = prev_a.get("variant") if prev_op == "add" else \
+                    ("all" if ("all",) in prev_out.get("ops", []) else "wrap") if prev_op == "move" else prev_op
+                ways.add((op, way))
+    missing = [(op, kind) for op in sc.READERS for kind in sc.READER_HAZARDS if (op, kind) not in seen]
+    assert not missing, missing
+    missing = [(op, w) for op in sc.READERS for w in ("stream", "host_async", "wrap", "all", "var_update", "set_variance",
+                                                      "process") if (op, w) not in ways]
+    assert not missing, missing
+
+
+def test_readers_after_hazards_read_sources_at_both_kinds_and_cut_both_ways(traces):
+    """each readers_after_* script reads the shown map and the snapshot, marks at both costmap sizes (update_origin
+    between every two marks), and cuts dense with a local map to densify as well as plain"""
+    for name in (n for n in HAND if n.startswith("readers_after_")):
+        s, trace = traces[name]
+        srcs = {(op, a["src"]) for op, a, _ in trace if "src" in a}
+        assert {(op, src) for op in ("grid_cloud", "split", "octrees") for src in ("shown", "snapshot")} <= srcs, name
+        assert {a["size"] for op, a, _ in trace if op == "costmap"} == set(sc.COST_SIZES), name
+        cuts = [(a["dense"], out["local_taken"]) for op, a, out in trace if op == "cut"]
+        assert any(d and n > 100 for d, n in cuts) and any(not d for d, _ in cuts), (name, cuts)
+        assert any(out["local"][1] > 100 for op, _, out in trace if op == "local"), name
+
+
+def _rises_and_falls(v):
+    return len(v) >= 3 and max(v) > v[0] and max(v) > v[-1]
+
+
+def test_node_frame_loop_sizes_rise_and_fall(traces):
+    """on one handle the grid cloud, the harvest and the costmap window (and what the costmap marks) grow and later
+    shrink, so every shared scratch is reused both larger and smaller than before; cuts are taken dense and plain"""
+    s, trace = traces["node_frame_loop"]
+    grid = [out["cloud"].shape[0] for op, a, out in trace if op == "grid_cloud"]
+    harvest = [out["local"][1] for op, _, out in trace if op == "local"]
+    window = [a["size"][0] * a["size"][1] for op, a, _ in trace if op == "costmap"]
+    marked = [out["marks"]["marked"] for op, _, out in trace if op == "costmap"]
+    for what, v in (("grid cloud", grid), ("harvest", harvest), ("costmap window", window), ("costmap marks", marked)):
+        assert _rises_and_falls(v), (what, v)
+    assert len(grid) == sc.NODE_FRAMES
+    cuts = [(a["dense"], out["local_taken"]) for op, a, out in trace if op == "cut"]
+    assert any(d and n > 0 for d, n in cuts) and any(not d and n > 0 for d, n in cuts), cuts
+
+
+def _same_output(a, b):
+    if isinstance(a, dict):
+        return a.keys() == b.keys() and all(_same_output(a[k], b[k]) for k in a)
+    if isinstance(a, (list, tuple)):
+        return len(a) == len(b) and all(_same_output(x, y) for x, y in zip(a, b))
+    if isinstance(a, np.ndarray):
+        return a.dtype == b.dtype and a.shape == b.shape and a.tobytes() == b.tobytes()
+    if isinstance(a, float):
+        return np.float64(a).tobytes() == np.float64(b).tobytes()
+    return a == b
+
+
+@pytest.mark.parametrize("name", ["node_frame_loop", "readers_after_stream_fold", "random_103"])
+def test_reader_traces_are_deterministic(traces, name):
+    """a second oracle run of the script gives the same outputs, bit for bit"""
+    s, trace = traces[name]
+    again = sc.run_oracle(sc.script_by_name(name))
+    assert len(again) == len(trace)
+    for i, ((op, _, out), (_, _, out2)) in enumerate(zip(trace, again)):
+        assert _same_output(out, out2), (name, i, op)
+
+
+def test_random_scripts_draw_the_later_readers():
+    ops = {op for seed in sc.SEEDS for op, _ in sc.random_script(seed).steps}
+    assert len(ops & set(sc.READERS)) >= 5, ops
 
 
 def test_every_add_variant_and_empty_call_is_scripted():

@@ -2,7 +2,9 @@
 add path has: one CUDA graph per call (the default), profiling on (fully serial, with per-kernel event timing), the
 padded shared-memory launch of GEM_B200_EXCLUSIVE and a small GEM_B200_FOLD_BLOCKS cap.  At every reader and at the end of a script everything observable is compared bit for bit:
 all layers, the state after each move, map_feature, the exports, the orthomosaic, the visual cloud, harvested records,
-process_points outputs and stats().  A difference names the script, the step and the schedule."""
+process_points outputs and stats(); and at the later readers the grid clouds, the split and its stats, the octree
+streams, the costmap grids, windows and marks, the ROS messages byte for byte, the device layers, the local map, the
+cuts and the global-map stack.  A difference names the script, the step and the schedule."""
 import ctypes as C
 
 import numpy as np
@@ -56,6 +58,7 @@ class DeviceRun:
         self.keep = []           # device and pinned inputs stay alive until the map is closed
         self.proc = None
         self.last_move = None
+        self.cost = {}           # window size -> [window, layer grid]
 
     def check(self, where, what, got, want):
         d = _same(got, want)
@@ -208,6 +211,102 @@ class DeviceRun:
         elif op == "sync":
             g.sync()
             self._stats(where, want["stats"])
+        elif op in sc.READERS:
+            self.reader(where, op, a, want)
+        else:
+            raise ValueError(op)
+
+    # ---- the later readers ----------------------------------------------------------------------------------------------
+    def _records(self, where, what, got, want):
+        self.check(where, what, got.cpu().numpy() if hasattr(got, "cpu") else got, want)
+
+    def _split_stats(self, where, st, want):
+        for k in ("points", "valid", "road", "obstacle"):
+            n = want[k].shape[0] if k in ("road", "obstacle") else want[k]
+            assert st[k] == n, f"{self.s.name} step {where} [{self.schedule}]: split {k} {st[k]} != {n}"
+        for k in ("mean", "stddev", "threshold"):
+            self.check(where, f"split {k}", np.float64(st[k]).view(np.uint64), np.float64(want[k]).view(np.uint64))
+
+    def _ros(self, where, name, call, want):
+        """the message into guarded device and pinned buffers at an offset that is not 16-byte aligned"""
+        import torch
+        nb = C.c_longlong(-1)
+        assert call(None, 0, C.byref(nb)) == 0 and nb.value == len(want), \
+            f"{self.s.name} step {where} [{self.schedule}]: {name} size {nb.value} != {len(want)}"
+        for kind, off in sc.ROS_OFFSETS.items():
+            n = len(want) + off + 2 * sc.ROS_GUARD
+            buf = torch.full((n,), 0xA5, dtype=torch.uint8, device="cuda") if kind == "cuda" else \
+                torch.full((n,), 0xA5, dtype=torch.uint8).pin_memory()
+            at = sc.ROS_GUARD + off
+            assert call(C.c_void_p(buf.data_ptr() + at), len(want), C.byref(nb)) == 0 and nb.value == len(want)
+            torch.cuda.synchronize()
+            got = buf.cpu().numpy().tobytes()
+            assert got[:at] == b"\xa5" * at and got[at + len(want):] == b"\xa5" * (n - at - len(want)), \
+                f"{self.s.name} step {where} [{self.schedule}]: {name} wrote outside its bytes ({kind})"
+            if got[at:at + len(want)] != want:
+                k = next(i for i in range(len(want)) if got[at + i] != want[i])
+                raise AssertionError(f"{self.s.name} step {where} [{self.schedule}]: {name} ({kind}) differs from byte {k} "
+                                     f"of {len(want)}")
+
+    def reader(self, where, op, a, want):
+        import torch
+        g, L = self.g, self.s.L
+        if op == "grid_cloud":
+            self._records(where, f"grid cloud {a['src']}", g.export_grid_cloud(a["src"]), want["cloud"])
+        elif op == "split":
+            road, obstacle, st = g.grid_cloud_split(a["src"])
+            self._records(where, "split road", road, want["road"])
+            self._records(where, "split obstacle", obstacle, want["obstacle"])
+            self._split_stats(where, st, want)
+        elif op == "octrees":
+            rs, os_, st = g.global_octrees(a["src"])
+            self._split_stats(where, st, want)
+            self.check(where, "road octree", rs.cpu().numpy(), want["road_stream"])
+            self.check(where, "obstacle octree", os_.cpu().numpy(), want["obstacle_stream"])
+        elif op == "costmap":
+            sx, sy = a["size"]
+            if a["size"] not in self.cost:
+                self.cost[a["size"]] = [sc.initial_window(sx, sy), torch.from_numpy(sc.initial_grid(sx, sy)).cuda()]
+            w, grid = self.cost[a["size"]]
+            nx, ny = sc.cost_origin(g.state()[0], sx, sy)
+            w = g.costmap_update_origin(w, nx, ny, sc.COST_FILL, grid)
+            self.cost[a["size"]][0] = w
+            assert np.float64(w[:3]).tobytes() == np.float64(want["window"][:3]).tobytes(), \
+                f"{self.s.name} step {where} [{self.schedule}]: costmap window {w} != {want['window']}"
+            marks = g.costmap_mark_map(w, grid, sc.COST_THRESH, a["src"], True)
+            self.check(where, f"costmap grid {a['size']}", grid.cpu().numpy(), want["grid"])
+            for k, v in want["marks"].items():
+                assert np.float64(marks[k]).tobytes() == np.float64(v).tobytes(), \
+                    f"{self.s.name} step {where} [{self.schedule}]: costmap marks {k} {marks[k]} != {v}"
+        elif op == "ros":
+            hc = gem_b200.RosHeader(**sc.ROS_HEADER).c()
+            lib, h = g._lib, g.handle
+            for name in ("visual_points", "grid_map", "orthomosaic"):   # visual_points first: it reads the map first
+                fn = getattr(lib, f"gem_ros_{name}")
+                self._ros(where, name, lambda p, c, nb, fn=fn: fn(h, C.byref(hc), p, c, nb), want["ros"][name])
+        elif op == "layer_device":
+            for name, b in want["device_layers"].items():
+                out = torch.full((L, L), -7, dtype=torch.int32 if name.startswith("color") else torch.float32, device="cuda")
+                g.get_layer_device(name, out)
+                torch.cuda.synchronize()
+                self.check(where, f"device layer {name}", out.cpu().numpy(), b)
+        elif op == "local":
+            centre, shift = self.last_move
+            rec, n = g.harvest_to_local_map(centre, shift, records=True)
+            orec, on = want["local"]
+            assert n == on, f"{self.s.name} step {where} [{self.schedule}]: harvested {n} != {on}"
+            self.check(where, "harvested records", rec, orec)
+            assert g.local_map_size() == want["local_size"], \
+                f"{self.s.name} step {where} [{self.schedule}]: local map {g.local_map_size()} != {want['local_size']}"
+        elif op == "cut":
+            cut = g.cut_submap(dense=a["dense"], seed=sc.CUT_SEED)
+            self._records(where, "dense cut" if a["dense"] else "cut", cut, want["cut"])
+            assert g.local_map_size() == 0
+            g.global_map_push(cut, a["pose"])
+            submaps, _, records = g.global_map_info()
+            assert (submaps, records) == (want["submaps"], want["global"].shape[0]), \
+                f"{self.s.name} step {where} [{self.schedule}]: global map {submaps} submaps, {records} records"
+            self._records(where, "global map", g.global_map_records(), want["global"])
         else:
             raise ValueError(op)
 
