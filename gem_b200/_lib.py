@@ -101,6 +101,18 @@ class GemVoxelGridInfo(C.Structure):
     _fields_ = [("count", C.c_int), ("used", C.c_int), ("passthrough", C.c_int)]
 
 
+PREFILTER_MAX_STEPS = 4
+
+
+class GemPrefilter(C.Structure):
+    _fields_ = [("nsteps", C.c_int), ("step", GemVoxelGridParams * PREFILTER_MAX_STEPS)]
+
+
+class GemProjection(C.Structure):
+    _fields_ = [("T_camera", C.c_double * 12), ("T_lidar", C.c_double * 16), ("width", C.c_int), ("height", C.c_int),
+                ("row_stride", C.c_int)]
+
+
 class GemMlsParams(C.Structure):
     _fields_ = [("search_radius", C.c_double), ("sqr_gauss_param", C.c_double), ("polynomial_fit", C.c_int), ("order", C.c_int),
                 ("upsampling", C.c_int), ("point_density", C.c_int), ("seed", C.c_ulonglong)]
@@ -258,6 +270,11 @@ SYMBOLS = {
     "gem_image_to_bgr8": (C.c_int, [_P, C.c_char_p, _P, C.c_int, C.c_int, C.c_int, _P, C.c_int]),
     "gem_add_pointcloud2_host_async": (C.c_int, [_P, C.POINTER(GemPointCloud2), _P, C.c_ulonglong, C.POINTER(GemCameraImage),
                                                  C.POINTER(GemFrame)]),
+    "gem_add_pointcloud2_filtered_host_async": (C.c_int, [_P, C.POINTER(GemPointCloud2), _P, C.c_ulonglong,
+                                                          C.POINTER(GemCameraImage), C.POINTER(GemPrefilter), C.POINTER(GemFrame)]),
+    "gem_add_points_filtered_stream": (C.c_int, [_P, _P, C.c_int, C.POINTER(GemPrefilter), _P, C.POINTER(GemProjection),
+                                                 C.POINTER(GemFrame)]),
+    "gem_prefilter_info": (C.c_int, [_P, C.POINTER(GemVoxelGridInfo), C.c_int]),
     "gem_pcd_header": (C.c_int, [C.c_longlong, C.c_int, C.c_char_p, C.c_int, _IP]),
     "gem_pcd_format": (C.c_int, [_P, _P, C.c_int, C.c_int, _P, C.c_longlong, C.POINTER(C.c_longlong)]),
     "gem_ros_grid_map": (C.c_int, [_P, C.POINTER(GemRosHeader), _P, C.c_longlong, C.POINTER(C.c_longlong)]),

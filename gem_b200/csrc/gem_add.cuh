@@ -157,6 +157,9 @@ __device__ __forceinline__ int next_chunk(const uint4 *chunk) { return (int)chun
 enum { SRC_XYZI = 0, SRC_SOA = 1, SRC_PCL32 = 2, SRC_KEYS = 3, SRC_RECORDS = 4 };
 // or-ed into SRC_XYZI / SRC_SOA / SRC_PCL32: the instantiation that runs every sensor model (transform_point<true>)
 constexpr int SRC_ANY_MODEL = 8;
+// or-ed into SRC_XYZI: the point count is min(n, *BinSource::n_dev), n the host's upper bound that sizes the grid (the
+// asynchronous pre-filtered add, whose count only the device knows)
+constexpr int SRC_DEVN = 16;
 
 struct RouteRec { // 20 bytes on the wire between tiles (gem_route.cuh)
     int gkey;     // global geographic linear index gx*L+gy
@@ -181,6 +184,7 @@ struct BinSource {
     int ncells;
     // SRC_RECORDS (tiled maps): records received from the other tiles (gkey < 0 = padding)
     const RouteRec *rec;
+    const int *n_dev; // SRC_DEVN
 };
 
 struct PointOut {
@@ -195,7 +199,7 @@ __device__ __forceinline__ PointOut bin_source_point(const MapGeom &g, const Fra
                                                      const SegTable *segs, const FrameParams *frames)
 {
     constexpr bool ANY = (SRC & SRC_ANY_MODEL) != 0;
-    constexpr int S = SRC & ~SRC_ANY_MODEL;
+    constexpr int S = SRC & ~(SRC_ANY_MODEL | SRC_DEVN);
     PointOut o;
     o.key = -1; o.geo = -1; o.h = -1.0f; o.hv = -1.0f; o.rgbf = 0u;
     if (S == SRC_XYZI) {
@@ -359,6 +363,7 @@ __global__ void __launch_bounds__(ADD_BLOCK)
 k_bin(MapGeom g, MapLayers ml, FrameParams f, BinSource in, int n, BinScratch sc, const __grid_constant__ RegionOps ro, int point_blocks,
       const __grid_constant__ SegTable segs, const FrameParams *frames)
 {
+    if constexpr ((SRC & SRC_DEVN) != 0) n = min(n, *in.n_dev);
     if ((int)blockIdx.x < point_blocks) {
         stamp_start(sc, 0);
         zero_next_counters(sc, blockIdx.x * blockDim.x + threadIdx.x);
@@ -1019,7 +1024,7 @@ __global__ void __launch_bounds__(ADD_BLOCK, 3)
 k_fold(MapGeom g, MapLayers ml, BinScratch sc, FoldSrc src, const __grid_constant__ RegionOps ro, int n, int fold_blocks, int slice, int do_fuse_i, int do_lowest_i,
        const int *n_dev)
 {
-    if (n_dev) n = min(n, *n_dev); // tiled maps: the number of marks is known on the device only (k_bin_peer)
+    if (n_dev) n = min(n, *n_dev); // tiled maps and pre-filtered adds: the number of marks is known on the device only
     extern __shared__ __align__(16) unsigned char s_dyn[]; // FOLD_SMEM_BYTES: the queue, the intensities (+ padding, see k_fold_long)
     int2 *s_first = reinterpret_cast<int2 *>(s_dyn);
     float *s_int = reinterpret_cast<float *>(s_first + FOLD_MARKS * ADD_BLOCK);

@@ -29,12 +29,18 @@
 // V8 Centroid: each of the four components starts at +0.0f, c += p in float point by point in V7 order, then one IEEE
 //    division c /= (float)count per component.  Intensity is averaged like x, y, z; a single point at -0.0 gives +0.0.
 // V9 Output: min(count, capacity) float4 into caller-owned device memory, count always reported.
+//
+// Every decision is taken on the device (DESIGN.md f20): a step reads its input count from device memory (the previous
+// step's count in a chain), runs its kernels and its sort at a host-known upper bound N of that count, and leaves its
+// count, V2 count and mode in its VoxStep.  Entries past the count take the cut points' key, so they join the run that
+// is dropped.  The sort runs on the fixed width GEM_VOX_KEY_BITS (gem_voxgrid.h proves that every key fits).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <string.h>
 
 #include "gem_kernels.cuh"
+#include "gem_voxgrid.h"
 
 namespace gem {
 
@@ -61,6 +67,15 @@ struct VoxAcc {
 struct VoxGrid {
     double minb[3];
     unsigned long long div0, div01, cut_key;
+};
+
+// one step on the device: its bounds pass, its grid, and what it decided (mode GEM_VOX_*; count: output points; drop: the
+// last run of the sorted keys holds cut points or entries past the count)
+struct VoxStep {
+    VoxAcc acc;
+    VoxGrid grid;
+    int mode, count, drop;
+    int n; // step 0: its input count (k_vox_init); a later step reads its predecessor's count
 };
 
 // Order-preserving encoding of a float (min / max are exact, so the reduction order is free; -0 and +0 only differ in
@@ -100,11 +115,23 @@ __device__ __forceinline__ bool vg_bounded(const VoxParams &P, const float4 &p)
     return vg_finite(p);
 }
 
+// Pass 0: the steps' accumulators start empty (one thread per step); step 0 takes its input count n0
+__global__ void k_vox_init(VoxStep *st, int nsteps, int n0)
+{
+    const int s = threadIdx.x;
+    if (s >= nsteps) return;
+    VoxStep z{};
+    z.n = s == 0 ? n0 : 0;
+    for (int a = 0; a < 3; a++) { z.acc.mn[a] = vg_key(3.402823466e38f); z.acc.mx[a] = vg_key(-3.402823466e38f); }
+    st[s] = z;
+}
+
 // Pass 1: V2 count, V3 count and bounds.  Grid-stride over 16-byte loads; per warp __reduce_*_sync, per block through
 // shared memory, then one atomic per quantity and block.
-__global__ void __launch_bounds__(VOX_BLOCK) k_vox_bounds(const float4 *__restrict__ in, int n, VoxParams P, VoxAcc *acc)
+__global__ void __launch_bounds__(VOX_BLOCK) k_vox_bounds(const float4 *__restrict__ in, int N, const int *nin, VoxParams P, VoxAcc *acc)
 {
     __shared__ unsigned sh[VOX_BLOCK / 32][8];
+    const int n = min(N, *nin);
     const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
     unsigned mn[3], mx[3], used = 0, bounded = 0;
     for (int a = 0; a < 3; a++) { mn[a] = vg_key(3.402823466e38f); mx[a] = vg_key(-3.402823466e38f); }
@@ -145,22 +172,53 @@ __global__ void __launch_bounds__(VOX_BLOCK) k_vox_bounds(const float4 *__restri
     }
 }
 
+// Between the passes, one thread: V5, V4 and V6 from the bounds (gem_voxgrid.h).  wide_passes: a GEM_VOX_WIDE grid
+// passes the input through (the asynchronous chain, which cannot refuse); otherwise it stays GEM_VOX_WIDE, writes nothing
+// and gem_voxel_grid refuses it.
+__global__ void k_vox_decide(VoxParams P, int N, const int *nin, VoxStep *st, int wide_passes)
+{
+    const int n = min(N, *nin);
+    VoxStep &S = *st;
+    S.drop = S.acc.used < N ? 1 : 0;
+    S.mode = GEM_VOX_EMPTY;
+    S.count = 0;
+    if (S.acc.bounded == 0) return; // V5
+    float mn[3], mx[3];
+    for (int a = 0; a < 3; a++) { mn[a] = vg_unkey(S.acc.mn[a]); mx[a] = vg_unkey(S.acc.mx[a]); }
+    VoxGrid G{};
+    const int mode = gem_vox_layout(mn, mx, P.inv, G.minb, &G.div0, &G.div01, &G.cut_key);
+    if (mode == GEM_VOX_PASS || (mode == GEM_VOX_WIDE && wide_passes && S.acc.used > 0)) { // V4: the input unchanged
+        S.mode = GEM_VOX_PASS;
+        S.count = n;
+    } else if (S.acc.used > 0) {
+        S.mode = mode;
+        S.grid = G; // count: k_vox_centroids
+    }
+}
+
 // Pass 2: one key per point, V6's mixed-radix index of (ijk2, ijk1, ijk0) for a V2 survivor, cut_key (one past the
 // largest voxel key) for a cut point, so that the cut points sort last as one run; the value is the input index.
 // floorf of the float product is exact, the difference with the floor value min_b is exact in double, and lies in
 // [0, div) because every survivor lies inside the V3 bounds.
-__global__ void __launch_bounds__(VOX_BLOCK) k_vox_keys(const float4 *__restrict__ in, int n, VoxParams P, VoxGrid G,
-                                                        unsigned long long *__restrict__ key, int *__restrict__ idx)
+// Entries past the step's count take cut_key as well; a step that is not GEM_VOX_GRID writes key 0 (its sort is not read).
+__global__ void __launch_bounds__(VOX_BLOCK) k_vox_keys(const float4 *__restrict__ in, int N, const int *nin, VoxParams P,
+                                                        const VoxStep *st, unsigned long long *__restrict__ key, int *__restrict__ idx)
 {
     const long long i = (long long)blockIdx.x * VOX_BLOCK + threadIdx.x;
-    if (i >= n) return;
-    const float4 p = in[i];
-    unsigned long long k = G.cut_key;
-    if (vg_used(P, p)) {
-        const unsigned long long i0 = (unsigned long long)(long long)((double)floorf(p.x * P.inv[0]) - G.minb[0]);
-        const unsigned long long i1 = (unsigned long long)(long long)((double)floorf(p.y * P.inv[1]) - G.minb[1]);
-        const unsigned long long i2 = (unsigned long long)(long long)((double)floorf(p.z * P.inv[2]) - G.minb[2]);
-        k = i0 + i1 * G.div0 + i2 * G.div01;
+    if (i >= N) return;
+    unsigned long long k = 0;
+    if (st->mode == GEM_VOX_GRID) {
+        const VoxGrid &G = st->grid;
+        k = G.cut_key;
+        if (i < *nin) {
+            const float4 p = in[i];
+            if (vg_used(P, p)) {
+                const unsigned long long i0 = (unsigned long long)(long long)((double)floorf(p.x * P.inv[0]) - G.minb[0]);
+                const unsigned long long i1 = (unsigned long long)(long long)((double)floorf(p.y * P.inv[1]) - G.minb[1]);
+                const unsigned long long i2 = (unsigned long long)(long long)((double)floorf(p.z * P.inv[2]) - G.minb[2]);
+                k = i0 + i1 * G.div0 + i2 * G.div01;
+            }
+        }
     }
     key[i] = k;
     idx[i] = (int)i;
@@ -196,19 +254,27 @@ __device__ __forceinline__ float4 vg_centroid(const VgSum &c, int count)
     return make_float4(vg_div1(c.s.x, c.nan.x, d), vg_div1(c.s.y, c.nan.y, d), vg_div1(c.s.z, c.nan.z, d), vg_div1(c.s.w, c.nan.w, d));
 }
 
-// Pass 3: V8, one thread per voxel (run of the sorted keys; sidx holds each run's input indices in ascending order).  A
+// Pass 3 of a GEM_VOX_PASS step: the input copied, min(count, capacity) points
+// Pass 3 of a GEM_VOX_GRID step: V8, one thread per voxel (run of the sorted keys; sidx holds each run's input indices in ascending order).  A
 // voxel of at most VOX_SHORT points is summed by its own lane.  The longer voxels of a warp are taken one after another
 // by the whole warp: the lanes gather 32 points at a time into shared memory (the next 32 are loaded while the current
 // ones are summed) and lane 0 adds them in order, so the sequential chain is V8's and nothing longer.  The centroid goes
 // straight to its voxel's output slot when that lies below the capacity.
 __global__ void __launch_bounds__(VOX_BLOCK) k_vox_centroids(const float4 *__restrict__ in, const int *__restrict__ sidx,
                                                              const int *__restrict__ cnt, const int *__restrict__ off,
-                                                             const VoxAcc *acc, int drop_last, float4 *__restrict__ out, int capacity)
+                                                             VoxStep *st, float4 *__restrict__ out, int capacity)
 {
     __shared__ float4 stage[VOX_BLOCK / 32][32];
     const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-    const int nvox = acc->nruns - drop_last;
     const long long v = (long long)blockIdx.x * VOX_BLOCK + threadIdx.x;
+    const int mode = st->mode;
+    if (mode == GEM_VOX_PASS) {
+        if (v < st->count && v < capacity) out[v] = in[v];
+        return;
+    }
+    if (mode != GEM_VOX_GRID) return;
+    const int nvox = st->acc.nruns - st->drop;
+    if (v == 0) st->count = nvox;
     if ((long long)blockIdx.x * VOX_BLOCK >= nvox) return; // whole warps leave together below
     const int c = v < nvox ? cnt[v] : 0;
     const int o = v < nvox ? off[v] : 0;

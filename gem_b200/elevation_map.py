@@ -848,6 +848,57 @@ class ElevationMap:
                                        C.byref(info)), self._h, "gem_voxel_grid")
         return out[:min(info.count, cap)], {k: getattr(info, k) for k, _ in _lib.GemVoxelGridInfo._fields_}
 
+    @staticmethod
+    def prefilter(steps) -> _lib.GemPrefilter:
+        """gem_prefilter from VoxelGrid steps as voxel_oracle.FILTER_LAUNCH writes them, (leaf, field, (lo, hi), negative)
+        in launch order; leaf is a number or three, field None, "x", "y", "z" or "intensity".  None or [] is no filter"""
+        steps = list(steps or [])
+        if len(steps) > _lib.PREFILTER_MAX_STEPS:
+            raise ValueError(f"prefilter: at most {_lib.PREFILTER_MAX_STEPS} steps")
+        pf = _lib.GemPrefilter()
+        pf.nsteps = len(steps)
+        for j, (leaf_size, field, limits, negative) in enumerate(steps):
+            leaf = [float(leaf_size)] * 3 if np.ndim(leaf_size) == 0 else [float(v) for v in leaf_size]
+            if len(leaf) != 3:
+                raise ValueError("prefilter: leaf is one number or three")
+            if field not in _lib.VOXEL_FIELDS:
+                raise ValueError(f"prefilter: field must be one of {list(_lib.VOXEL_FIELDS)}")
+            lo, hi = (float(v) for v in limits)
+            pf.step[j] = _lib.GemVoxelGridParams((C.c_float * 3)(*leaf), _lib.VOXEL_FIELDS[field], lo, hi, 1 if negative else 0)
+        return pf
+
+    def add_points_filtered_stream(self, xyzi, prefilter, frame: GemFrame, bgr=None, T_camera=None, T_lidar=None):
+        """gem_add_points_filtered_stream (DESIGN.md f20): the VoxelGrid steps `prefilter` (see prefilter()) over `xyzi`, a
+        contiguous (n, 4) float32 CUDA tensor, the colour lookup from `bgr` (an (H, W, 3) uint8 CUDA tensor with the
+        calibration T_camera / T_lidar, or None) and the pipelined add, with no host synchronisation.  xyzi must stay
+        untouched until two further add calls have completed"""
+        import torch
+        if not (_is_device(xyzi) and xyzi.dtype == torch.float32 and xyzi.dim() == 2 and xyzi.shape[1] == 4
+                and xyzi.is_contiguous()):
+            raise ValueError("add_points_filtered_stream: xyzi must be a contiguous (n, 4) float32 CUDA tensor")
+        pf = prefilter if isinstance(prefilter, _lib.GemPrefilter) else self.prefilter(prefilter)
+        n = int(xyzi.shape[0])
+        proj = None
+        if bgr is not None:
+            if not (_is_device(bgr) and bgr.dtype == torch.uint8 and bgr.dim() == 3 and bgr.shape[2] == 3 and bgr.is_contiguous()):
+                raise ValueError("add_points_filtered_stream: bgr must be a contiguous (H, W, 3) uint8 CUDA tensor")
+            proj = _lib.GemProjection()
+            proj.T_camera[:] = [float(v) for v in np.asarray(T_camera, np.float64).reshape(-1)]
+            proj.T_lidar[:] = [float(v) for v in np.asarray(T_lidar, np.float64).reshape(-1)]
+            proj.height, proj.width = int(bgr.shape[0]), int(bgr.shape[1])
+            proj.row_stride = 3 * proj.width
+        torch.cuda.current_stream(xyzi.device).synchronize()   # the library reads on its own stream
+        check(self._lib.gem_add_points_filtered_stream(self._h, _ptr(xyzi) if n else None, n, C.byref(pf),
+                                                       _ptr(bgr) if bgr is not None else None,
+                                                       C.byref(proj) if proj is not None else None, C.byref(frame)),
+              self._h, "gem_add_points_filtered_stream")
+
+    def prefilter_info(self, nsteps: int = _lib.PREFILTER_MAX_STEPS) -> list:
+        """gem_prefilter_info: [{count, used, passthrough}] of the newest pre-filtered add's steps (synchronises)"""
+        out = (_lib.GemVoxelGridInfo * max(int(nsteps), 1))()
+        check(self._lib.gem_prefilter_info(self._h, out, int(nsteps)), self._h, "gem_prefilter_info")
+        return [{k: getattr(out[j], k) for k, _ in _lib.GemVoxelGridInfo._fields_} for j in range(int(nsteps))]
+
     # -- raw sensor messages: PointCloud2 and cv_bridge's 8-bit images (DESIGN.md f12) -------------------------------------
     @staticmethod
     def pointcloud2_mapping(layout: PointCloud2Layout, data_bytes: int | None = None) -> dict:
@@ -916,15 +967,23 @@ class ElevationMap:
         return out
 
     def add_pointcloud2_host_async(self, layout: PointCloud2Layout, data, frame: GemFrame, image: CameraImage | None = None,
-                                   data_bytes: int | None = None):
+                                   data_bytes: int | None = None, prefilter=None):
         """gem_add_pointcloud2_host_async: one sensor_msgs/PointCloud2 (host bytes: numpy, bytes or a CPU tensor, pinned
         or pageable) and optionally its camera image, decoded, colourised and added pipelined.  Pinned buffers must stay
-        untouched until the call after next or sync(); pageable ones may be reused at once."""
+        untouched until the call after next or sync(); pageable ones may be reused at once.  prefilter (VoxelGrid steps,
+        see prefilter(), or a GemPrefilter): gem_add_pointcloud2_filtered_host_async, the steps between the decode and
+        the colour (DESIGN.md f20)"""
         ptr, nb = _host_bytes(data) if layout.points else (None, 0)
         nb = nb if data_bytes is None else int(data_bytes)
-        check(self._lib.gem_add_pointcloud2_host_async(self._h, C.byref(layout.c), ptr, nb,
-                                                       C.byref(image.c) if image is not None else None, C.byref(frame)),
-              self._h, "gem_add_pointcloud2_host_async")
+        img = C.byref(image.c) if image is not None else None
+        if prefilter is None:
+            check(self._lib.gem_add_pointcloud2_host_async(self._h, C.byref(layout.c), ptr, nb, img, C.byref(frame)),
+                  self._h, "gem_add_pointcloud2_host_async")
+            return
+        pf = prefilter if isinstance(prefilter, _lib.GemPrefilter) else self.prefilter(prefilter)
+        check(self._lib.gem_add_pointcloud2_filtered_host_async(self._h, C.byref(layout.c), ptr, nb, img, C.byref(pf),
+                                                                C.byref(frame)),
+              self._h, "gem_add_pointcloud2_filtered_host_async")
 
     # -- the MLS densification of the dense_mapping signal (DESIGN.md f10) ------------------------------------------------
     GEM_MLS = {"search_radius": 0.5, "sqr_gauss_param": 0.25, "polynomial_fit": True, "order": 5,

@@ -476,7 +476,8 @@ int gem_costmap_inflate(gem_map *m, const gem_costmap_window *w, const gem_costm
  *      per component.  Intensity is averaged like x, y, z (a lone -0.0 comes out +0.0); no other field is carried.
  *   V9 min(count, capacity) float4 go to out_xyzi_device; *info always receives count (output points), used (V2 survivors)
  *      and passthrough.  capacity = 0 is a size query.
- *   Host-synchronous; works on any handle, tiled ones included; neither reads nor modifies the map and does not issue the
+ *   Host-synchronous (one synchronisation: the steps of gem_add_pointcloud2_filtered_host_async enqueued, then the info
+ *   read back); works on any handle, tiled ones included; neither reads nor modifies the map and does not issue the
  *   deferred fold.  A bad leaf, n < 0, NULL points with n > 0, capacity < 0, NULL out with capacity > 0, a bad field id
  *   and overlapping input and output ranges are GEM_ERR_INVALID (chain calls, as the KITTI launch does, through two
  *   buffers).  Uses a handle-owned scratch of about 32 bytes per input point, grown on demand: a failed growth is
@@ -636,6 +637,49 @@ int gem_image_to_bgr8(gem_map *m, const char *encoding, const void *src_device, 
                       void *dst_device, int dst_step);
 int gem_add_pointcloud2_host_async(gem_map *m, const gem_pointcloud2 *layout, const void *data_host, unsigned long long data_bytes,
                                    const gem_camera_image *img, const gem_frame *frame);
+
+/* ---- the demos' VoxelGrid pre-filter inside the asynchronous add (DESIGN.md f20) ----
+ * gem_prefilter: the VoxelGrid nodelets in front of the node, in launch order (filter.launch: one step; filter_kitti.launch:
+ *   three); nsteps == 0 is no filter.  Each step is gem_voxel_grid with these parameters.
+ * gem_add_pointcloud2_filtered_host_async: gem_add_pointcloud2_host_async with the pre-filter between the decode and the
+ *   colour lookup.  All on the handle's stream, with no host synchronisation and no read-back of any count: H2D copy
+ *   (copy stream), decode into a handle buffer, the steps alternating between two handle buffers, the last one into the
+ *   ring's staging set, the colour lookup by the handle's mode, the pipelined add.  The map, gem_stats and the steps'
+ *   infos equal those of decode -> gem_voxel_grid per step -> gem_colourise_points -> gem_add_points_stream, bit for bit.
+ *   Kernels and sorts run at the raw width * height; the filtered count stays on the device, and gem_stats.points_in
+ *   reports it (fetched with the other counters).  A raw cloud of 0 points flushes, as gem_add_pointcloud2_host_async;
+ *   a filtered count of 0 is an add of nothing.  Same ring, host-buffer rules and growth as
+ *   gem_add_pointcloud2_host_async (the two, and gem_add_points_host_async, may be interleaved); the step scratch (about
+ *   64 bytes per raw point) grows in the same way.  DEFINED: the composition is decode -> filter -> colour.  The reference
+ *   filters the message and decodes the result; the two are equal wherever x, y, z and intensity are FLOAT32 (the only
+ *   layouts where the node maps them: the decode keeps those four fields, and the colour comes after the filter in both).
+ *   Elsewhere the result is what decode-first gives.
+ *   DEFINED: a step whose voxel grid gem_voxel_grid refuses (bounds whose products with 1 / leaf are not finite, a span of
+ *   few voxels near FLT_MAX) passes its input through, with passthrough = 1.
+ * gem_add_points_filtered_stream: the same from n float4 {x, y, z, intensity} in device memory; bgr_device (BGR8,
+ *   projection's size and row stride) may be NULL for no colour, and projection is read only when it is not.  The input
+ *   is read until two further add calls have completed (gem_add_points_stream's rule); it is never written.
+ * Both return GEM_ERR_INVALID with nothing enqueued for: a step gem_voxel_grid refuses (bad leaf or field id), nsteps
+ *   outside 0..GEM_PREFILTER_MAX_STEPS, n (raw width * height) > max_points, a sensor with cloud_width != 0 (the nodelet
+ *   publishes an unorganised cloud, so the pixel index of the stereo model is the index in the filtered cloud), and
+ *   whatever gem_add_pointcloud2_host_async / gem_add_points_stream refuse.
+ * gem_prefilter_info: host-synchronous; out[s] = count, used and passthrough of step s of the newest filtered call (steps
+ *   that call did not run, and every step before the first filtered call, read 0); nsteps in 0..GEM_PREFILTER_MAX_STEPS. */
+enum { GEM_PREFILTER_MAX_STEPS = 4 };
+typedef struct gem_prefilter {
+    int nsteps;
+    gem_voxel_grid_params step[GEM_PREFILTER_MAX_STEPS];
+} gem_prefilter;
+typedef struct gem_projection {
+    double T_camera[12], T_lidar[16]; /* as gem_colourise_points                              */
+    int width, height, row_stride;    /* the BGR8 image; row_stride in bytes >= 3 * width     */
+} gem_projection;
+int gem_add_pointcloud2_filtered_host_async(gem_map *m, const gem_pointcloud2 *layout, const void *data_host,
+                                            unsigned long long data_bytes, const gem_camera_image *img,
+                                            const gem_prefilter *prefilter, const gem_frame *frame);
+int gem_add_points_filtered_stream(gem_map *m, const void *xyzi_device, int n, const gem_prefilter *prefilter,
+                                   const void *bgr_device, const gem_projection *projection, const gem_frame *frame);
+int gem_prefilter_info(gem_map *m, gem_voxel_grid_info *out, int nsteps);
 
 /* ---- saving point clouds as PCD files (savingMap / savingSubMap / pointcloudinterpolation's pcl::io::savePCDFile,
  * ElevationMapping.cpp:430-476, :1117; DESIGN.md f13) ----

@@ -446,6 +446,48 @@ class ElevationMap {
     {
         check(gem_add_pointcloud2_host_async(h_, lay.layout(), data_host, data_bytes, img, &frame), "gem_add_pointcloud2_host_async");
     }
+    // the demos' VoxelGrid nodelets inside the asynchronous add (DESIGN.md f20): the steps in launch order, then the
+    // colour lookup and the pipelined add, with no host synchronisation.  Prefilter::filterLaunch() / filterKittiLaunch()
+    // are GEM's two launches.  addPointsFilteredStream reads xyzi_device until two further add calls have completed;
+    // bgr_device may be null (no colour).  prefilterInfo synchronises and returns the newest filtered call's steps.
+    struct Prefilter {
+        gem_prefilter c{};
+        Prefilter &add(float leaf, int field, double lo, double hi, bool negative = false)
+        {
+            if (c.nsteps >= GEM_PREFILTER_MAX_STEPS) throw std::runtime_error("Prefilter: at most GEM_PREFILTER_MAX_STEPS steps");
+            gem_voxel_grid_params &p = c.step[c.nsteps++];
+            p.leaf_size[0] = p.leaf_size[1] = p.leaf_size[2] = leaf;
+            p.field = field;
+            p.limit_min = lo;
+            p.limit_max = hi;
+            p.limit_negative = negative ? 1 : 0;
+            return *this;
+        }
+        static Prefilter filterLaunch() { return Prefilter().add(0.1f, GEM_VOXEL_FIELD_X, -10.0, 10.0); }
+        static Prefilter filterKittiLaunch()
+        {
+            return Prefilter().add(0.2f, GEM_VOXEL_FIELD_X, -40.0, 40.0).add(0.2f, GEM_VOXEL_FIELD_Z, -25.0, 25.0).add(0.2f, GEM_VOXEL_FIELD_Y, -40.0, 40.0);
+        }
+    };
+    void addPointCloud2HostAsync(const PointCloud2Layout &lay, const void *data_host, unsigned long long data_bytes,
+                                 const gem_camera_image *img, const Prefilter &pf, const gem_frame &frame)
+    {
+        check(gem_add_pointcloud2_filtered_host_async(h_, lay.layout(), data_host, data_bytes, img, &pf.c, &frame),
+              "gem_add_pointcloud2_filtered_host_async");
+    }
+    void addPointsFilteredStream(const void *xyzi_device, size_t n, const Prefilter &pf, const void *bgr_device,
+                                 const gem_projection *projection, const gem_frame &frame)
+    {
+        if (n > (size_t)std::numeric_limits<int>::max()) throw std::runtime_error("addPointsFilteredStream: more than INT_MAX points");
+        check(gem_add_points_filtered_stream(h_, xyzi_device, (int)n, &pf.c, bgr_device, projection, &frame),
+              "gem_add_points_filtered_stream");
+    }
+    std::vector<gem_voxel_grid_info> prefilterInfo(int nsteps)
+    {
+        std::vector<gem_voxel_grid_info> out((size_t)std::max(nsteps, 0));
+        check(gem_prefilter_info(h_, out.data(), nsteps), "gem_prefilter_info");
+        return out;
+    }
     // pointcloudinterpolation's MovingLeastSquares (GEM's dense_mapping signal, ElevationMapping.cpp:1072-1118; DESIGN.md
     // f10) over n PointXYZRGBICT records in device memory: min(count, capacity) new records go to out_device, which must
     // not overlap the input (capacity 0 is a size query).  gemMlsParams() is GEM's setting.
